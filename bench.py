@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — throughput of the batched hot paths on N B200s (one process per GPU).
+"""bench.py — throughput of the batched hot paths on N H100s (one process per GPU).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload ekf|pf|mpc]
+                  [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
          --master-port P bench.py --gpus N --steps K --warmup W
 
@@ -19,10 +20,14 @@ index-addressed generators; the only inter-GPU traffic is one all-gather of 8 do
 libcrb's own NCCL communicator (crb_gather_stats) INSIDE the captured graph.
 
 Timing rules followed: W >= 3 warm-up steps; inputs rotate over 3 buffer sets whose total exceeds the
-126 MB L2; the K steps (+ stats tail + all-gather) are captured once and replayed >= 10 times, every replay
-timed with CUDA events on the launching stream, the whole series bracketed by barrier + synchronize, each replay's
-time maxed over ranks; `ms_per_step` is the MEDIAN replay / K and the minimum is reported beside it; SM clocks
+50 MB L2; the K steps (+ stats tail + all-gather) are captured once into a CUDA graph, replayed once untimed and
+then once timed with CUDA events on the launching stream, so exactly K steps are timed; the timed replay is
+bracketed by barrier + synchronize and its time maxed over ranks; `ms_per_step` is that time / K; SM clocks
 sampled with nvidia-smi during the timed region.
+
+--dump-outputs DIR writes what the headline's last timed step computed (the EKF state x and covariance P of a
+fixed, seeded sample of 2^19 agents, float32, and their agent indices, float64) as DIR/<name>.npy.  Inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 
 `--impl reference` times the CPU restatement of the reference (oracle/, the only implementation of the
 path that can run here: Eigen/IPOPT are absent) on the box's host cores with all threads.
@@ -78,11 +83,11 @@ def peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)", d
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)", {}
+    return 3350.0, "nominal (H100 SXM data sheet: 3.35 TB/s HBM3)", {}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -285,18 +290,15 @@ def pinned(a):
 # =========================================================================================================
 # workloads: each returns a dict with value / ms_per_step / roofline / e2e / cpu_baseline pieces
 # =========================================================================================================
-REPLAYS = 10
 LAST_TIMING = {}
 
 
-def time_device_steps(step_fn, steps, warmup, world, after_fn=None, eng=None, graph=True, reps=None):
+def time_device_steps(step_fn, steps, warmup, world, after_fn=None, eng=None, graph=True):
     """W untimed steps, then the K steps (+ the optional tail: stats reduction and the all-gather) captured ONCE
-    into a CUDA graph and replayed `reps` (>= 10) times.  Every replay is timed with its own pair of CUDA events
-    on the launching stream; the series is bracketed by barrier + synchronize on both sides and each replay's time
-    is maxed over ranks.  Returns (median replay ms, mode); LAST_TIMING holds min / median / all replays.  If
-    capture is not possible the K steps are enqueued directly, also `reps` times."""
+    into a CUDA graph, replayed once untimed and once timed: exactly K steps are timed, with a pair of CUDA events
+    on the launching stream, bracketed by barrier + synchronize on both sides and maxed over ranks.  Returns
+    (ms of the K steps, mode).  If capture is not possible the K steps are enqueued directly."""
     import torch
-    reps = REPLAYS if reps is None else reps
     for k in range(warmup):
         step_fn(k)
     if after_fn is not None:
@@ -321,36 +323,26 @@ def time_device_steps(step_fn, steps, warmup, world, after_fn=None, eng=None, gr
             eng.bind_current_stream()
             g = None
     barrier_sync(world)
-    evs = []
-    for r in range(reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        if g is not None:
-            g.replay()
-        else:
-            for k in range(steps):
-                step_fn(warmup + k)
-            if after_fn is not None:
-                after_fn()
-        e1.record()
-        evs.append((e0, e1))
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    if g is not None:
+        g.replay()
+    else:
+        for k in range(steps):
+            step_fn(warmup + k)
+        if after_fn is not None:
+            after_fn()
+    e1.record()
     barrier_sync(world)
-    ms = torch.tensor([a.elapsed_time(b) for a, b in evs], dtype=torch.float64, device="cuda")
-    if world > 1:
-        import torch.distributed as dist
-        dist.all_reduce(ms, op=dist.ReduceOp.MAX)
-    v = ms.cpu().numpy()
+    ms = max_over_ranks(e0.elapsed_time(e1), world)
     LAST_TIMING.clear()
-    LAST_TIMING.update(replays=int(reps), steps_per_replay=int(steps), ms_median=float(np.median(v)),
-                       ms_min=float(v.min()), ms_max=float(v.max()), mode=mode)
-    return float(np.median(v)), mode
+    LAST_TIMING.update(timed_steps=int(steps), ms=ms, mode=mode)
+    return ms, mode
 
 
 def timing_record(steps):
     t = dict(LAST_TIMING)
-    return dict(replays=t.get("replays"), steps_per_replay=t.get("steps_per_replay"),
-                ms_per_step_median=t.get("ms_median", 0.0) / steps, ms_per_step_min=t.get("ms_min", 0.0) / steps,
-                ms_per_step_max=t.get("ms_max", 0.0) / steps, launch=t.get("mode"))
+    return dict(timed_steps=t.get("timed_steps"), ms_per_step=t.get("ms", 0.0) / steps, launch=t.get("mode"))
 
 
 def time_host_steps(step_fn, steps, warmup, world):
@@ -476,7 +468,10 @@ def as_shipped_O0(fn, units, budget_s=1.0):
     return v
 
 
-def bench_ekf(eng, rank, world, steps, warmup, with_cpu):
+DUMP_AGENTS = 1 << 19
+
+
+def bench_ekf(eng, rank, world, steps, warmup, with_cpu, dump=None):
     import torch
     from cpprobotics_b200 import synth
     n = EKF_N
@@ -498,6 +493,13 @@ def bench_ekf(eng, rank, world, steps, warmup, with_cpu):
 
     ms, mode = time_device_steps(step, steps, warmup, world, after, eng=eng)
     timing = timing_record(steps)
+    if dump is not None:
+        # the last timed step updated buffer set (warmup + steps - 1) % NSETS in place; later timings reuse the sets
+        x, P = sets[(warmup + steps - 1) % NSETS][:2]
+        idx = np.sort(np.random.default_rng(20240611).choice(n, size=min(DUMP_AGENTS, n), replace=False))
+        sel = torch.from_numpy(idx).to(dev)
+        dump.update(ekf_x=x.index_select(1, sel).cpu().numpy(), ekf_P=P.index_select(1, sel).cpu().numpy(),
+                    ekf_agent_index=(rank * n + idx).astype(np.float64))
     launches = steps + 2 + (1 if world > 1 else 0)   # K filter kernels + two stats-reduction kernels (+ NCCL's)
     value = world * n * steps / (ms * 1e-3)
     # roofline of the dominant kernel (one launch per step): algorithmic bytes / avg launch duration,
@@ -538,8 +540,7 @@ def bench_ekf(eng, rank, world, steps, warmup, with_cpu):
                              frac=achieved / peak, traffic=traffic_for("ekf"), peak_source=peak_src,
                              kernel="crb_ekf_step_kernel",
                              algorithmic_bytes_per_launch=EKF_BYTES * n,
-                             ms_per_launch_median=k_timing["ms_per_step_median"],
-                             ms_per_launch_min=k_timing["ms_per_step_min"],
+                             ms_per_launch=k_timing["ms_per_step"],
                              copy_gbs_same_run=copy_gbs, frac_of_copy_same_run=achieved / copy_gbs),
                e2e=dict(value=world * n * e_steps / (ms_e * 1e-3), unit="updates/s",
                         h2d_bytes_per_step=96 * n, d2h_bytes_per_step=80 * n,
@@ -609,7 +610,7 @@ def bench_pf(eng, rank, world, steps, warmup, with_cpu):
     out = dict(metric="PF particle updates/sec (predict+weight, 8 landmarks)", value=value,
                unit="particles/s", ms_per_step=ms_k / steps, timing=timing_record(steps),
                config=dict(workload="pf_predict_weight_2^20_particles_8_landmarks_per_gpu",
-                           l2=f"{len(sets)} rotating buffer sets, {len(sets) * 29} MB > 126 MB L2"),
+                           l2=f"{len(sets)} rotating buffer sets, {len(sets) * 29} MB > 50 MB L2"),
                roofline=dict(bound="hbm", achieved=achieved, peak=peak, unit="GB/s",
                              frac=achieved / peak, traffic=traffic_for("pf"), peak_source=peak_src,
                              kernel="crb_pf_predict_weight_lean_kernel",
@@ -674,7 +675,7 @@ def cpu_pf(host=None, lm=None):
 
 
 def mpc_flops(iters_sum, n, T):
-    """Executed-work flop model (DESIGN.md §MPC): per outer iteration one backward sweep (~470 flop /
+    """Executed-work flop model (DESIGN.md §3, MPC): per outer iteration one backward sweep (~470 flop /
     stage, structured) and ~1.2 forward sweeps (~150 flop / stage incl. polynomial sin/cos)."""
     return iters_sum * (T - 1) * (470.0 + 1.2 * 150.0)
 
@@ -685,12 +686,14 @@ FP32_PEAK = {}
 def fp32_peak(eng):
     """Non-tensor fp32 FMA rate MEASURED in this run on this GPU (crb_probe_fp32_peak); nominal as fallback."""
     if "v" not in FP32_PEAK:
-        sm_max = float(peaks()[2].get("sm_max_mhz", 1965.0))
-        nominal = 148 * 128 * 2 * sm_max * 1e6 / 1e12
+        import torch
+        sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+        sm_max = float(peaks()[2].get("sm_max_mhz", 1980.0))
+        nominal = sms * 128 * 2 * sm_max * 1e6 / 1e12
         try:
             v = eng.probe_fp32_peak()
             FP32_PEAK.update(v=v, src=f"measured in this run: crb_probe_fp32_peak (register-only FFMA kernel, best of 5); "
-                                      f"nominal 148 SM x 128 lanes x 2 x {sm_max:.0f} MHz = {nominal:.1f}")
+                                      f"nominal {sms} SM x 128 lanes x 2 x {sm_max:.0f} MHz = {nominal:.1f}")
         except Exception as exc:   # pragma: no cover
             FP32_PEAK.update(v=nominal, src=f"nominal (probe failed: {exc})")
     return FP32_PEAK["v"], FP32_PEAK["src"]
@@ -758,8 +761,7 @@ def bench_mpc(eng, rank, world, steps, warmup, with_cpu, n=None, label=None, wit
                              frac=tfl / fpk, traffic=traffic, peak_source=fpk_src,
                              kernel=kernel, flop_model="executed iterations x (T-1) x (470 + 1.2 x 150) flop, DESIGN.md",
                              solves_per_s_kernel_only=world * n * steps / (ms_k * 1e-3),
-                             ms_per_launch_median=k_timing["ms_per_step_median"],
-                             ms_per_launch_min=k_timing["ms_per_step_min"],
+                             ms_per_launch=k_timing["ms_per_step"],
                              algorithmic_bytes_per_launch=MPC_BYTES * n,
                              traffic_over_algorithmic=(traffic / (MPC_BYTES * n)) if traffic else None,
                              io_gbs=achieved_io, io_frac_of_hbm=achieved_io / peak))
@@ -781,10 +783,8 @@ def bench_mpc(eng, rank, world, steps, warmup, with_cpu, n=None, label=None, wit
                 eng.stats_reduce(cost, status, iters2, i0=rank * n, out=stats)
                 gather_stats(stats, world, eng, out=table)
             ms_h, _ = time_device_steps(step_hinted, steps, 1, world, eng=eng)
-            t_h = timing_record(steps)
             same = bool(torch.equal(iters2, want_iters)) and bool(torch.equal(cost, want_cost))
             hinted[name] = dict(value=world * n * steps / (ms_h * 1e-3), unit="solves/s", ms_per_step=ms_h / steps,
-                                ms_per_step_median=t_h["ms_per_step_median"], ms_per_step_min=t_h["ms_per_step_min"],
                                 speedup_vs_index_order=ms / ms_h, same_bits_as_index_order=same)
         hinted["what"] = ("crb_mpc_solve_batched_hinted: iteration counts of the agents' previous solve as scheduling "
                           "hints (receding-horizon MPC), stats + gather included like the headline step; "
@@ -944,7 +944,7 @@ def bench_ekf_large(eng, rank, world, steps, warmup):
     gbs = EKF_BYTES * n * steps / (ms * 1e-3) / 1e9
     return dict(metric="EKF updates/sec, 2^24 agents x 1 step", value=world * n * steps / (ms * 1e-3),
                 unit="updates/s", ms_per_step=ms / steps,
-                config=dict(workload="ekf_2^24_agents_1_step_per_gpu", l2="3.1 GB per launch >> 126 MB L2"),
+                config=dict(workload="ekf_2^24_agents_1_step_per_gpu", l2="3.1 GB per launch >> 50 MB L2"),
                 roofline=dict(bound="hbm", achieved=gbs, peak=peaks()[0], unit="GB/s", frac=gbs / peaks()[0],
                               traffic=None, kernel="crb_ekf_step_kernel",
                               algorithmic_bytes_per_launch=EKF_BYTES * n))
@@ -1041,8 +1041,9 @@ def run_ours(args):
     restore = (lambda: None)
     if cpu:
         restore, pin_note = cpu_pin_one_numa_node()
+    dump = {} if args.dump_outputs else None
     with ClockSampler(local) as clk:
-        head = bench_ekf(eng, rank, world, args.steps, args.warmup, with_cpu=cpu)
+        head = bench_ekf(eng, rank, world, args.steps, args.warmup, with_cpu=cpu, dump=dump)
         if args.workload in ("all", "pf"):
             res["pf"] = bench_pf(eng, rank, world, args.steps, args.warmup, with_cpu=cpu)
         if args.workload in ("all", "pf"):
@@ -1071,7 +1072,7 @@ def run_ours(args):
     restore()
     cfg = {"workload": "ekf_2^20_agents_1_step_per_gpu (BASELINE.json configs[1])",
            "agents_per_gpu": EKF_N, "global_agents": EKF_N * world,
-           "l2": "3 rotating buffer sets, 303 MB of inputs > 126 MB L2",
+           "l2": "3 rotating buffer sets, 303 MB of inputs > 50 MB L2",
            "collective": "one all-gather of 8 doubles per rank (libcrb crb_gather_stats, NCCL) inside the captured "
                          "graph, once per replay of K steps",
            "launch": head["launch_mode"], "timing": head["timing"]}
@@ -1120,6 +1121,10 @@ def run_ours(args):
     if res:
         line["extra"] = res
     if rank == 0:
+        if dump is not None:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, a in dump.items():
+                np.save(os.path.join(args.dump_outputs, name + ".npy"), a)
         print(json.dumps(line), flush=True)
     eng.close()
     if world > 1:
@@ -1183,6 +1188,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="all", choices=["all", "ekf", "ekf100", "ekf16m", "pf", "mpc", "lqr"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline's last-step outputs (seeded sample) as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":

@@ -1,8 +1,8 @@
-"""cpprobotics_b200 — B200-native batched small-matrix engine for the CppRobotics hot paths.
+"""cpprobotics_b200 — H100-native batched small-matrix engine for the CppRobotics hot paths.
 
-The product is libcrb.so (hand-written sm_100a CUDA behind the C ABI of include/crb.h); this package
+The product is libcrb.so (hand-written sm_90a CUDA behind the C ABI of include/crb.h); this package
 is the thin Python host layer the tests and the bench use to reach it.  There is no CPU path here:
-importing works anywhere (so the build can be checked without a GPU), computing needs a B200.
+importing works anywhere (so the build can be checked without a GPU), computing needs an H100.
 """
 from ._lib import CrbError, EkfParams, MpcParams, PfParams, load_library  # noqa: F401
 from .engine import (Engine, ekf_default_params, mpc_default_params,  # noqa: F401

@@ -133,7 +133,7 @@ def load_library() -> C.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise CrbError(
-            f"{LIB_PATH} not found: build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+            f"{LIB_PATH} not found: build it with `python __graft_entry__.py` (nvcc, sm_90a). "
             "cpprobotics_b200 has no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in PROTOTYPES.items():

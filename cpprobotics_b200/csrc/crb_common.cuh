@@ -88,10 +88,8 @@ int crb_ctx_mpc_ws_reserve(crb_ctx* ctx, size_t bytes);
 extern "C" int crb_comm_destroy(crb_ctx* ctx);
 extern "C" int crb_comm_allreduce_sum_f64(crb_ctx* ctx, double* buf_dev, int64_t count);
 
-// Strided host<->device block copy for the *_host pipelines.  Measured on this platform
-// (scripts/pcie_probe.py + bench e2e): plain 1-D copies reach 48 (H2D) / 57 (D2H) GB/s, one
-// cudaMemcpy2DAsync per array ~31 GB/s per direction in duplex, and splitting it into per-row 1-D copies is
-// SLOWER (enqueue-bound: 2.0-2.8e8 vs 3.45e8 EKF updates/s end to end), so the 2-D copy stays.
+// Strided host<->device block copy for the *_host pipelines: one cudaMemcpy2DAsync per array.  Splitting it
+// into per-row 1-D copies makes the pipeline enqueue-bound (scripts/pcie_probe.py compares the two).
 static inline cudaError_t crb_copy_rows(void* dst, size_t dpitch, const void* src, size_t spitch,
                                         size_t width, size_t rows, cudaMemcpyKind kind, cudaStream_t st) {
   return cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, rows, kind, st);
@@ -101,9 +99,8 @@ static inline cudaError_t crb_copy_rows(void* dst, size_t dpitch, const void* sr
 // mapped into this device's address space (cudaHostAlloc / cudaMallocHost / crb_host_alloc, or
 // cudaHostRegister'ed memory) can be dereferenced by a kernel directly, so the resident kernel is launched
 // on it and its coalesced 128-byte loads/stores ride PCIe in both directions at once with no staging
-// copy.  Measured on B200 + PCIe Gen5 (scripts/zerocopy_probe.py): EKF 2^20 agents 370 M updates/s vs 326
-// staged (65 GB/s duplex total = what the platform gives any mix of directions), PF 1337 M vs 941 M
-// particles/s.  Pageable pointers return false and take the staged pipeline.  CRB_HOST_ZEROCOPY=0
+// copy (scripts/zerocopy_probe.py compares it with the staged pipeline).  Pageable pointers return false and
+// take the staged pipeline.  CRB_HOST_ZEROCOPY=0
 // forces the staged pipeline (A/B, tests).  NULL counts as mappable (optional arrays).
 static inline bool crb_zero_copy_enabled() {
   static int on = -1;
@@ -127,9 +124,9 @@ static inline bool crb_host_mapped(T* host, T** dev) {
   return true;
 }
 
-// Programmatic dependent launch (PDL): back-to-back launches of the short streaming kernels (EKF step 30 us,
-// PF step 11 us) otherwise pay ~1.5 us each for the drain of kernel N plus the launch and prologue of
-// kernel N+1.  With the launch attribute below, kernel N+1's CTAs are scheduled as soon as every CTA of
+// Programmatic dependent launch (PDL): back-to-back launches of the short streaming kernels (EKF step, PF
+// step: tens of microseconds) otherwise pay the drain of kernel N plus the launch and prologue of kernel N+1
+// on every launch.  With the launch attribute below, kernel N+1's CTAs are scheduled as soon as every CTA of
 // kernel N has executed crb_pdl_launch_dependents() (or exited); they run their address arithmetic and
 // then block in crb_pdl_wait() until kernel N has completed and its writes are visible, so a truly
 // dependent sequence (EKF step k+1 reading step k's state) stays correct.  Both instructions are no-ops in
@@ -177,7 +174,7 @@ __device__ __forceinline__ void st_stream(float* p, float v) { __stcs(p, v); }
 // a degree-7/8 polynomial, one final rounding to float (sysdeps/ieee754/flt-32/s_sinf.c, s_cosf.c,
 // sincosf.h, s_sincosf_data.c).  On x86-64 hosts with FMA (every server CPU of the last decade) glibc's ifunc
 // picks the build of those files compiled with -mfma, in which each a + b * c of the source is ONE fused
-// operation: that is what is restated here with explicit fma(), operation for operation, and the B200's FP64
+// operation: that is what is restated here with explicit fma(), operation for operation, and the GPU's FP64
 // pipe (IEEE DFMA / DMUL) reproduces it bit for bit.  Checked against the host libm on 3.2e8 floats in
 // |y| < 120 (oracle/crb_oracle.c:crb_oracle_libm_sincosf, tests/test_oracle_ekf.py): sin AND cos identical on
 // every one of them.  (On a host without FMA, glibc's plain build differs from this on 2e-8 of the inputs, by

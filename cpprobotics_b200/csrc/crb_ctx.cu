@@ -33,8 +33,8 @@ int crb_init(crb_ctx** out, int device_id) {
   CRB_REQUIRE(device_id < count, "device_id out of range");
   cudaDeviceProp prop;
   CRB_CUDA(cudaGetDeviceProperties(&prop, device_id));
-  if (prop.major != 10) {
-    crb_set_error("crb_init: device %d is sm_%d%d; libcrb is built for sm_100a only", device_id,
+  if (prop.major != 9 || prop.minor != 0) {
+    crb_set_error("crb_init: device %d is sm_%d%d; libcrb is built for sm_90a only", device_id,
                   prop.major, prop.minor);
     return CRB_ERR_UNSUPPORTED;
   }

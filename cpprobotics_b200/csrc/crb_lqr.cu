@@ -1,4 +1,4 @@
-// crb_lqr.cu — batched discrete LQR gain by the reference's fixed-point DARE iteration, for sm_100a.
+// crb_lqr.cu — batched discrete LQR gain by the reference's fixed-point DARE iteration, for sm_90a.
 //
 // Replaces solve_DARE() + dlqr() of src/lqr_steer_control.cpp:75-96 (nx = 4, nu = 1, scalar R) and
 // src/lqr_speed_steer_control.cpp:85-106 (nx = 5, nu = 2, 2x2 R) for n independent agents per launch

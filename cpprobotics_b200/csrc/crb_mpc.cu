@@ -1,4 +1,4 @@
-// crb_mpc.cu — batched bicycle-model MPC solve for sm_100a.
+// crb_mpc.cu — batched bicycle-model MPC solve for sm_90a.
 //
 // Replaces mpc_solve() + FG_EVAL of the reference, src/model_predictive_control.cpp:188-346 (the
 // CppAD + IPOPT solve of the speed-and-steering NLP), for n independent agents per launch, plus the
@@ -616,8 +616,8 @@ static int mpc_launch(crb_ctx* ctx, cudaStream_t st, int64_t count, int64_t ld, 
     return crb_mpc_tasks_launch(ctx, st, count, ld, T, x0, xref, u_init, scratch, ld_out, sol, u0, cost,
                                 status, iters, p, hint);
   // Experiment kept for A/B (CRB_MPC_L2=1): an L2 persisting access-policy window over the solver
-  // workspace.  Measured on B200: 36.1 M solves/s with it vs 60.0 M without (the set-aside shrinks the
-  // normal L2 and the 152 MB workspace thrashes it), so it is OFF by default.
+  // workspace.  OFF by default: the set-aside shrinks the normal L2 and a workspace several times the L2's
+  // size thrashes it.
   static int l2_mode = -1;
   static size_t l2_max_window = 0, l2_persist = 0;
   if (l2_mode < 0) {
@@ -724,7 +724,7 @@ extern "C" int crb_mpc_solve_batched(crb_ctx* ctx, int64_t n, int T, const float
 // The same solve with a scheduling hint per problem (device, [n]): an estimate of its work, e.g. the `iters` the
 // previous solve of the same agent returned (receding-horizon MPC calls the solver every control step,
 // src/model_predictive_control.cpp:372-378).  Problems with the largest hints start first, which removes most of the
-// tail in which a few late-started long problems run alone (DESIGN.md 3.3).  Results are bit-identical to
+// tail in which a few late-started long problems run alone (DESIGN.md 3).  Results are bit-identical to
 // crb_mpc_solve_batched; hint must not alias `iters` (it is read while results are written).
 extern "C" int crb_mpc_solve_batched_hinted(crb_ctx* ctx, int64_t n, int T, const float* x0, const float* xref,
                                             const float* u_init, const crb_mpc_params* prm, float* sol,
@@ -754,7 +754,7 @@ extern "C" int crb_mpc_solve_batched_host(crb_ctx* ctx, int64_t n, int T, const 
   if (chunk_pref == 0) {
     const char* e = getenv("CRB_MPC_CHUNK");
     // 8192 problems x CRB_N_PIPE = 8 slots: every chunk is resident at once and the first solve starts
-    // after 1/8 of the upload (measured, pinned buffers: 44.5 M solves/s vs 41.8 at 32768, 40.5 at 4096)
+    // after 1/8 of the upload
     chunk_pref = e ? atoll(e) : 8192;
     if (chunk_pref < 128) chunk_pref = 8192;
   }
@@ -771,12 +771,12 @@ extern "C" int crb_mpc_solve_batched_host(crb_ctx* ctx, int64_t n, int T, const 
   // Outputs in pinned + mapped memory are written by the kernel itself (see crb_host_mapped): problems
   // finish at different times, so the stores trickle over PCIe underneath the solve instead of queueing
   // as D2H copies behind it.  Inputs stay on the copy engine: a kernel that reads them over PCIe stalls
-  // its whole (single) wave on the link first (measured: 34.7 M solves/s fully zero-copy vs 37.2 staged).
+  // its whole (single) wave on the link first.
   float *msol = nullptr, *mu0 = nullptr, *mcost = nullptr;
   int32_t *mstat = nullptr, *mit = nullptr;
   // (only the first-generation kernel: its warps store 32 consecutive problems per instruction, whereas the task
   // kernel retires problems in completion order, i.e. as scattered 4-byte stores, which PCIe turns into one
-  // transaction each: measured 4.2 M solves/s instead of 45 M)
+  // transaction each)
   const bool direct_out = mpc_variant() == 0 && crb_zero_copy_enabled() && crb_host_mapped(sol, &msol) &&
                           crb_host_mapped(u0, &mu0) && crb_host_mapped(cost, &mcost) &&
                           crb_host_mapped(status, &mstat) && crb_host_mapped(iters, &mit);

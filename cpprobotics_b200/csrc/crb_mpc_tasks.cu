@@ -1,4 +1,4 @@
-// crb_mpc_tasks.cu — resident-slot MPC solver for sm_100a: persistent CTAs, roll-outs in shared memory,
+// crb_mpc_tasks.cu — resident-slot MPC solver for sm_90a: persistent CTAs, roll-outs in shared memory,
 // sweeps regrouped by kind.
 //
 // Same solver, same bits as crb_mpc_solve_kernel (crb_mpc.cu) and oracle/crb_oracle_mpc.c; replaces
@@ -7,26 +7,26 @@
 //
 //   * One persistent CTA per SM.  A CTA owns S problem SLOTS.  Both roll-out buffers of a slot (X, U: the
 //     data every sweep reads and writes with a dependent chain behind it) and its scalar state stay in
-//     SHARED MEMORY for the whole solve (976 B per slot at T = 20, ~230 slots per SM).  The stage gains and
+//     SHARED MEMORY for the whole solve (976 B per slot at T = 20, up to MPC_TASK_SLOTS per SM).  The stage gains and
 //     the translated reference (written once per backward sweep / once per problem, read by the next
 //     forward sweeps) go to a per-CTA slab of 80-byte stage records in global memory that the CTA reuses for
-//     every problem it ever solves: 148 x S x 1.5 KB ~ 50 MB, resident in the 126 MB L2.  The first version
-//     of the solver streamed a 2.3 KB per-problem workspace through HBM ~20 times per solve (3.1 GB of DRAM
-//     traffic for 53 MB of input + output); here DRAM sees the inputs and the outputs.
+//     every problem it ever solves (SMs x S x 1.5 KB), kept in L2 by an evict_last policy.  The first version
+//     of the solver streamed a 2.3 KB per-problem workspace through HBM ~20 times per solve; here DRAM sees
+//     mostly the inputs and the outputs.
 //   * A problem is advanced one SWEEP at a time (refill = retire + load + initial roll-out, backward,
 //     forward); between sweeps everything it needs is in its slot, so ANY thread can run its next sweep.
 //     Each warp repeatedly takes up to 32 slots that wait for the same kind of sweep and runs that sweep
 //     with one problem per lane.  An adaptive solver diverges badly under a fixed problem-to-lane map
 //     (4..15 outer iterations, 1..5 line-search passes: 16.5 of 32 lanes active in the first version);
 //     regrouped, the lanes of a warp always execute the same sweep kind for the same stage count.
-//   * Problems are pulled from a global counter 32 at a time, so the 148 CTAs balance themselves and the
+//   * Problems are pulled from a global counter 32 at a time, so the CTAs balance themselves and the
 //     inputs of a refill are coalesced 128-byte rows of the SoA arrays.
 //
 // Scheduling state per CTA (shared memory): one ring queue of waiting slots per sweep kind and one lock
 // word.  A warp enters ONE short critical section per task: it appends the slots of the sweep it just
 // finished to the queues of the kinds they wait for next, then takes up to 32 slots from the fullest
-// queue.  (The first version scanned a phase word per slot with 40 ballots under the lock: ncu showed 37 %
-// of all warp samples in that scan and in the lock's spin loop.)  Warps that find nothing wait on a
+// queue.  (The first version scanned a phase word per slot with 40 ballots under the lock, and warps spent
+// much of their time in that scan and in the lock's spin loop.)  Warps that find nothing wait on a
 // sequence word that every post bumps, not on the lock.  All waiting loops are bounded: on overrun the
 // kernel raises the error word in the slab header instead of hanging the GPU.
 #include "crb_common.cuh"
@@ -34,6 +34,10 @@
 #include "crb_mpc_tasks.cuh"
 
 #define MPC_TASK_QS 256  // ring size of the per-kind queues (power of two >= slots per CTA)
+// Slots per CTA at most.  The per-CTA stage-record slabs (SMs x S x (T-1) x 80 B) must leave the 50 MB L2 room
+// for the streaming inputs and outputs: at T = 20 the ~230 slots that shared memory holds make a 46 MB slab.
+// Measured on an H100 SXM (400 W limit), 2^16 problems, T = 20: 52 M solves/s at 160 slots vs 44 M at 230.
+#define MPC_TASK_SLOTS 160
 
 struct MpcTaskArgs {
   int64_t count, ld_in, ld_out;
@@ -70,9 +74,9 @@ __device__ __forceinline__ unsigned lanemask_lt() {
 }
 
 // RING_BULK = false (default): records staged by cp.async commit groups; true (CRB_MPC_RING=bulk): by one 80-byte
-// cp.async.bulk (TMA) per lane and stage on mbarriers.  Measured on B200, config 4: 53.0 M solves/s vs 37.4 M - the
-// TMA engine is built for tiles, and 32 separate 80-byte descriptors per warp and stage cost more than 160 LDGSTS
-// lanes; kept as a compile-time variant (a run-time branch cost 3-5 % in registers and code size).
+// cp.async.bulk (TMA) per lane and stage on mbarriers.  The TMA engine is built for tiles, and 32 separate 80-byte
+// descriptors per warp and stage cost more than 160 LDGSTS lanes; kept as a compile-time variant (a run-time
+// branch costs registers and code size).
 template <bool RING_BULK>
 __global__ void __launch_bounds__(MPC_TASK_MAX_WARPS * 32, 1)
 crb_mpc_tasks_kernel(const __grid_constant__ MpcTaskArgs A, const __grid_constant__ MpcP p) {
@@ -316,7 +320,7 @@ static bool mpc_tasks_geometry(int sm_count, int T, int64_t count, MpcTaskGeom* 
   for (;; --nwarps) {
     fixed = sizeof(MpcSched) + (size_t)nwarps * MPC_RING_BYTES + (size_t)nwarps * MPC_RING_D * 8;
     size_t s = (smem_cap - fixed) / ((size_t)mpc_slot_words(T) * sizeof(float));
-    if (s > MPC_TASK_QS) s = MPC_TASK_QS;
+    if (s > MPC_TASK_SLOTS) s = MPC_TASK_SLOTS;
     S = (int)s;
     if (env_slots > 0 && env_slots < S) S = env_slots;
     if (nwarps == 1) break;
@@ -368,8 +372,8 @@ int crb_mpc_tasks_launch(crb_ctx* ctx, cudaStream_t st, int64_t count, int64_t l
   a.count = count; a.ld_in = ld; a.ld_out = ld_out;
   a.T = T; a.S = g.S; a.slot_words = mpc_slot_words(T);
   {
-    // CRB_MPC_FILL (A/B, read once; default 0 = off).  Measured on B200: holding back batches thinner than 24 / 28 /
-    // 32 slots costs 1 / 2 / 3 % (config 4) - the idle wait is worth more than the fuller warp.
+    // CRB_MPC_FILL (A/B, read once; default 0 = off): hold back batches thinner than this many slots.  Off by
+    // default: the idle wait is worth more than the fuller warp.
     static int fill = -1;
     if (fill < 0) {
       const char* e = getenv("CRB_MPC_FILL");
@@ -389,8 +393,8 @@ int crb_mpc_tasks_launch(crb_ctx* ctx, cudaStream_t st, int64_t count, int64_t l
   a.sol = sol; a.u0 = u0; a.cost = cost; a.status = status; a.iters = iters;
   a.perm = nullptr;
   CRB_CUDA(cudaMemsetAsync(base, 0, MPC_TASK_HEADER_BYTES, st));
-  // With many SM-generations of problems there is no tail to win back and the 15 % scattered refills cost ~3 %
-  // (measured at 2^20 problems): the hints are used up to 6 generations (~170 000 problems on a B200).
+  // With many SM-generations of problems there is no tail to win back and the 15 % scattered refills cost more
+  // than they save: the hints are used up to 6 generations (6 x CTAs x slots problems).
   if (hint != nullptr && count <= 6 * (int64_t)g.grid * g.S) {
     int32_t* perm = (int32_t*)(base + MPC_TASK_HEADER_BYTES + mpc_tasks_slab_bytes(g, T));
     unsigned* hist = (unsigned*)(base + 256);

@@ -13,7 +13,7 @@ All arrays are SoA field-major float32 (`[fields, n]`, C-contiguous); see includ
 without a suffix take CUDA tensors (torch is only the device allocator / stream owner); `*_host`
 methods take host arrays (numpy or CPU torch tensors, ideally pinned) and run the chunked
 copy/compute pipeline inside libcrb.  Nothing here computes: every call goes through the C ABI, and
-raises when libcrb.so or a B200 is missing.
+raises when libcrb.so or an H100 is missing.
 """
 from __future__ import annotations
 

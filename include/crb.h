@@ -1,4 +1,4 @@
-/* crb.h — C ABI of the B200 batched small-matrix engine for the CppRobotics hot paths.
+/* crb.h — C ABI of the H100 batched small-matrix engine for the CppRobotics hot paths.
  *
  * The reference (onlytailei/CppRobotics) has no plugin / FFI surface: its hot functions are free
  * functions inside executable translation units.  This header therefore *defines* the seam at the
@@ -260,8 +260,8 @@ int crb_mpc_solve_batched_host(crb_ctx* ctx, int64_t n, int T, const float* x0, 
  * of the problem's work - in a receding-horizon loop (the caller's loop, :372-378, solves the same vehicle every
  * control step) the `iters` of the agent's previous solve.  The solver is adaptive (3..21 outer iterations on the bench
  * batch); starting the problems with the largest hints first removes most of the tail in which a few late-started
- * long problems run alone (+20 % at 65 536 problems; with more than ~6 SM-generations of problems, ~170 000 on a
- * B200, there is no tail and the hint is ignored).  The hint changes the ORDER in which problems start and nothing
+ * long problems run alone (with more than ~6 SM-generations of problems there is no tail and the hint is
+ * ignored).  The hint changes the ORDER in which problems start and nothing
  * else: results are bit-identical to crb_mpc_solve_batched for any hint.  hint must not alias iters. */
 int crb_mpc_solve_batched_hinted(crb_ctx* ctx, int64_t n, int T, const float* x0, const float* xref,
                                  const float* u_init, const crb_mpc_params* prm, float* sol, float* u0,

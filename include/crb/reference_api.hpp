@@ -1,5 +1,5 @@
 // reference_api.hpp — host C++ with the reference's own names, argument order and value semantics,
-// on top of the C ABI (crb.h).  A CppRobotics main() re-targets to the B200 engine by including this
+// on top of the C ABI (crb.h).  A CppRobotics main() re-targets to the H100 engine by including this
 // header instead of <Eigen/Eigen> for the hot functions and linking libcrb.so.
 //
 //   ekf_estimation(xEst, PEst, z, u, Q, R)        src/extended_kalman_filter.cpp:64-78
@@ -13,7 +13,7 @@
 // Eigen is not a dependency: crb::Mat<R,C> is a POD with the memory layout of
 // Eigen::Matrix<float,R,C> (column-major, contiguous, no padding), enough of its interface for the
 // call sites above.  Errors: the reference reports none; these shims throw std::runtime_error with
-// crb_last_error_string() (e.g. when no B200 is present: there is no CPU fallback).
+// crb_last_error_string() (e.g. when no H100 is present: there is no CPU fallback).
 //
 // These are single-agent calls (n = 1, or NP particles) through the *_host entry points: they exist for
 // drop-in compatibility and for tests; throughput comes from calling the batched C ABI directly.

@@ -26,7 +26,7 @@ HOT = ["crb_ekf_step_kernel<256, 4>", "crb_ekf_step_tma_kernel<256, 2>", "crb_pf
        "crb_mpc_tasks_kernel", "crb_mpc_solve_kernel<0>", "crb_lqr_dlqr_kernel<4, 1>", "crb_probe_ffma_kernel"]
 WATCH = ["FFMA2", "FADD2", "FMUL2", "FFMA", "FMUL", "FADD", "DFMA", "DMUL", "DADD", "MUFU", "UBLKCP", "UTMALDG", "LDGSTS",
          "SYNCS", "LDG", "STG", "LDS", "STS", "ATOMS", "ATOMG", "NANOSLEEP", "SHFL", "VOTE", "HMMA", "UTCHMMA", "UTCQMMA", "BRA"]
-out = [f"# {tag} — SASS evidence per hot kernel (`cuobjdump -sass cpprobotics_b200/lib/libcrb.so`, sm_100a)", "",
+out = [f"# {tag} — SASS evidence per hot kernel (`cuobjdump -sass cpprobotics_b200/lib/libcrb.so`, sm_90a)", "",
        "Counts are static instructions of the kernel.  `FFMA2/FADD2/FMUL2` = packed binary32 (two IEEE-rounded lanes per issue "
        "slot); `UBLKCP` = `cp.async.bulk` (TMA engine, 1-D); `LDGSTS` = `cp.async`; `SYNCS` = mbarrier; `DFMA/DMUL` = the "
        "binary64 sin/cos that carries the host libm's bits; `ATOMS` = shared-memory atomics (the task scheduler's lock).  "

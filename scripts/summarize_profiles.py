@@ -57,7 +57,7 @@ def launches(tag):
 
 
 def captures(tag):
-    out = [f"# {tag} — ncu summary of the three hot kernels (B200, `--set full --clock-control none`)", "",
+    out = [f"# {tag} — ncu summary of the three hot kernels (H100, `--set full --clock-control none`)", "",
            f"Captured by `scripts/gpu_round.sh {tag}` (`ncu ... -k regex:<kernel> -s 2 -c 2 python bench.py --steps 4 "
            "--warmup 3 --no-cpu --workload <w>`);", f"raw reports `gpurun_out/prof_{{ekf,pf,mpc}}_{tag}.ncu-rep` "
            "(scratch, not tracked).  Durations under ncu are cold-cache and serialised; bench numbers are CUDA-event "

@@ -1,6 +1,6 @@
 // Executes the resampling<100>(), solve_DARE() and dlqr() shims of include/crb/reference_api.hpp and dumps what
 // they return.  Linked against tests/cpp/mock_crb.c on a CPU-only machine (marshalling check) or against the
-// real libcrb.so on a B200.  usage: ref_api_shim_check in.bin out.bin
+// real libcrb.so on an H100.  usage: ref_api_shim_check in.bin out.bin
 //   in : seed, px[100][4] (Eigen 4xNP column-major), pw[100], A4[16] B4[4] Q4[16] R4, A5[25] B5[10] Q5[25] R5[4]
 //   out: px[100][4], pw[100], draws[100], X4[16] K4[4], X5[25] K5[10]
 #include <cstdio>

@@ -94,7 +94,7 @@ def test_reference_style_main_matches_oracle(tmp_path):
     pxo, pwo = O.pf_predict_weight_batched(px, pw, nz, lm)
     assert np.abs(pxg - pxo).max() <= 1e-5 * max(1.0, np.abs(pxo).max())
     pwn, xeo, Peo, _ = O.pf_estimate(pxo, pwo)
-    assert np.abs(pwg - pwn).max() <= 2e-3 * np.abs(pwn).max()       # weight conditioning, see DESIGN.md 3.2
+    assert np.abs(pwg - pwn).max() <= 2e-3 * np.abs(pwn).max()       # weight conditioning, see DESIGN.md 3.1
     assert np.abs(xeg - xeo).max() <= 1e-3 and np.abs(Peg - Peo.T.reshape(-1)).max() <= 1e-3
     assert p == out.size
 
