@@ -19,6 +19,10 @@ CRB_COMM_ID_BYTES = 128
 CRB_PF_RESULT_LEN = 24
 CRB_PF_MAX_LANDMARKS = 64
 CRB_MPC_MAX_T = 32
+CRB_DWA_MAX_OBSTACLES = 256
+CRB_DWA_MAX_SPEED_SAMPLES = 64
+CRB_DWA_MAX_YAWRATE_SAMPLES = 512
+CRB_DWA_MAX_STEPS = 1000
 
 c_f32p = C.POINTER(C.c_float)
 c_i32p = C.POINTER(C.c_int32)
@@ -41,6 +45,12 @@ class MpcParams(C.Structure):
                 ("w_ddelta", C.c_float), ("w_x", C.c_float), ("w_y", C.c_float),
                 ("w_yaw", C.c_float), ("w_v", C.c_float), ("max_iter", C.c_int),
                 ("du_th", C.c_float), ("max_ls", C.c_int), ("j_tol", C.c_float)]
+
+
+class DwaParams(C.Structure):
+    _fields_ = [(name, C.c_float) for name in (
+        "max_speed", "min_speed", "max_yawrate", "max_accel", "robot_radius", "max_dyawrate",
+        "v_reso", "yawrate_reso", "dt", "predict_time", "to_goal_cost_gain", "speed_cost_gain")]
 
 
 # name -> (restype, argtypes); every symbol include/crb.h declares
@@ -106,6 +116,11 @@ PROTOTYPES = {
     "crb_lqr_dlqr_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
                                        C.c_void_p]),
+    "crb_dwa_default_params": (None, [C.POINTER(DwaParams)]),
+    "crb_dwa_rollout_points": (C.c_int, [C.POINTER(DwaParams), C.POINTER(C.c_int)]),
+    "crb_dwa_control_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_int, C.POINTER(DwaParams), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "crb_dwa_motion_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float]),
     "crb_stats_reduce": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p]),
     "crb_probe_fp32_peak": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),

@@ -8,6 +8,8 @@ Method names follow the reference functions they replace:
   Engine.mpc_solve           <- mpc_solve()             src/model_predictive_control.cpp:255-346
   Engine.mpc_plant_update    <- update()                src/model_predictive_control.cpp:69-81
   Engine.calc_ref_trajectory <- calc_ref_trajectory()   src/model_predictive_control.cpp:130-170
+  Engine.dwa_control         <- dwa_control()           src/dynamic_window_approach.cpp:148-155
+  Engine.dwa_motion          <- motion()                src/dynamic_window_approach.cpp:43-50
 
 All arrays are SoA field-major float32 (`[fields, n]`, C-contiguous); see include/crb.h.  Methods
 without a suffix take CUDA tensors (torch is only the device allocator / stream owner); `*_host`
@@ -23,7 +25,7 @@ from typing import Optional
 import numpy as np
 
 from . import _lib
-from ._lib import EkfParams, MpcParams, PfParams, check, load_library
+from ._lib import DwaParams, EkfParams, MpcParams, PfParams, check, load_library
 
 try:  # torch is the device-memory / stream / distributed plumbing, never the compute path
     import torch
@@ -46,6 +48,12 @@ def pf_default_params() -> PfParams:
 def mpc_default_params() -> MpcParams:
     p = MpcParams()
     load_library().crb_mpc_default_params(C.byref(p))
+    return p
+
+
+def dwa_default_params() -> DwaParams:
+    p = DwaParams()
+    load_library().crb_dwa_default_params(C.byref(p))
     return p
 
 
@@ -318,6 +326,47 @@ class Engine:
             _ptr(K, np.float32, device=True, name="K"), _ptr(X, np.float32, device=True, name="X"),
             _ptr(iters, np.int32, device=True, name="iters")), "crb_lqr_dlqr_batched")
         return K
+
+    # ---- DWA ----------------------------------------------------------------------------------------
+    def dwa_control(self, x, u, goal, obstacles, params: Optional[DwaParams] = None, cost=None, best=None,
+                    traj=None):
+        """dwa_control() for n robots: x [5,n] (x, y, yaw, v, yawrate), u [2,n] in/out (only u[1] is read),
+        goal [2,n], obstacles [n_ob,2] shared by all robots; optional outputs cost [n] f32, best [n] int32 (flat
+        v-major sample index or -1), traj [5*n_pts,n] (n_pts from dwa_rollout_points).  CUDA tensors; only
+        enqueues."""
+        n = int(x.shape[-1])
+        _shape(x, 5, n, "x"); _shape(u, 2, n, "u"); _shape(goal, 2, n, "goal")
+        if obstacles.dim() != 2 or int(obstacles.shape[1]) != 2:
+            raise ValueError(f"obstacles: expected shape (n_ob, 2), got {tuple(obstacles.shape)}")
+        prm = params if params is not None else dwa_default_params()
+        if cost is not None:
+            _shape(cost, 1, n, "cost")
+        if best is not None:
+            _shape(best, 1, n, "best")
+        if traj is not None:
+            _shape(traj, 5 * self.dwa_rollout_points(prm), n, "traj")
+        check(self.lib.crb_dwa_control_batched(
+            self.ctx, n, _ptr(x, np.float32, device=True, name="x"), _ptr(u, np.float32, device=True, name="u"),
+            _ptr(goal, np.float32, device=True, name="goal"),
+            _ptr(obstacles, np.float32, device=True, name="obstacles"), int(obstacles.shape[0]), C.byref(prm),
+            _ptr(cost, np.float32, device=True, name="cost"), _ptr(best, np.int32, device=True, name="best"),
+            _ptr(traj, np.float32, device=True, name="traj")), "crb_dwa_control_batched")
+
+    def dwa_rollout_points(self, params: Optional[DwaParams] = None) -> int:
+        """Points per rollout (steps + 1): 32 for the reference's Config."""
+        k = C.c_int(0)
+        prm = params if params is not None else dwa_default_params()
+        check(self.lib.crb_dwa_rollout_points(C.byref(prm), C.byref(k)), "crb_dwa_rollout_points")
+        return int(k.value)
+
+    def dwa_motion(self, x, u, dt: Optional[float] = None):
+        """motion() in place on x [5,n] with u [2,n]; dt defaults to the reference's Config.dt."""
+        n = int(x.shape[-1])
+        _shape(x, 5, n, "x"); _shape(u, 2, n, "u")
+        d = dwa_default_params().dt if dt is None else dt
+        check(self.lib.crb_dwa_motion_batched(self.ctx, n, _ptr(x, np.float32, device=True, name="x"),
+                                              _ptr(u, np.float32, device=True, name="u"), C.c_float(d)),
+              "crb_dwa_motion_batched")
 
     # ---- multi-GPU: the communicator lives in libcrb (crb_comm.cu), not in torch --------------------
     @staticmethod

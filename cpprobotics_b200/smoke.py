@@ -16,6 +16,7 @@ def run() -> None:
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     if root not in sys.path:
         sys.path.insert(0, root)
+    from oracle import dwa as OD  # checker only
     from oracle import oracle as O  # checker only
 
     from . import synth
@@ -103,5 +104,22 @@ def run() -> None:
     keys = {tuple(c) for c in src.T}
     assert all(tuple(c) in keys for c in got.T[:: max(1, npf // 256)]), "a resampled particle is not a copy of an input"
     print(f"smoke PF    full iteration n={npf}: sum_w / xEst match the oracle, particles resampled on the device")
+    # DWA: 4097 robots against the demo's 10 obstacles, bit-identical to the oracle
+    nd = 4097
+    xw, uw, gw = synth.dwa_inputs(nd)
+    ob = synth.DWA_DEMO_OBSTACLES
+    n_pts = eng.dwa_rollout_points()
+    xwd, uwd, gwd, obd = (torch.from_numpy(a).to(dev) for a in (xw, uw, gw, ob))
+    cw = torch.empty(nd, dtype=torch.float32, device=dev)
+    bw = torch.empty(nd, dtype=torch.int32, device=dev)
+    tw = torch.empty((5 * n_pts, nd), dtype=torch.float32, device=dev)
+    eng.dwa_control(xwd, uwd, gwd, obd, cost=cw, best=bw, traj=tw)
+    torch.cuda.synchronize()
+    rw = OD.dwa_control(xw, uw, gw, ob)
+    same = all(np.array_equal(a.cpu().numpy().view(np.uint32), b.view(np.uint32))
+               for a, b in ((uwd, rw["u"]), (cw, rw["cost"]), (bw, rw["best"]), (tw, rw["traj"])))
+    assert same, "DWA GPU result is not bit-identical to the oracle"
+    print(f"smoke DWA   n={nd} obstacles={len(ob)}: bit-identical to the oracle; "
+          f"{int((bw >= 0).sum().item())}/{nd} robots with an admissible sample")
     print(f"smoke ok: {eng.launches} kernel launches through libcrb.so")
     eng.close()

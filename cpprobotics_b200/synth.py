@@ -186,3 +186,47 @@ def lqr_inputs(n: int, nx: int, i0: int = 0, seed: int = 0xC0FFEE, dt: float = 0
         A[4 + nx * 4] = 1.0
         B[4 + nx * 1] = np.float32(dt)
     return A, B, np.eye(nx, dtype=np.float32).reshape(-1), np.eye(nu, dtype=np.float32).reshape(-1)
+
+
+# ---- dynamic window approach (src/dynamic_window_approach.cpp) --------------------------------------------
+# main()'s obstacle list (:169-180), start state (:167) and goal (:168)
+DWA_DEMO_OBSTACLES = np.array([[-1, -1], [0, 2], [4, 2], [5, 4], [5, 5], [5, 6], [5, 9], [8, 9], [7, 9], [12, 12]],
+                              np.float32)
+DWA_DEMO_START = (0.0, 0.0, 3.141592653 / 8.0, 0.0, 0.0)
+DWA_DEMO_GOAL = (10.0, 10.0)
+
+
+def dwa_inputs(n: int, seed: int = 0xC0FFEE, i0: int = 0, max_speed: float = 1.0, min_speed: float = -0.5,
+               max_yawrate: float = 40.0 * 3.141592653 / 180.0):
+    """x [5,n] (x, y, yaw, v, yawrate), u [2,n] (u[1] = the previous yaw rate), goal [2,n], float32.
+    Robots in the demo's arena ([-2, 12]^2, goal anywhere in it), v and yaw rate inside the limits; one robot in
+    four sits exactly at a speed limit and one in four at a yaw-rate limit, so its window is clipped (:55-58)."""
+    idx = np.arange(i0, i0 + n, dtype=np.uint64)
+    f = np.float32
+    x = np.empty((5, n), np.float32)
+    x[0] = uniform(seed, 110, idx, -2.0, 12.0)
+    x[1] = uniform(seed, 111, idx, -2.0, 12.0)
+    x[2] = uniform(seed, 112, idx, -np.pi, np.pi)
+    x[3] = uniform(seed, 113, idx, min_speed, max_speed)
+    x[4] = uniform(seed, 114, idx, -max_yawrate, max_yawrate)
+    pick_v = u01(seed, 115, idx)
+    pick_w = u01(seed, 116, idx)
+    x[3] = np.where(pick_v < 0.125, f(max_speed), np.where(pick_v < 0.25, f(min_speed), x[3]))
+    x[4] = np.where(pick_w < 0.125, f(max_yawrate), np.where(pick_w < 0.25, f(-max_yawrate), x[4]))
+    u = np.empty((2, n), np.float32)
+    u[0] = x[3]
+    u[1] = x[4]
+    goal = np.empty((2, n), np.float32)
+    goal[0] = uniform(seed, 117, idx, -2.0, 12.0)
+    goal[1] = uniform(seed, 118, idx, -2.0, 12.0)
+    return np.ascontiguousarray(x), np.ascontiguousarray(u), np.ascontiguousarray(goal)
+
+
+def dwa_obstacles(k: int, seed: int = 0xC0FFEE) -> np.ndarray:
+    """[k, 2] rows (ox, oy), obstacle j a function of (seed, j, k) only: uniform in a square around the demo's
+    arena that grows with k so that the density stays the demo's (10 in 14 m x 14 m) and most robots keep an
+    admissible sample."""
+    idx = np.arange(k, dtype=np.uint64)
+    h = 7.0 * max(1.0, np.sqrt(k / 10.0))
+    ob = np.stack([uniform(seed, 120, idx, 5.0 - h, 5.0 + h), uniform(seed, 121, idx, 5.0 - h, 5.0 + h)], axis=1)
+    return np.ascontiguousarray(ob.astype(np.float32))

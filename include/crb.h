@@ -17,6 +17,9 @@
  *   crb_mpc_calc_ref_trajectory_batched <- calc_ref_trajectory() :130-170 + calc_nearest_index() :107-127
  *   crb_lqr_dlqr_batched                <- solve_DARE() + dlqr()  src/lqr_steer_control.cpp:75-96,
  *                                          src/lqr_speed_steer_control.cpp:85-106
+ *   crb_dwa_control_batched             <- dwa_control()         src/dynamic_window_approach.cpp:148-155
+ *                                         (calc_dynamic_window :52-60, calc_final_input :115-145 and the costs)
+ *   crb_dwa_motion_batched              <- motion()              src/dynamic_window_approach.cpp:43-50
  *   crb_stats_*                         <- (no reference counterpart) per-GPU summary statistics, the
  *                                          only thing that ever crosses NVLink (one all-gather).
  *
@@ -297,6 +300,49 @@ int crb_mpc_calc_ref_trajectory_batched(crb_ctx* ctx, int64_t n, int T, const fl
 int crb_lqr_dlqr_batched(crb_ctx* ctx, int64_t n, int nx, int nu, const float* A, const float* B,
                          const float* Q, const float* R, int maxiter, float eps, float* K, float* X,
                          int32_t* iters);
+
+/* ---- dynamic window approach (src/dynamic_window_approach.cpp) ------------------------------------ */
+/* class Config :25-41: the same members in the same order. */
+typedef struct crb_dwa_params {
+  float max_speed, min_speed, max_yawrate, max_accel, robot_radius, max_dyawrate;
+  float v_reso, yawrate_reso, dt, predict_time, to_goal_cost_gain, speed_cost_gain;
+} crb_dwa_params;
+/* The reference's values, including its truncated PI (3.141592653, :16):
+ * max_yawrate = max_dyawrate = (float)(40.0 * PI / 180.0), yawrate_reso = (float)(0.1 * PI / 180.0). */
+void crb_dwa_default_params(crb_dwa_params* p);
+
+/* Limits.  Every parameter must be finite, v_reso, yawrate_reso and dt > 0, and
+ *   min(2 max_accel dt, max_speed - min_speed) / v_reso + 2          <= CRB_DWA_MAX_SPEED_SAMPLES
+ *   min(2 max_dyawrate dt, 2 max_yawrate) / yawrate_reso + 2         <= CRB_DWA_MAX_YAWRATE_SAMPLES
+ *   rollout steps (the reference's `time += dt` loop, :67-72)        <= CRB_DWA_MAX_STEPS
+ * otherwise CRB_ERR_INVALID_ARG.  A window is sampled by the reference's float accumulation (:126-127); for a
+ * state so large that v + v_reso == v the reference never terminates, here the axis stops at its cap. */
+#define CRB_DWA_MAX_OBSTACLES 256
+#define CRB_DWA_MAX_SPEED_SAMPLES 64
+#define CRB_DWA_MAX_YAWRATE_SAMPLES 512
+#define CRB_DWA_MAX_STEPS 1000
+/* Points of every rollout (steps + 1): 32 for the defaults.  CRB_ERR_INVALID_ARG for parameters out of the
+ * limits above. */
+int crb_dwa_rollout_points(const crb_dwa_params* p, int* n_pts);
+
+/*   x [5][n] (x, y, yaw, v, yawrate), goal [2][n], u [2][n] in/out (in: only u[1] is read, :121-122)
+ *   ob [n_ob][2] rows (ox, oy) shared by the whole batch (may be NULL when n_ob = 0)
+ *   optional outputs, NULL = not written:
+ *     cost [n]  the final min_cost (10000 when no sample is admissible)
+ *     best [n]  int32: v-major flat index of the chosen sample, or -1
+ *     traj [5*n_pts][n]  field 5k+j = component j of point k of the chosen rollout (NaN when best = -1)
+ * All DEVICE pointers (x, u, goal may be NULL when n = 0: a no-op).  Bit-exact with the reference: its float sample grid, std::max / std::min, the double
+ * pow / sqrt of the goal cost, glibc's sinf / cosf / acosf, and its selection rule `min_cost >= cost`
+ * (the last sample in v-major order with the minimum cost wins, a NaN cost never does, u = (0, u[1]) when
+ * nothing is admissible).  Only enqueues on the context's stream (capturable in a CUDA graph).
+ * Replaces: dwa_control() :148-155 (calc_dynamic_window :52-60, calc_final_input :115-145, calc_trajectory
+ * :63-74, calc_obstacle_cost :77-101, calc_to_goal_cost :103-113). */
+int crb_dwa_control_batched(crb_ctx* ctx, int64_t n, const float* x, float* u, const float* goal,
+                            const float* ob, int n_ob, const crb_dwa_params* prm, float* cost,
+                            int32_t* best, float* traj);
+/* x [5][n] in/out, u [2][n] (DEVICE; NULL allowed when n = 0).  dt finite and > 0.
+ * Replaces: motion(x, u, dt) :43-50, the plant step of main() :194. */
+int crb_dwa_motion_batched(crb_ctx* ctx, int64_t n, float* x, const float* u, float dt);
 
 /* ---- multi-GPU: communicator owned by the context (NCCL, opened at run time) ---------------------- */
 /* The batch shards over GPUs by contiguous agent ranges (one crb_ctx per device, one host thread or process

@@ -9,6 +9,7 @@
 //   calc_ref_trajectory(...)                      src/model_predictive_control.cpp:130-170
 //   resampling(px, pw, gen, uni_d)                src/particle_filter.cpp:120-148
 //   solve_DARE / dlqr (4x4 and 5x5)               src/lqr_steer_control.cpp:75-96, lqr_speed_steer_control.cpp:85-106
+//   dwa_control(x, u, config, goal, ob), motion(x, u, dt)   src/dynamic_window_approach.cpp:148-155, :43-50
 //
 // Eigen is not a dependency: crb::Mat<R,C> is a POD with the memory layout of
 // Eigen::Matrix<float,R,C> (column-major, contiguous, no padding), enough of its interface for the
@@ -324,6 +325,60 @@ inline crb::Matrix25f dlqr(crb::Matrix5f A, crb::Matrix52f B, crb::Matrix5f Q, c
   crb::Matrix25f K;
   crb::dlqr_impl<5, 2>(A.data(), B.data(), Q.data(), R.data(), K.data(), nullptr);
   return K;
+}
+
+// src/dynamic_window_approach.cpp.  Its State, Control, Point, Traj and Obstacle (:18-23) are aliases of exactly
+// these std types, and its Config (:25-41) is the program's own class, read here by member name.
+namespace crb {
+template <class Config>
+inline crb_dwa_params dwa_params_of(const Config& c) {
+  crb_dwa_params p;
+  p.max_speed = c.max_speed; p.min_speed = c.min_speed; p.max_yawrate = c.max_yawrate;
+  p.max_accel = c.max_accel; p.robot_radius = c.robot_radius; p.max_dyawrate = c.max_dyawrate;
+  p.v_reso = c.v_reso; p.yawrate_reso = c.yawrate_reso; p.dt = c.dt; p.predict_time = c.predict_time;
+  p.to_goal_cost_gain = c.to_goal_cost_gain; p.speed_cost_gain = c.speed_cost_gain;
+  return p;
+}
+}  // namespace crb
+
+// dwa_control :148-155: sets u and returns the chosen rollout (empty when no sample is admissible, like the
+// reference).  ob must have at most CRB_DWA_MAX_OBSTACLES rows.
+template <class Config>
+inline std::vector<std::array<float, 5>> dwa_control(std::array<float, 5> x, std::array<float, 2>& u, Config config,
+                                                     std::array<float, 2> goal,
+                                                     std::vector<std::array<float, 2>> ob) {
+  crb_ctx* ctx = crb::Session::get();
+  const crb_dwa_params prm = crb::dwa_params_of(config);
+  int n_pts = 0;
+  crb::check(crb_dwa_rollout_points(&prm, &n_pts), "crb_dwa_rollout_points");
+  const size_t n_ob = ob.size();
+  // x [5] | u [2] | goal [2] | ob [n_ob][2] | best [1] | traj [5 n_pts]  (n = 1: SoA and AoS coincide)
+  float* dx = crb::Session::scratch(10 + 2 * n_ob + 5 * (size_t)n_pts);
+  float *du = dx + 5, *dg = du + 2, *dob = dg + 2, *dbest = dob + 2 * n_ob, *dtraj = dbest + 1;
+  crb::check(crb_memcpy_h2d(ctx, dx, x.data(), 5 * sizeof(float)), "h2d");
+  crb::check(crb_memcpy_h2d(ctx, du, u.data(), 2 * sizeof(float)), "h2d");
+  crb::check(crb_memcpy_h2d(ctx, dg, goal.data(), 2 * sizeof(float)), "h2d");
+  if (n_ob) crb::check(crb_memcpy_h2d(ctx, dob, ob.data(), 2 * n_ob * sizeof(float)), "h2d");
+  crb::check(crb_dwa_control_batched(ctx, 1, dx, du, dg, dob, (int)n_ob, &prm, nullptr, (int32_t*)dbest, dtraj),
+             "crb_dwa_control_batched");
+  int32_t best = -1;
+  std::vector<std::array<float, 5>> traj((size_t)n_pts);
+  crb::check(crb_memcpy_d2h(ctx, u.data(), du, 2 * sizeof(float)), "d2h");
+  crb::check(crb_memcpy_d2h(ctx, &best, dbest, sizeof(best)), "d2h");
+  crb::check(crb_memcpy_d2h(ctx, traj.data(), dtraj, 5 * (size_t)n_pts * sizeof(float)), "d2h");
+  if (best < 0) traj.clear();
+  return traj;
+}
+
+// motion :43-50 (the plant step of main() :194)
+inline std::array<float, 5> motion(std::array<float, 5> x, std::array<float, 2> u, float dt) {
+  crb_ctx* ctx = crb::Session::get();
+  float* dx = crb::Session::scratch(7);
+  crb::check(crb_memcpy_h2d(ctx, dx, x.data(), 5 * sizeof(float)), "h2d");
+  crb::check(crb_memcpy_h2d(ctx, dx + 5, u.data(), 2 * sizeof(float)), "h2d");
+  crb::check(crb_dwa_motion_batched(ctx, 1, dx, dx + 5, dt), "crb_dwa_motion_batched");
+  crb::check(crb_memcpy_d2h(ctx, x.data(), dx, 5 * sizeof(float)), "d2h");
+  return x;
 }
 
 #endif  // CRB_REFERENCE_API_HPP_
