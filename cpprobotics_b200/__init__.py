@@ -4,9 +4,10 @@ The product is libcrb.so (hand-written sm_90a CUDA behind the C ABI of include/c
 is the thin Python host layer the tests and the bench use to reach it.  There is no CPU path here:
 importing works anywhere (so the build can be checked without a GPU), computing needs an H100.
 """
-from ._lib import CrbError, DwaParams, EkfParams, MpcParams, PfParams, load_library  # noqa: F401
+from ._lib import CrbError, DwaParams, EkfParams, MpcParams, MptgParams, PfParams, load_library  # noqa: F401
 from .engine import (Engine, dwa_default_params, ekf_default_params,  # noqa: F401
-                     mpc_default_params, pf_default_params)
+                     mpc_default_params, mptg_default_params, pf_default_params)
 
-__all__ = ["Engine", "CrbError", "EkfParams", "PfParams", "MpcParams", "DwaParams", "load_library",
-           "ekf_default_params", "pf_default_params", "mpc_default_params", "dwa_default_params"]
+__all__ = ["Engine", "CrbError", "EkfParams", "PfParams", "MpcParams", "DwaParams", "MptgParams", "load_library",
+           "ekf_default_params", "pf_default_params", "mpc_default_params", "dwa_default_params",
+           "mptg_default_params"]

@@ -23,6 +23,13 @@ CRB_DWA_MAX_OBSTACLES = 256
 CRB_DWA_MAX_SPEED_SAMPLES = 64
 CRB_DWA_MAX_YAWRATE_SAMPLES = 512
 CRB_DWA_MAX_STEPS = 1000
+CRB_MPTG_MAX_ITER = 1000
+CRB_MPTG_MAX_STEPS = 16384
+CRB_MPTG_CONVERGED = 0
+CRB_MPTG_MAX_ITER_REACHED = 1
+CRB_MPTG_EMPTY_TRAJ = 2
+CRB_MPTG_STEP_CAP = 3
+CRB_MPTG_OUT_OF_RANGE = 4
 
 c_f32p = C.POINTER(C.c_float)
 c_i32p = C.POINTER(C.c_int32)
@@ -51,6 +58,11 @@ class DwaParams(C.Structure):
     _fields_ = [(name, C.c_float) for name in (
         "max_speed", "min_speed", "max_yawrate", "max_accel", "robot_radius", "max_dyawrate",
         "v_reso", "yawrate_reso", "dt", "predict_time", "to_goal_cost_gain", "speed_cost_gain")]
+
+
+class MptgParams(C.Structure):
+    _fields_ = [("base_l", C.c_float), ("ds", C.c_float), ("max_iter", C.c_int32), ("cost_th", C.c_float),
+                ("h_step", C.c_float * 3)]
 
 
 # name -> (restype, argtypes); every symbol include/crb.h declares
@@ -121,6 +133,13 @@ PROTOTYPES = {
     "crb_dwa_control_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_int, C.POINTER(DwaParams), C.c_void_p, C.c_void_p, C.c_void_p]),
     "crb_dwa_motion_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float]),
+    "crb_mptg_default_params": (None, [C.POINTER(MptgParams)]),
+    "crb_mptg_optimize_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.POINTER(MptgParams), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]),
+    "crb_mptg_generate_trajectory_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                                       C.POINTER(MptgParams), C.c_int, C.c_void_p, C.c_void_p,
+                                                       C.c_void_p, C.c_void_p]),
     "crb_stats_reduce": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p]),
     "crb_probe_fp32_peak": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),

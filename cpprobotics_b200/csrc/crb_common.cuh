@@ -231,3 +231,82 @@ __device__ __forceinline__ void crb_sincosf_libm(float y, float& sn, float& cs) 
   sn = (n & 1) ? pc : ps;
   cs = (n & 1) ? ps : pc;
 }
+
+// ---- tanf with the HOST libm's bits ---------------------------------------------------------------------
+// The reference calls std::tan on a float (include/motion_model.h:105), i.e. glibc's tanf.  glibc 2.39 computes
+// it with fdlibm's binary32 s_tanf.c / k_tanf.c (Sun Microsystems, freely redistributable): |x| <= pi/4 goes
+// straight to __kernel_tanf(x, 0, 1); above that, __ieee754_rem_pio2f reduces by pi/2 with the same binary64
+// reduce_fast as sinf (n from the 2^24/pi product, then x - n * pi/2 as a separate multiply and subtract: unlike
+// sinf's, this file is not built with FMA) and splits the remainder into y0 = (float)r, y1 = (float)(r - y0);
+// __kernel_tanf(y0, y1, +-1) then works in float only.  Restated operation for operation with explicitly rounded
+// intrinsics, so it does not depend on the TU's -fmad setting.  Checked against the host tanf on every one of the
+// 2,246,049,792 floats with |x| < 120 (oracle/crb_oracle_mptg.c: crb_oracle_libm_tanf_census, tests/test_mptg.py).
+// |x| >= 120 (glibc's reduce_large) is not restated: crb_tanf_libm_in_range() says whether x is inside the
+// proven range, and callers must not use the result outside it.  Inf and NaN give NaN, as glibc does.
+__device__ __forceinline__ bool crb_tanf_libm_in_range(float x) {
+  const unsigned ix = __float_as_uint(x) & 0x7fffffffu;
+  return ix < 0x42f00000u || ix >= 0x7f800000u;  // |x| < 120, or not finite
+}
+static __device__ __noinline__ float crb_tanf_kernel(float x, float y, int iy) {  // __kernel_tanf, iy = +1 / -1
+  const float pio4 = 7.8539812565e-01f, pio4lo = 3.7748947079e-08f;
+  const float T0 = 3.3333334327e-01f, T1 = 1.3333334029e-01f, T2 = 5.3968254477e-02f, T3 = 2.1869488060e-02f,
+              T4 = 8.8632395491e-03f, T5 = 3.5920790397e-03f, T6 = 1.4562094584e-03f, T7 = 5.8804126456e-04f,
+              T8 = 2.4646313977e-04f, T9 = 7.8179444245e-05f, T10 = 7.1407252108e-05f, T11 = -1.8558637748e-05f,
+              T12 = 2.5907305826e-05f;
+  const int hx = __float_as_int(x);
+  const int ix = hx & 0x7fffffff;
+  if (ix < 0x39000000) {  // |x| < 2^-13
+    if (iy == 1) return x;
+    if (ix == 0) return __fdiv_rn(1.0f, fabsf(x));  // glibc's one / fabsf(x) for x = +-0, iy = -1
+    return __fdiv_rn(-1.0f, x);
+  }
+  const bool big = ix >= 0x3f2ca140;  // |x| >= 0.6744
+  if (big) {
+    if (hx < 0) {
+      x = -x;
+      y = -y;
+    }
+    const float z = __fsub_rn(pio4, x), w = __fsub_rn(pio4lo, y);
+    x = __fadd_rn(z, w);
+    y = 0.0f;
+    if (fabsf(x) < 0x1p-13f) {  // (1 - ((hx >> 30) & 2)) * iy * (1.0f - 2 * iy * x): products by +-1, +-2 are exact
+      const float sg = (float)((1 - ((hx >> 30) & 2)) * iy);
+      return __fmul_rn(sg, __fsub_rn(1.0f, __fmul_rn((float)(2 * iy), x)));
+    }
+  }
+  const float z = __fmul_rn(x, x);
+  const float w = __fmul_rn(z, z);
+  float r = __fadd_rn(T1, __fmul_rn(w, __fadd_rn(T3, __fmul_rn(w, __fadd_rn(T5, __fmul_rn(w, __fadd_rn(T7,
+            __fmul_rn(w, __fadd_rn(T9, __fmul_rn(w, T11))))))))));
+  float v = __fmul_rn(z, __fadd_rn(T2, __fmul_rn(w, __fadd_rn(T4, __fmul_rn(w, __fadd_rn(T6, __fmul_rn(w,
+            __fadd_rn(T8, __fmul_rn(w, __fadd_rn(T10, __fmul_rn(w, T12)))))))))));
+  const float s = __fmul_rn(z, x);
+  r = __fadd_rn(y, __fmul_rn(z, __fadd_rn(__fmul_rn(s, __fadd_rn(r, v)), y)));
+  r = __fadd_rn(r, __fmul_rn(T0, s));
+  const float ww = __fadd_rn(x, r);
+  if (big) {
+    const float fv = (float)iy;
+    const float q = __fsub_rn(__fdiv_rn(__fmul_rn(ww, ww), __fadd_rn(ww, fv)), r);
+    return __fmul_rn((float)(1 - ((hx >> 30) & 2)), __fsub_rn(fv, __fmul_rn(2.0f, __fsub_rn(x, q))));
+  }
+  if (iy == 1) return ww;
+  // -1 / (x + r) to full precision
+  const float zz = __int_as_float(__float_as_int(ww) & (int)0xfffff000);
+  const float vv = __fsub_rn(r, __fsub_rn(zz, x));
+  const float a = __fdiv_rn(-1.0f, ww);
+  const float t = __int_as_float(__float_as_int(a) & (int)0xfffff000);
+  const float ss = __fadd_rn(1.0f, __fmul_rn(t, zz));
+  return __fadd_rn(t, __fmul_rn(a, __fadd_rn(ss, __fmul_rn(t, vv))));
+}
+__device__ __forceinline__ float crb_tanf_libm(float x) {
+  const unsigned ix = __float_as_uint(x) & 0x7fffffffu;
+  if (ix <= 0x3f490fdau) return crb_tanf_kernel(x, 0.0f, 1);  // |x| <= pi/4
+  if (ix >= 0x7f800000u) return __fsub_rn(x, x);             // inf, NaN
+  // reduce_fast (|x| < 120; larger x gets no meaningful result, see crb_tanf_libm_in_range)
+  const double dx = (double)x;
+  const int n = ((int)__dmul_rn(dx, 0x1.45F306DC9C883p+23) + 0x800000) >> 24;
+  const double d = __dsub_rn(dx, __dmul_rn((double)n, 0x1.921FB54442D18p0));
+  const float y0 = __double2float_rn(d);
+  const float y1 = __double2float_rn(__dsub_rn(d, (double)y0));
+  return crb_tanf_kernel(y0, y1, 1 - ((n & 1) << 1));
+}

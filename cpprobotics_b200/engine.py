@@ -10,6 +10,8 @@ Method names follow the reference functions they replace:
   Engine.calc_ref_trajectory <- calc_ref_trajectory()   src/model_predictive_control.cpp:130-170
   Engine.dwa_control         <- dwa_control()           src/dynamic_window_approach.cpp:148-155
   Engine.dwa_motion          <- motion()                src/dynamic_window_approach.cpp:43-50
+  Engine.mptg_optimize       <- TrajectoryOptimizer::optimizer_traj()  include/trajectory_optimizer.h:53-128
+  Engine.mptg_generate_trajectory <- MotionModel::generate_trajectory() include/motion_model.h:110-131
 
 All arrays are SoA field-major float32 (`[fields, n]`, C-contiguous); see include/crb.h.  Methods
 without a suffix take CUDA tensors (torch is only the device allocator / stream owner); `*_host`
@@ -25,7 +27,7 @@ from typing import Optional
 import numpy as np
 
 from . import _lib
-from ._lib import DwaParams, EkfParams, MpcParams, PfParams, check, load_library
+from ._lib import DwaParams, EkfParams, MpcParams, MptgParams, PfParams, check, load_library
 
 try:  # torch is the device-memory / stream / distributed plumbing, never the compute path
     import torch
@@ -54,6 +56,12 @@ def mpc_default_params() -> MpcParams:
 def dwa_default_params() -> DwaParams:
     p = DwaParams()
     load_library().crb_dwa_default_params(C.byref(p))
+    return p
+
+
+def mptg_default_params() -> MptgParams:
+    p = MptgParams()
+    load_library().crb_mptg_default_params(C.byref(p))
     return p
 
 
@@ -367,6 +375,61 @@ class Engine:
         check(self.lib.crb_dwa_motion_batched(self.ctx, n, _ptr(x, np.float32, device=True, name="x"),
                                               _ptr(u, np.float32, device=True, name="u"), C.c_float(d)),
               "crb_dwa_motion_batched")
+
+    # ---- model-predictive trajectory generation ---------------------------------------------------------
+    @staticmethod
+    def mptg_default_params() -> MptgParams:
+        """The demo's base_l, ds, max_iter, cost_th and h_step (src/model_predictive_trajectory_generator.cpp)."""
+        return mptg_default_params()
+
+    def mptg_optimize(self, state, target, param, params: Optional[MptgParams] = None, traj=None, traj_len=None,
+                      cost=None, status=None, iters=None):
+        """optimizer_traj() for n problems: state [4,n] (x, y, yaw, v), target [3,n] (x, y, yaw), param [4,n] in/out
+        (distance, steering_sequence[0..2]).  Optional outputs: traj [3*max_pts,n] (max_pts = traj.shape[0] // 3; the
+        first min(traj_len, max_pts) points are written), traj_len [n] int32, cost [n] f32, status [n] int32
+        (CRB_MPTG_*), iters [n] int32.  CUDA tensors; only enqueues."""
+        n = int(state.shape[-1])
+        _shape(state, 4, n, "state"); _shape(target, 3, n, "target"); _shape(param, 4, n, "param")
+        prm = params if params is not None else mptg_default_params()
+        max_pts = self._mptg_max_pts(traj, n)
+        for a, name in ((traj_len, "traj_len"), (cost, "cost"), (status, "status"), (iters, "iters")):
+            if a is not None:
+                _shape(a, 1, n, name)
+        check(self.lib.crb_mptg_optimize_batched(
+            self.ctx, n, _ptr(state, np.float32, device=True, name="state"),
+            _ptr(target, np.float32, device=True, name="target"), _ptr(param, np.float32, device=True, name="param"),
+            C.byref(prm), max_pts, _ptr(traj, np.float32, device=True, name="traj"),
+            _ptr(traj_len, np.int32, device=True, name="traj_len"), _ptr(cost, np.float32, device=True, name="cost"),
+            _ptr(status, np.int32, device=True, name="status"), _ptr(iters, np.int32, device=True, name="iters")),
+            "crb_mptg_optimize_batched")
+
+    def mptg_generate_trajectory(self, state, param, params: Optional[MptgParams] = None, traj=None, traj_len=None,
+                                 last=None, status=None):
+        """MotionModel::generate_trajectory() for n parameters: state [4,n], param [4,n]; optional outputs traj
+        [3*max_pts,n], traj_len [n] int32, last [3,n] (generate_last_state), status [n] int32.  CUDA tensors."""
+        n = int(state.shape[-1])
+        _shape(state, 4, n, "state"); _shape(param, 4, n, "param")
+        prm = params if params is not None else mptg_default_params()
+        max_pts = self._mptg_max_pts(traj, n)
+        if last is not None:
+            _shape(last, 3, n, "last")
+        for a, name in ((traj_len, "traj_len"), (status, "status")):
+            if a is not None:
+                _shape(a, 1, n, name)
+        check(self.lib.crb_mptg_generate_trajectory_batched(
+            self.ctx, n, _ptr(state, np.float32, device=True, name="state"),
+            _ptr(param, np.float32, device=True, name="param"), C.byref(prm), max_pts,
+            _ptr(traj, np.float32, device=True, name="traj"), _ptr(traj_len, np.int32, device=True, name="traj_len"),
+            _ptr(last, np.float32, device=True, name="last"), _ptr(status, np.int32, device=True, name="status")),
+            "crb_mptg_generate_trajectory_batched")
+
+    @staticmethod
+    def _mptg_max_pts(traj, n: int) -> int:
+        if traj is None:
+            return 0
+        if traj.dim() != 2 or int(traj.shape[0]) % 3 or int(traj.shape[1]) != n:
+            raise ValueError(f"traj: expected shape (3*max_pts, {n}), got {tuple(traj.shape)}")
+        return int(traj.shape[0]) // 3
 
     # ---- multi-GPU: the communicator lives in libcrb (crb_comm.cu), not in torch --------------------
     @staticmethod

@@ -17,6 +17,7 @@ def run() -> None:
     if root not in sys.path:
         sys.path.insert(0, root)
     from oracle import dwa as OD  # checker only
+    from oracle import mptg as OM  # checker only
     from oracle import oracle as O  # checker only
 
     from . import synth
@@ -121,5 +122,27 @@ def run() -> None:
     assert same, "DWA GPU result is not bit-identical to the oracle"
     print(f"smoke DWA   n={nd} obstacles={len(ob)}: bit-identical to the oracle; "
           f"{int((bw >= 0).sum().item())}/{nd} robots with an admissible sample")
+    # MPTG: 4097 trajectory optimisations around the demo's target, the same as the checker (any NaN equals any NaN)
+    nm, mp = 4097, 64
+    sm, tm, pm = synth.mptg_inputs(nm)
+    smd, tmd, pmd = (torch.from_numpy(a).to(dev) for a in (sm, tm, pm))
+    trm = torch.zeros((3 * mp, nm), dtype=torch.float32, device=dev)
+    i32 = [torch.empty(nm, dtype=torch.int32, device=dev) for _ in range(3)]
+    cm = torch.empty(nm, dtype=torch.float32, device=dev)
+    eng.mptg_optimize(smd, tmd, pmd, traj=trm, traj_len=i32[0], cost=cm, status=i32[1], iters=i32[2])
+    torch.cuda.synchronize()
+    rm = OM.optimize(sm, tm, pm, max_pts=mp, traj_fill=0.0)
+
+    def same_nan(a, b):
+        a, b = a.cpu().numpy(), np.asarray(b)
+        if a.dtype.kind != "f":
+            return np.array_equal(a, b)
+        na, nb = np.isnan(a), np.isnan(b)
+        return np.array_equal(na, nb) and np.array_equal(a[~na].view(np.uint32), b[~nb].view(np.uint32))
+    ok = all(same_nan(g, rm[k]) for g, k in ((pmd, "param"), (trm, "traj"), (i32[0], "traj_len"), (cm, "cost"),
+                                            (i32[1], "status"), (i32[2], "iters")))
+    assert ok, "MPTG GPU result is not bit-identical to the checker"
+    print(f"smoke MPTG  n={nm}: bit-identical to the checker; "
+          f"{int((i32[1] == 0).sum().item())}/{nm} converged")
     print(f"smoke ok: {eng.launches} kernel launches through libcrb.so")
     eng.close()

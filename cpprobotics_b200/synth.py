@@ -230,3 +230,35 @@ def dwa_obstacles(k: int, seed: int = 0xC0FFEE) -> np.ndarray:
     h = 7.0 * max(1.0, np.sqrt(k / 10.0))
     ob = np.stack([uniform(seed, 120, idx, 5.0 - h, 5.0 + h), uniform(seed, 121, idx, 5.0 - h, 5.0 + h)], axis=1)
     return np.ascontiguousarray(ob.astype(np.float32))
+
+
+# ---- model-predictive trajectory generation (src/model_predictive_trajectory_generator.cpp) -------------------
+# main()'s start state (:26, CONST_V 3.0), target (:27) and initial parameter (:30)
+MPTG_DEMO_STATE = (0.0, 0.0, 0.0, 3.0)
+MPTG_DEMO_TARGET = (5.0, 2.0, 0.0)
+MPTG_DEMO_PARAM = (6.0, 0.0, 0.0, 0.0)
+
+
+def mptg_inputs(n: int, seed: int = 0xC0FFEE, i0: int = 0):
+    """state [4,n] (x, y, yaw, v), target [3,n] (x, y, yaw), param [4,n] (distance, steering_sequence[0..2]),
+    float32; problem i a function of (seed, i0 + i) only.  Around the demo: start at the origin with v = 3, target
+    x in [3, 8], y in [-3, 3], yaw in [-0.6, 0.6], initial parameter (hypot(x, y) + 1, {0, 0, 0}).  One problem in
+    64 is a corner case, by index: distance -1 (an empty roll-out), steering[0] = 150 (tanf outside the exact
+    range), distance 2000 (more than CRB_MPTG_MAX_STEPS steps), start yaw 200 (sinf / cosf outside the exact
+    range), a target behind the start (rarely converges)."""
+    idx = np.arange(i0, i0 + n, dtype=np.uint64)
+    state = np.zeros((4, n), np.float32)
+    state[3] = 3.0
+    target = np.empty((3, n), np.float32)
+    target[0] = uniform(seed, 130, idx, 3.0, 8.0)
+    target[1] = uniform(seed, 131, idx, -3.0, 3.0)
+    target[2] = uniform(seed, 132, idx, -0.6, 0.6)
+    param = np.zeros((4, n), np.float32)
+    param[0] = np.hypot(target[0].astype(np.float64), target[1].astype(np.float64)) + 1.0
+    corner = idx % np.uint64(64)
+    param[0] = np.where(corner == 1, np.float32(-1.0), param[0])
+    param[1] = np.where(corner == 2, np.float32(150.0), param[1])
+    param[0] = np.where(corner == 3, np.float32(2000.0), param[0])
+    state[2] = np.where(corner == 4, np.float32(200.0), state[2])
+    target[0] = np.where(corner == 5, np.float32(-4.0), target[0])
+    return np.ascontiguousarray(state), np.ascontiguousarray(target), np.ascontiguousarray(param)

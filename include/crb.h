@@ -20,6 +20,10 @@
  *   crb_dwa_control_batched             <- dwa_control()         src/dynamic_window_approach.cpp:148-155
  *                                         (calc_dynamic_window :52-60, calc_final_input :115-145 and the costs)
  *   crb_dwa_motion_batched              <- motion()              src/dynamic_window_approach.cpp:43-50
+ *   crb_mptg_optimize_batched           <- TrajectoryOptimizer::optimizer_traj()  include/trajectory_optimizer.h:53-200
+ *                                         (MotionModel::generate_last_state, quadratic_interpolation,
+ *                                          update of include/motion_model.h:59-150)
+ *   crb_mptg_generate_trajectory_batched <- MotionModel::generate_trajectory()  include/motion_model.h:110-131
  *   crb_stats_*                         <- (no reference counterpart) per-GPU summary statistics, the
  *                                          only thing that ever crosses NVLink (one all-gather).
  *
@@ -343,6 +347,74 @@ int crb_dwa_control_batched(crb_ctx* ctx, int64_t n, const float* x, float* u, c
 /* x [5][n] in/out, u [2][n] (DEVICE; NULL allowed when n = 0).  dt finite and > 0.
  * Replaces: motion(x, u, dt) :43-50, the plant step of main() :194. */
 int crb_dwa_motion_batched(crb_ctx* ctx, int64_t n, float* x, const float* u, float dt);
+
+/* ---- model-predictive trajectory generation (include/trajectory_optimizer.h, include/motion_model.h) ---- */
+/* Shared by the batch: MotionModel's base_l and ds, and optimizer_traj's max_iter, cost_th and h_step. */
+typedef struct crb_mptg_params {
+  float base_l, ds;
+  int32_t max_iter;
+  float cost_th;
+  float h_step[3];
+} crb_mptg_params;
+/* The demo's values (src/model_predictive_trajectory_generator.cpp:19-33): base_l 1.0, ds 0.1, max_iter 100,
+ * cost_th 0.1f, h_step {0.2f, 0.005f, 0.005f}. */
+void crb_mptg_default_params(crb_mptg_params* p);
+
+/* Limits: every float parameter finite, ds > 0, base_l != 0, h_step[k] > 0, 0 <= max_iter <= CRB_MPTG_MAX_ITER,
+ * max_pts >= 0; otherwise CRB_ERR_INVALID_ARG.  A roll-out (the `for (float i = 0; i < horizon; i += horizon/n)`
+ * loop, :124, :145) may take at most CRB_MPTG_MAX_STEPS steps. */
+#define CRB_MPTG_MAX_ITER 1000
+#define CRB_MPTG_MAX_STEPS 16384
+
+/* Per-problem status.  The reference has no status; the last three mark problems it does not define or whose
+ * bits this library cannot reproduce, and such a problem stops there instead of returning a different answer.
+ *   CRB_MPTG_CONVERGED          cost < cost_th (:110); for generate_trajectory: the roll-out completed
+ *   CRB_MPTG_MAX_ITER_REACHED   max_iter updates made without converging (:63, :127)
+ *   CRB_MPTG_EMPTY_TRAJ         the nominal roll-out of an iteration has no step (distance <= 0, v < 0, a NaN
+ *                               parameter): the reference reads sample_traj.back() of an empty vector (:105)
+ *   CRB_MPTG_STEP_CAP           a roll-out needs more than CRB_MPTG_MAX_STEPS steps (the reference's loop stalls
+ *                               at i + dt == i, or runs for very long)
+ *   CRB_MPTG_OUT_OF_RANGE       a roll-out needs tanf of a finite steering with |kp| >= 120, or starts from a yaw
+ *                               that is not in (-120, 120): outside the range where this library's tanf / sinf /
+ *                               cosf are proven equal to glibc's */
+#define CRB_MPTG_CONVERGED 0
+#define CRB_MPTG_MAX_ITER_REACHED 1
+#define CRB_MPTG_EMPTY_TRAJ 2
+#define CRB_MPTG_STEP_CAP 3
+#define CRB_MPTG_OUT_OF_RANGE 4
+
+/* optimizer_traj(max_iter, cost_th, h_step) :53-128 for n independent problems.
+ *   state [4][n] (x, y, yaw, v), target [3][n] (x, y, yaw)
+ *   param [4][n] in/out (distance, steering_sequence[0..2]); steering_sequence[0] is never changed (:121-123)
+ *   optional outputs, NULL = not written:
+ *     traj [3*max_pts][n]  field 3k+j = component j (x, y, yaw) of point k of the returned Traj; only the first
+ *                          min(traj_len, max_pts) points are written, the rest of the array is left as it is
+ *     traj_len [n]         int32: the returned Traj's full size (also when it exceeds max_pts)
+ *     cost [n]             the cost of the returned Traj's last point (:108-109)
+ *     status [n], iters [n] int32: CRB_MPTG_* and the number of parameter updates made (:121-124)
+ *   On each status:
+ *     CONVERGED       param as returned; traj / traj_len / cost of the trajectory that converged
+ *     MAX_ITER_REACHED param after the last update; traj / traj_len / cost of the roll-out made at the START of
+ *                     the last iteration, i.e. of the parameter before that update (the reference's quirk); with
+ *                     max_iter = 0 traj_len = 0, cost = NaN and param is unchanged
+ *     EMPTY_TRAJ, STEP_CAP, OUT_OF_RANGE
+ *                     param and iters as they stood when the problem stopped, traj_len = 0, cost = NaN
+ * All DEVICE pointers (state, target, param may be NULL when n = 0: a no-op).  Bit-exact with the reference
+ * built for x86-64 with glibc 2.39: float arithmetic without contraction, the std::pow / std::sqrt of the cost
+ * and YAW_P2P in double, Eigen's 3x3 cofactor inverse (DESIGN.md), glibc's tanf / sinf / cosf, and the line
+ * search's `cost <= mincost` rule (a tie goes to alpha 1.5, a NaN or +inf cost never wins).  Only enqueues on
+ * the context's stream (capturable in a CUDA graph). */
+int crb_mptg_optimize_batched(crb_ctx* ctx, int64_t n, const float* state, const float* target, float* param,
+                              const crb_mptg_params* prm, int max_pts, float* traj, int32_t* traj_len,
+                              float* cost, int32_t* status, int32_t* iters);
+/* MotionModel::generate_trajectory(p) :110-131 (only prm->base_l and prm->ds are used, all are validated).
+ *   state [4][n], param [4][n] in; optional outputs traj [3*max_pts][n] and traj_len [n] as above, last [3][n] =
+ *   generate_last_state(p) :133-150 (the start's x, y, yaw for an empty roll-out), status [n].
+ *   status CONVERGED (the roll-out completed), STEP_CAP or OUT_OF_RANGE; on the last two traj_len = 0 and
+ *   last = NaN.  DEVICE pointers, NULL allowed when n = 0. */
+int crb_mptg_generate_trajectory_batched(crb_ctx* ctx, int64_t n, const float* state, const float* param,
+                                         const crb_mptg_params* prm, int max_pts, float* traj,
+                                         int32_t* traj_len, float* last, int32_t* status);
 
 /* ---- multi-GPU: communicator owned by the context (NCCL, opened at run time) ---------------------- */
 /* The batch shards over GPUs by contiguous agent ranges (one crb_ctx per device, one host thread or process

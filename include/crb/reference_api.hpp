@@ -10,6 +10,7 @@
 //   resampling(px, pw, gen, uni_d)                src/particle_filter.cpp:120-148
 //   solve_DARE / dlqr (4x4 and 5x5)               src/lqr_steer_control.cpp:75-96, lqr_speed_steer_control.cpp:85-106
 //   dwa_control(x, u, config, goal, ob), motion(x, u, dt)   src/dynamic_window_approach.cpp:148-155, :43-50
+//   MotionModel, TrajectoryOptimizer::optimizer_traj(...)    include/motion_model.h, include/trajectory_optimizer.h
 //
 // Eigen is not a dependency: crb::Mat<R,C> is a POD with the memory layout of
 // Eigen::Matrix<float,R,C> (column-major, contiguous, no padding), enough of its interface for the
@@ -380,5 +381,138 @@ inline std::array<float, 5> motion(std::array<float, 5> x, std::array<float, 2> 
   crb::check(crb_memcpy_d2h(ctx, x.data(), dx, 5 * sizeof(float)), "d2h");
   return x;
 }
+
+// include/motion_model.h:22-92 and include/trajectory_optimizer.h:32-51: the same types, members and constructors.
+// MotionModel's trajectories and TrajectoryOptimizer::optimizer_traj run through the batched entry points with
+// n = 1.  The optimizer's drawing (visualize, save) and its console message on convergence are not reproduced.
+namespace cpprobotics {
+struct Parameter {
+  float distance;
+  std::array<float, 3> steering_sequence{{0, 0, 0}};
+  Parameter(float distance_, std::array<float, 3> steering_sequence_)
+      : distance(distance_), steering_sequence(steering_sequence_) {}
+};
+struct TrajState {
+  float x;
+  float y;
+  float yaw;
+  TrajState(float x_, float y_, float yaw_) : x(x_), y(y_), yaw(yaw_) {}
+};
+using Traj = std::vector<TrajState>;
+
+namespace detail {
+// state [4] | target [3] | param [4] | len, status, iters | last [3] | traj [3 max_pts]  (n = 1: SoA is AoS)
+inline float* mptg_scratch(int max_pts) { return crb::Session::scratch(17 + 3 * (size_t)max_pts); }
+inline Traj mptg_read_traj(crb_ctx* ctx, const float* dtraj, int len) {
+  std::vector<float> buf(3 * (size_t)len);
+  if (len) crb::check(crb_memcpy_d2h(ctx, buf.data(), dtraj, buf.size() * sizeof(float)), "d2h");
+  Traj t;
+  t.reserve((size_t)len);
+  for (int k = 0; k < len; ++k) t.push_back(TrajState(buf[3 * k], buf[3 * k + 1], buf[3 * k + 2]));
+  return t;
+}
+}  // namespace detail
+
+class MotionModel {
+ public:
+  const float base_l;
+  const float ds;
+  State state;
+  MotionModel(float base_l_, float ds_, State state_) : base_l(base_l_), ds(ds_), state(state_) {}
+  // generate_trajectory :110-131
+  Traj generate_trajectory(Parameter p) const {
+    int len = 0;
+    float last[3];
+    return run(p, 256, &len, last, true);
+  }
+  // generate_last_state :133-150
+  TrajState generate_last_state(Parameter p) const {
+    int len = 0;
+    float last[3];
+    run(p, 0, &len, last, false);
+    return TrajState(last[0], last[1], last[2]);
+  }
+  crb_mptg_params params() const {
+    crb_mptg_params prm;
+    crb_mptg_default_params(&prm);
+    prm.base_l = base_l;
+    prm.ds = ds;
+    return prm;
+  }
+
+ private:
+  Traj run(const Parameter& p, int max_pts, int* len, float* last, bool want_traj) const {
+    crb_ctx* ctx = crb::Session::get();
+    const crb_mptg_params prm = params();
+    for (;;) {
+      float* d = detail::mptg_scratch(max_pts);
+      const float st[4] = {state.x, state.y, state.yaw, state.v};
+      const float q[4] = {p.distance, p.steering_sequence[0], p.steering_sequence[1], p.steering_sequence[2]};
+      crb::check(crb_memcpy_h2d(ctx, d, st, sizeof(st)), "h2d");
+      crb::check(crb_memcpy_h2d(ctx, d + 7, q, sizeof(q)), "h2d");
+      crb::check(crb_mptg_generate_trajectory_batched(ctx, 1, d, d + 7, &prm, max_pts, want_traj ? d + 17 : nullptr,
+                                                      (int32_t*)(d + 11), d + 14, (int32_t*)(d + 12)),
+                 "crb_mptg_generate_trajectory_batched");
+      int32_t ls[2];
+      crb::check(crb_memcpy_d2h(ctx, ls, d + 11, sizeof(ls)), "d2h");
+      crb::check(crb_memcpy_d2h(ctx, last, d + 14, 3 * sizeof(float)), "d2h");
+      if (ls[1] != CRB_MPTG_CONVERGED)
+        throw std::runtime_error("generate_trajectory: the roll-out stopped with status " + std::to_string(ls[1]));
+      *len = ls[0];
+      if (!want_traj) return Traj();
+      if (ls[0] <= max_pts) return detail::mptg_read_traj(ctx, d + 17, ls[0]);
+      max_pts = ls[0];
+    }
+  }
+};
+
+class TrajectoryOptimizer {
+ public:
+  MotionModel m_model;
+  Parameter p;
+  TrajState target;
+  TrajectoryOptimizer(MotionModel m_model_, Parameter init_p_, TrajState target_)
+      : m_model(m_model_), p(init_p_), target(target_) {}
+  // optimizer_traj :53-128: updates p and returns the last nominal trajectory.  A problem the reference leaves
+  // undefined, or that is outside the exact range of the restated libm (crb.h, CRB_MPTG_*), throws.
+  Traj optimizer_traj(int max_iter, float cost_th, std::vector<float> h_step, bool visualize = false,
+                      bool save = false) {
+    (void)visualize;
+    (void)save;
+    if (h_step.size() < 3) throw std::runtime_error("optimizer_traj: h_step needs 3 entries");
+    crb_ctx* ctx = crb::Session::get();
+    crb_mptg_params prm = m_model.params();
+    prm.max_iter = max_iter;
+    prm.cost_th = cost_th;
+    for (int k = 0; k < 3; ++k) prm.h_step[k] = h_step[k];
+    int max_pts = 256;
+    for (;;) {
+      float* d = detail::mptg_scratch(max_pts);
+      const float st[4] = {m_model.state.x, m_model.state.y, m_model.state.yaw, m_model.state.v};
+      const float tg[3] = {target.x, target.y, target.yaw};
+      const float q[4] = {p.distance, p.steering_sequence[0], p.steering_sequence[1], p.steering_sequence[2]};
+      crb::check(crb_memcpy_h2d(ctx, d, st, sizeof(st)), "h2d");
+      crb::check(crb_memcpy_h2d(ctx, d + 4, tg, sizeof(tg)), "h2d");
+      crb::check(crb_memcpy_h2d(ctx, d + 7, q, sizeof(q)), "h2d");
+      crb::check(crb_mptg_optimize_batched(ctx, 1, d, d + 4, d + 7, &prm, max_pts, d + 17, (int32_t*)(d + 11),
+                                           nullptr, (int32_t*)(d + 12), (int32_t*)(d + 13)),
+                 "crb_mptg_optimize_batched");
+      int32_t ls[2];
+      crb::check(crb_memcpy_d2h(ctx, ls, d + 11, sizeof(ls)), "d2h");
+      if (ls[1] != CRB_MPTG_CONVERGED && ls[1] != CRB_MPTG_MAX_ITER_REACHED)
+        throw std::runtime_error("optimizer_traj: stopped with status " + std::to_string(ls[1]));
+      if (ls[0] > max_pts) {  // the same problem again with room for the whole trajectory
+        max_pts = ls[0];
+        continue;
+      }
+      float qo[4];
+      crb::check(crb_memcpy_d2h(ctx, qo, d + 7, sizeof(qo)), "d2h");
+      p.distance = qo[0];
+      for (int k = 0; k < 3; ++k) p.steering_sequence[k] = qo[k + 1];
+      return detail::mptg_read_traj(ctx, d + 17, ls[0]);
+    }
+  }
+};
+}  // namespace cpprobotics
 
 #endif  // CRB_REFERENCE_API_HPP_
