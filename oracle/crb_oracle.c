@@ -342,6 +342,71 @@ int64_t crb_oracle_check_ff_product(double pre, uint32_t lo_bits, uint32_t hi_bi
   return bad;
 }
 
+/* (c) resampleid = (float)((double)(float)(j / NP) + U / NP) (:131-133) as crb_pf_gather2_kernel computes it
+ *     (pf_resample_id_rcp): both quotients as q = a r, q += fma(-q, NP, a) r with r = RN(1 / NP).  Counts the
+ *     (j, NP, U) where either double quotient is not the correctly rounded one or the float result differs:
+ *     - every NP in [1, n_max] at j in {0, 1, 2, NP/2, NP-2, NP-1} and 32 hashed j;
+ *     - every j in [0, NP) for each NP of ns[0..n_ns);
+ *     - all 2^23 floats U in [1, 2) (the Philox draws) for each NP of ns, at a hashed j.
+ *     Away from those j the U of a case is hashed too.  *evaluated receives the number of cases. */
+static inline uint64_t splitmix64(uint64_t x) {
+  x += 0x9E3779B97F4A7C15ull;
+  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+  return x ^ (x >> 31);
+}
+static inline float u12_from_bits(uint32_t m) { return 1.0f + (float)(m & 0x7FFFFFu) * 1.1920928955078125e-07f; }
+static inline int resample_id_rcp_bad(int64_t j, int64_t n, float U) {
+  const double n_d = (double)n, inv_n = 1.0 / n_d;
+  const double jd = (double)j;
+  double q = jd * inv_n;
+  q = fma(fma(-q, n_d, jd), inv_n, q);
+  const double ud = (double)U;
+  double t = ud * inv_n;
+  t = fma(fma(-t, n_d, ud), inv_n, t);
+  const float got = (float)((double)(float)q + t);
+  const double q_ref = jd / n_d, t_ref = ud / n_d;
+  const float want = (float)((double)(float)q_ref + t_ref);
+  return q != q_ref || t != t_ref || got != want;
+}
+int64_t crb_oracle_check_resample_id_rcp(int64_t n_max, const int64_t* ns, int n_ns, int64_t* evaluated) {
+  int64_t bad = 0, cnt = 0;
+#ifdef _OPENMP
+#pragma omp parallel for reduction(+ : bad, cnt) schedule(dynamic, 4096)
+#endif
+  for (int64_t n = 1; n <= n_max; ++n) {
+    const int64_t fixed[6] = {0, 1, 2, n / 2, n - 2, n - 1};
+    for (int k = 0; k < 6 + 32; ++k) {
+      const uint64_t h = splitmix64(((uint64_t)n << 6) | (uint64_t)k);
+      const int64_t j = k < 6 ? fixed[k] : (int64_t)(h % (uint64_t)n);
+      if (j < 0 || j >= n) continue;
+      bad += resample_id_rcp_bad(j, n, u12_from_bits((uint32_t)(h >> 32)));
+      ++cnt;
+    }
+  }
+  for (int s = 0; s < n_ns; ++s) {
+    const int64_t n = ns[s];
+#ifdef _OPENMP
+#pragma omp parallel for reduction(+ : bad, cnt) schedule(static)
+#endif
+    for (int64_t j = 0; j < n; ++j) {
+      const uint64_t h = splitmix64((uint64_t)j ^ ((uint64_t)n << 32));
+      bad += resample_id_rcp_bad(j, n, u12_from_bits((uint32_t)h));
+      ++cnt;
+    }
+#ifdef _OPENMP
+#pragma omp parallel for reduction(+ : bad, cnt) schedule(static)
+#endif
+    for (int64_t m = 0; m < ((int64_t)1 << 23); ++m) {
+      const int64_t j = (int64_t)(splitmix64((uint64_t)m + ((uint64_t)n << 24)) % (uint64_t)n);
+      bad += resample_id_rcp_bad(j, n, u12_from_bits((uint32_t)m));
+      ++cnt;
+    }
+  }
+  if (evaluated) *evaluated = cnt;
+  return bad;
+}
+
 /* raw Philox4x32-10 block (for the known-answer vectors of the Random123 distribution) */
 void crb_oracle_philox4x32(const uint32_t ctr[4], const uint32_t key[2], uint32_t out[4]) {
   uint32_t c[4] = {ctr[0], ctr[1], ctr[2], ctr[3]};

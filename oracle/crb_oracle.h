@@ -72,6 +72,7 @@ int crb_oracle_num_threads(void);
 /* verification aids for arithmetic shortcuts of the CUDA PF kernel (see crb_oracle.c) */
 int64_t crb_oracle_check_const_division(float d, uint32_t lo_bits, uint32_t hi_bits);
 int64_t crb_oracle_check_ff_product(double pre, uint32_t lo_bits, uint32_t hi_bits);
+int64_t crb_oracle_check_resample_id_rcp(int64_t n_max, const int64_t* ns, int n_ns, int64_t* evaluated);
 
 /* glibc's sinf / cosf restated (binary64 polynomial, what the kernels' crb_sincosf_libm executes) */
 void crb_oracle_libm_sincosf(float y, float* sn, float* cs);

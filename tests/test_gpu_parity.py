@@ -819,7 +819,20 @@ def test_pf_step_is_the_composition_of_the_reference_stages(engine, n):
     assert np.array_equal(pxd3.cpu().numpy(), px2)
 
 
-def _pf_shard_worker(rank, world, port, n, q):
+def _pf_inputs_at(n, centre):
+    """synth.pf_inputs and its landmarks; with a centre, moved rigidly there and shrunk to a 5 cm cloud."""
+    px, pw, noise = synth.pf_inputs(n)
+    lm = synth.pf_landmarks(8)
+    if centre is not None:
+        lm = lm.astype(np.float64)
+        for f in (0, 1):
+            px[f] = (centre[f] + (px[f].astype(np.float64) - synth.PF_TRUTH[f]) * 0.25).astype(np.float32)
+            lm[:, 1 + f] += centre[f] - synth.PF_TRUTH[f]
+        lm = lm.astype(np.float32)
+    return px, pw, noise, lm
+
+
+def _pf_shard_worker(rank, world, port, n, q, centre=None):
     import torch
     import torch.distributed as dist
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
@@ -832,8 +845,7 @@ def _pf_shard_worker(rank, world, port, n, q):
         buf.copy_(torch.frombuffer(bytearray(eng.comm_unique_id()), dtype=torch.uint8))
     dist.broadcast(buf, 0)
     eng.comm_init(world, rank, bytes(buf.cpu().numpy().tobytes()))
-    px, pw, noise = synth.pf_inputs(n)
-    lm = synth.pf_landmarks(8)
+    px, pw, noise, lm = _pf_inputs_at(n, centre)
     k = n // world
     sl = slice(rank * k, (rank + 1) * k)
     pxd, pwd, nd = (torch.from_numpy(np.ascontiguousarray(a[..., sl])).cuda() for a in (px, pw, noise))
@@ -881,3 +893,37 @@ def test_pf_sharded_over_two_gpus_equals_the_single_gpu_estimate(engine):
         np.testing.assert_allclose(res[20], want[20], rtol=1e-9)
         k = n // world
         np.testing.assert_allclose(w, want_w[rank * k:(rank + 1) * k], rtol=1e-6, atol=0)
+
+
+@pytest.mark.gpu
+def test_pf_sharded_covariance_far_from_the_origin(engine):
+    """The sharded moments are centred on rank 0's particle 0, broadcast to every rank: a 5 cm cloud 10^5 m from the
+    origin keeps PEst at float accuracy, entry by entry within 1e-6 sqrt(P_rr P_cc) of the float64 two-pass
+    covariance around the single-GPU xEst, and xEst within one float ulp of the single-GPU one."""
+    import socket
+    import torch
+    import torch.multiprocessing as mp
+    n, world, centre = 400_000, min(2, torch.cuda.device_count()), (1e5, 1e5)
+    px, pw, noise, lm = _pf_inputs_at(n, centre)
+    pxd, pwd, nd = _dev(px, pw, noise)
+    nxt = torch.empty_like(pxd)
+    want = engine.pf_step(pxd, pwd, nxt, nd, lm, nth=0.0).cpu().numpy()
+    gx = pxd.cpu().numpy()
+    s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
+    ctx = mp.get_context("spawn")
+    q = ctx.Queue()
+    procs = [ctx.Process(target=_pf_shard_worker, args=(r, world, port, n, q, centre)) for r in range(world)]
+    for p in procs:
+        p.start()
+    got = sorted([q.get(timeout=240) for _ in range(world)], key=lambda t: t[0])
+    for p in procs:
+        p.join(timeout=60)
+    gw = np.concatenate([w for _, _, w in got]).astype(np.float64)   # the globally normalised weights
+    for rank, res, w in got:
+        assert (np.abs(res[0:4] - want[0:4]) <= np.spacing(np.abs(want[0:4]).astype(np.float32))).all()
+        d = (gx - res[0:4].astype(np.float32)[:, None]).astype(np.float64)   # around this rank's xEst
+        C = (d * gw) @ d.T
+        P = res[4:20].reshape(4, 4).T
+        assert np.array_equal(P, P.T)
+        err = np.abs(P - C) / np.sqrt(np.outer(np.diag(C), np.diag(C)))
+        assert err.max() <= 1e-6, err.max()

@@ -101,6 +101,21 @@ def test_kernel_arithmetic_identities():
     assert L.crb_oracle_check_ff_product(pre, bits(1e-30), bits(1.0)) == 0
 
 
+def test_resample_id_reciprocal_is_the_correctly_rounded_quotient():
+    """crb_pf_step's gather computes resampleid = (float)(base(j) + U / NP), base(j) = (float)(j / NP), with both
+    double quotients as Markstein sequences around r = RN(1 / NP) instead of divisions.  Census: every NP <= 2^21 at
+    the edge j and 32 hashed j, every j for five NP, and every Philox U in [1, 2) for those NP - the quotients and the
+    float result must be the correctly rounded ones, without exception."""
+    L = O.lib()
+    L.crb_oracle_check_resample_id_rcp.restype = C.c_int64
+    L.crb_oracle_check_resample_id_rcp.argtypes = [C.c_int64, C.POINTER(C.c_int64), C.c_int, C.POINTER(C.c_int64)]
+    ns = (C.c_int64 * 5)(3, 1025, 1_000_000, (1 << 21) - 1, 1 << 21)
+    evaluated = C.c_int64(0)
+    bad = L.crb_oracle_check_resample_id_rcp(1 << 21, ns, len(ns), C.byref(evaluated))
+    assert evaluated.value > 5 * (1 << 23) + (1 << 21) * 38 - 16
+    assert bad == 0
+
+
 def test_estimate_tail_matches_numpy():
     n = 5000
     px, pw, noise = synth.pf_inputs(n)
