@@ -34,7 +34,6 @@ struct crb_ctx {
   int ekf_tma_attr_set;
   int pf_step_attr_set;   // shared-memory carve-out preference of the crb_pf_step kernels (per device)
   int mpc_v0_attr_set;
-  unsigned* tickets;      // 64 zeroed words of device memory: "last block finishes the job" counters (kept at zero)
   // NCCL communicator (crb_comm.cu); NULL = single GPU
   void* comm;
   int comm_world, comm_rank;

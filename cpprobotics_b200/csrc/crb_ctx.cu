@@ -53,8 +53,6 @@ int crb_init(crb_ctx** out, int device_id) {
   for (int i = 0; i < CRB_N_PIPE && err == cudaSuccess; ++i)
     err = cudaStreamCreateWithFlags(&c->pipe_stream[i], cudaStreamNonBlocking);
   if (err == cudaSuccess) err = cudaMallocHost(&c->host_scratch, 4096);
-  if (err == cudaSuccess) err = cudaMalloc(&c->tickets, 64 * sizeof(unsigned));
-  if (err == cudaSuccess) err = cudaMemset(c->tickets, 0, 64 * sizeof(unsigned));
   if (err != cudaSuccess) {
     crb_set_error("crb_init: %s", cudaGetErrorString(err));
     crb_destroy(c);
@@ -84,7 +82,6 @@ int crb_destroy(crb_ctx* ctx) {
   if (ctx->scratch) cudaFree(ctx->scratch);
   if (ctx->mpc_ws) cudaFree(ctx->mpc_ws);
   if (ctx->host_scratch) cudaFreeHost(ctx->host_scratch);
-  if (ctx->tickets) cudaFree(ctx->tickets);
   if (ctx->ev_start) cudaEventDestroy(ctx->ev_start);
   if (ctx->ev_stop) cudaEventDestroy(ctx->ev_stop);
   if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);

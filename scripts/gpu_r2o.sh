@@ -1,19 +1,7 @@
 #!/bin/bash
-# PF four-launch iteration and MPC hinted order: parity subset + A/B timings.
+# MPC hinted order: parity subset + timing.
 OUT=gpurun_out; mkdir -p $OUT
 [ -n "$SKIP_PYTEST" ] || timeout 600 python -m pytest tests/test_gpu_parity.py -x -q -k "pf_step or hinted or pf_sharded or resample" > $OUT/o_pytest.log 2>&1; echo "pytest rc=$?" >> $OUT/o_pytest.log
-CRB_PF_STEP=1 timeout 300 python bench.py --workload pf --no-cpu --steps 20 --warmup 5 > $OUT/o_pf1.json 2> $OUT/o_pf1.err
-CRB_PF_STEP=2 timeout 300 python bench.py --workload pf --no-cpu --steps 20 --warmup 5 > $OUT/o_pf2.json 2> $OUT/o_pf2.err
-CRB_PF_STEP=2 CRB_PDL=0 timeout 300 python bench.py --workload pf --no-cpu --steps 20 --warmup 5 > $OUT/o_pf2_nopdl.json 2> $OUT/o_pf2_nopdl.err
 timeout 400 python bench.py --workload mpc --no-cpu --steps 20 --warmup 5 > $OUT/o_mpc.json 2> $OUT/o_mpc.err
 tail -4 $OUT/o_pytest.log
-for f in o_pf1 o_pf2 o_pf2_nopdl; do python - <<PY
-import json
-try:
-    d=json.loads([l for l in open("$OUT/$f.json") if l.startswith('{')][-1])
-    print("$f", "PF iter ms", d["extra"]["pf_full_iteration"]["ms_per_step"], "pf frac", d["roofline"]["pf"]["frac"])
-except Exception as e:
-    print("$f failed", e); print(open("$OUT/$f.err").read()[-1500:])
-PY
-done
 python scripts/show_bench.py $OUT/o_mpc.json 2>&1 | grep "MPC" || tail -20 $OUT/o_mpc.err

@@ -1,19 +1,7 @@
 #!/bin/bash
-# MPC hinted order with one bin for the short problems + marginal in-graph cost of the PF iteration kernels.
+# MPC hinted order with one bin for the short problems.
 OUT=gpurun_out; mkdir -p $OUT
 timeout 600 python -m pytest tests/test_gpu_parity.py -x -q -k "hinted" > $OUT/q_pytest.log 2>&1; echo "pytest rc=$?" >> $OUT/q_pytest.log
 timeout 400 python bench.py --workload mpc --no-cpu --steps 20 --warmup 5 > $OUT/q_mpc.json 2> $OUT/q_mpc.err
-for sk in 0 1 2 4 6 7; do
-  CRB_PF_SKIP=$sk timeout 300 python bench.py --workload pf --no-cpu --steps 10 --warmup 3 > $OUT/q_pf_skip$sk.json 2> $OUT/q_pf_skip$sk.err
-done
 tail -3 $OUT/q_pytest.log
 python scripts/show_bench.py $OUT/q_mpc.json 2>&1 | grep "MPC" || tail -20 $OUT/q_mpc.err
-for sk in 0 1 2 4 6 7; do python - <<PY
-import json
-try:
-    d=json.loads([l for l in open("$OUT/q_pf_skip$sk.json") if l.startswith('{')][-1])
-    print("skip $sk", "PF iter us", 1e3*d["extra"]["pf_full_iteration"]["ms_per_step"])
-except Exception as e:
-    print("skip $sk failed", e); print(open("$OUT/q_pf_skip$sk.err").read()[-800:])
-PY
-done

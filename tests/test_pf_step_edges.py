@@ -353,8 +353,8 @@ def test_pf_step_closed_loop_ping_pong(engine, n):
 
 @pytest.mark.gpu
 def test_pf_step_results_do_not_depend_on_earlier_calls(engine):
-    """The scratch space grows and shrinks between forms, and the seven-launch form's ticket counters must be back
-    at zero after every call: 2^21+1, 1025, 2^21+1 on one context equal fresh contexts bit for bit."""
+    """The scratch space grows and shrinks between forms and is reused without being cleared, so nothing one call
+    leaves in it may reach the next: 2^21+1, 1025, 2^21+1 on one context equal fresh contexts bit for bit."""
     import torch
 
     def run(eng, n):
