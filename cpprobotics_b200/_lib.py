@@ -30,6 +30,15 @@ CRB_MPTG_MAX_ITER_REACHED = 1
 CRB_MPTG_EMPTY_TRAJ = 2
 CRB_MPTG_STEP_CAP = 3
 CRB_MPTG_OUT_OF_RANGE = 4
+CRB_SLP_UNIFORM = 0
+CRB_SLP_BIASED = 1
+CRB_SLP_LANE = 2
+CRB_SLP_MAX_NXY = 4096
+CRB_SLP_MAX_NH = 1024
+CRB_SLP_MAX_NS = 1 << 20
+CRB_SLP_MAX_STATES = 65536
+CRB_SLP_OK = 0
+CRB_SLP_OUT_OF_RANGE = 1
 
 c_f32p = C.POINTER(C.c_float)
 c_i32p = C.POINTER(C.c_int32)
@@ -63,6 +72,10 @@ class DwaParams(C.Structure):
 class MptgParams(C.Structure):
     _fields_ = [("base_l", C.c_float), ("ds", C.c_float), ("max_iter", C.c_int32), ("cost_th", C.c_float),
                 ("h_step", C.c_float * 3)]
+
+
+class SlpSampler(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("nxy", C.c_int32), ("nh", C.c_int32), ("ns", C.c_int32), ("d", C.c_int32)]
 
 
 # name -> (restype, argtypes); every symbol include/crb.h declares
@@ -140,6 +153,12 @@ PROTOTYPES = {
     "crb_mptg_generate_trajectory_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                                        C.POINTER(MptgParams), C.c_int, C.c_void_p, C.c_void_p,
                                                        C.c_void_p, C.c_void_p]),
+    "crb_slp_default_params": (None, [C.POINTER(MptgParams), C.POINTER(C.c_float)]),
+    "crb_slp_states_per_query": (C.c_int, [C.POINTER(SlpSampler)]),
+    "crb_slp_sample_states_batched": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(SlpSampler), C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.c_void_p]),
+    "crb_slp_search_nearest_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int,
+                                                 C.c_void_p, C.c_void_p, C.c_void_p]),
     "crb_stats_reduce": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p]),
     "crb_probe_fp32_peak": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),

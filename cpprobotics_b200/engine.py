@@ -12,6 +12,10 @@ Method names follow the reference functions they replace:
   Engine.dwa_motion          <- motion()                src/dynamic_window_approach.cpp:43-50
   Engine.mptg_optimize       <- TrajectoryOptimizer::optimizer_traj()  include/trajectory_optimizer.h:53-128
   Engine.mptg_generate_trajectory <- MotionModel::generate_trajectory() include/motion_model.h:110-131
+  Engine.slp_sample_states   <- calc_{uniform_polar,biased_polar,lane}_states()  src/state_lattice_planner.cpp:29-113
+  Engine.slp_search_nearest  <- search_nearest_one_from_lookuptable()            src/state_lattice_planner.cpp:115-135
+  Engine.slp_generate_path   <- generate_path()                                  src/state_lattice_planner.cpp:137-155
+  slp_load_table             <- main()'s CSVIterator + std::stod reading         src/state_lattice_planner.cpp:214-226
 
 All arrays are SoA field-major float32 (`[fields, n]`, C-contiguous); see include/crb.h.  Methods
 without a suffix take CUDA tensors (torch is only the device allocator / stream owner); `*_host`
@@ -63,6 +67,55 @@ def mptg_default_params() -> MptgParams:
     p = MptgParams()
     load_library().crb_mptg_default_params(C.byref(p))
     return p
+
+
+def slp_default_params():
+    """The state lattice planner's optimizer settings and start speed (src/state_lattice_planner.cpp:22-24,
+    :146-148): (MptgParams, CONST_V)."""
+    p, v = MptgParams(), C.c_float(0.0)
+    load_library().crb_slp_default_params(C.byref(p), C.byref(v))
+    return p, float(v.value)
+
+
+_libc = None
+
+
+def _strtod(s: str) -> float:
+    """std::stod: C's strtod on the field (leading blanks skipped, the longest valid prefix parsed); ValueError where
+    stod throws (nothing parsed, or ERANGE)."""
+    global _libc
+    if _libc is None:
+        _libc = C.CDLL(None, use_errno=True)
+        _libc.strtod.restype = C.c_double
+        _libc.strtod.argtypes = [C.c_char_p, C.POINTER(C.c_char_p)]
+    b = s.encode()
+    buf = C.create_string_buffer(b)
+    end = C.c_char_p()
+    C.set_errno(0)
+    v = _libc.strtod(buf, C.byref(end))
+    if C.cast(end, C.c_void_p).value == C.addressof(buf):
+        raise ValueError(f"stod: no conversion of {s!r}")
+    if C.get_errno() == 34:  # ERANGE
+        raise ValueError(f"stod: {s!r} is out of range")
+    return v
+
+
+def slp_load_table(path) -> np.ndarray:
+    """Reads a lookup table the way the reference's main() does (src/state_lattice_planner.cpp:214-226): CSV rows
+    split at ',', the first row (the header) skipped, the first 6 fields of each row parsed with std::stod and
+    narrowed to float.  Returns float32 [rows, 6] (x, y, yaw, s, km, kf).  A row with fewer than 6 fields, or a field
+    stod refuses, raises ValueError."""
+    rows = []
+    with open(path, "rb") as fh:
+        lines = fh.read().decode().split("\n")
+    if lines and lines[-1] == "":
+        lines.pop()   # the newline that ends the last row starts no row
+    for k, line in enumerate(lines[1:], start=2):
+        cells = line.split(",")
+        if len(cells) < 6:
+            raise ValueError(f"{path}:{k}: {len(cells)} fields, 6 needed")
+        rows.append([_strtod(c) for c in cells[:6]])
+    return np.asarray(rows, np.float64).reshape(-1, 6).astype(np.float32)
 
 
 def _ptr(a, dtype, *, device: Optional[bool], name: str) -> int:
@@ -430,6 +483,88 @@ class Engine:
         if traj.dim() != 2 or int(traj.shape[0]) % 3 or int(traj.shape[1]) != n:
             raise ValueError(f"traj: expected shape (3*max_pts, {n}), got {tuple(traj.shape)}")
         return int(traj.shape[0]) // 3
+
+    # ---- state lattice planner ----------------------------------------------------------------------------
+    @staticmethod
+    def slp_default_params():
+        """(MptgParams, CONST_V): the optimizer settings and start speed generate_path uses."""
+        return slp_default_params()
+
+    @staticmethod
+    def slp_load_table(path) -> np.ndarray:
+        """lookuptable.csv read the reference's way: float32 [rows, 6] on the host (see slp_load_table)."""
+        return slp_load_table(path)
+
+    def slp_states_per_query(self, sampler) -> int:
+        """S, the output slots per query of a crb_slp_sampler (SlpSampler)."""
+        s = self.lib.crb_slp_states_per_query(C.byref(sampler))
+        if s < 0:
+            check(s, "crb_slp_states_per_query")
+        return int(s)
+
+    def slp_sample_states(self, sampler, qp, target=None, n_states=None, status=None):
+        """The terminal-state samplers for n_q queries: sampler a SlpSampler (kind, nxy, nh, ns, d shared by the batch),
+        qp [F,n_q] per-query floats (UNIFORM F = 4: a_min, a_max, p_min, p_max; BIASED F = 5: goal_angle and the same
+        four; LANE F = 5: l_center, l_heading, l_width, v_width, d).  Returns (target [3, n_q*S], state j of query q in
+        column q*S + j, NaN past n_states[q]; n_states [n_q] int32; status [n_q] int32, CRB_SLP_*), allocating what is
+        not given.  CUDA tensors; only enqueues."""
+        n = int(qp.shape[-1])
+        S = self.slp_states_per_query(sampler)
+        _shape(qp, 4 if sampler.kind == _lib.CRB_SLP_UNIFORM else 5, n, "qp")
+        if target is None:
+            target = torch.empty((3, n * S), dtype=torch.float32, device=qp.device)
+        if n_states is None:
+            n_states = torch.empty(n, dtype=torch.int32, device=qp.device)
+        if status is None:
+            status = torch.empty(n, dtype=torch.int32, device=qp.device)
+        _shape(target, 3, n * S, "target"); _shape(n_states, 1, n, "n_states"); _shape(status, 1, n, "status")
+        check(self.lib.crb_slp_sample_states_batched(
+            self.ctx, n, C.byref(sampler), _ptr(qp, np.float32, device=True, name="qp"),
+            _ptr(target, np.float32, device=True, name="target"),
+            _ptr(n_states, np.int32, device=True, name="n_states"), _ptr(status, np.int32, device=True, name="status")),
+            "crb_slp_sample_states_batched")
+        return target, n_states, status
+
+    def slp_search_nearest(self, target, table, k0=None, param=None, row=None):
+        """search_nearest_one_from_lookuptable() for n targets: target [3,n], table [rows,6] (lookuptable.csv's
+        columns), k0 [n] or None (0).  Returns (param [4,n] = (|xy|, k0, km, kf) of the nearest row, NaN when none is
+        nearer than FLT_MAX; row [n] int32, -1 then), allocating what is not given.  CUDA tensors; only enqueues."""
+        n = int(target.shape[-1])
+        _shape(target, 3, n, "target")
+        if table.dim() != 2 or int(table.shape[1]) != 6:
+            raise ValueError(f"table: expected shape (rows, 6), got {tuple(table.shape)}")
+        if k0 is not None:
+            _shape(k0, 1, n, "k0")
+        if param is None:
+            param = torch.empty((4, n), dtype=torch.float32, device=target.device)
+        if row is None:
+            row = torch.empty(n, dtype=torch.int32, device=target.device)
+        _shape(param, 4, n, "param"); _shape(row, 1, n, "row")
+        check(self.lib.crb_slp_search_nearest_batched(
+            self.ctx, n, _ptr(target, np.float32, device=True, name="target"),
+            _ptr(table, np.float32, device=True, name="table"), int(table.shape[0]),
+            _ptr(k0, np.float32, device=True, name="k0"), _ptr(param, np.float32, device=True, name="param"),
+            _ptr(row, np.int32, device=True, name="row")), "crb_slp_search_nearest_batched")
+        return param, row
+
+    def slp_generate_path(self, target, table, k0=None, params: Optional[MptgParams] = None, v: Optional[float] = None,
+                          max_pts: int = 0):
+        """generate_path() :137-155 for n terminal states: the lookup-table search, start states (0, 0, 0, v) and
+        optimizer_traj, one launch each.  target [3,n], table [rows,6], k0 [n] or None; params and v default to
+        slp_default_params().  Returns dict(param [4,n] as optimised, traj [3*max_pts,n] (NaN past traj_len, None when
+        max_pts = 0), traj_len, cost, status (CRB_MPTG_*), iters, row).  CUDA tensors; only enqueues."""
+        p0, v0 = slp_default_params()
+        n = int(target.shape[-1])
+        dev = target.device
+        param, row = self.slp_search_nearest(target, table, k0)
+        state = torch.zeros((4, n), dtype=torch.float32, device=dev)
+        state[3] = v0 if v is None else v
+        traj = torch.full((3 * max_pts, n), float("nan"), dtype=torch.float32, device=dev) if max_pts > 0 else None
+        traj_len, status, iters = (torch.empty(n, dtype=torch.int32, device=dev) for _ in range(3))
+        cost = torch.empty(n, dtype=torch.float32, device=dev)
+        self.mptg_optimize(state, target, param, params if params is not None else p0, traj=traj, traj_len=traj_len,
+                           cost=cost, status=status, iters=iters)
+        return dict(param=param, traj=traj, traj_len=traj_len, cost=cost, status=status, iters=iters, row=row)
 
     # ---- multi-GPU: the communicator lives in libcrb (crb_comm.cu), not in torch --------------------
     @staticmethod

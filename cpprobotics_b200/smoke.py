@@ -144,5 +144,21 @@ def run() -> None:
     assert ok, "MPTG GPU result is not bit-identical to the checker"
     print(f"smoke MPTG  n={nm}: bit-identical to the checker; "
           f"{int((i32[1] == 0).sum().item())}/{nm} converged")
+    # SLP: the biased sampler for 33 queries, the search in a synthetic 64-row table and the optimizer, as the checker
+    from oracle import slp as OS  # checker only
+    from ._lib import SlpSampler
+    fs, qs = synth.slp_inputs(33, 1)
+    ss = SlpSampler(fs["kind"], fs["nxy"], fs["nh"], fs["ns"], fs["d"])
+    tbs = synth.slp_table(64)
+    tsd, nsd, std_ = eng.slp_sample_states(ss, torch.from_numpy(qs).to(dev))
+    gs = eng.slp_generate_path(tsd, torch.from_numpy(tbs).to(dev), max_pts=32)
+    torch.cuda.synchronize()
+    os_ = OS.sample(OS.sampler(fs["kind"], fs["nxy"], fs["nh"], fs["ns"], fs["d"]), qs)
+    og = OS.generate_path(os_["target"], tbs, max_pts=32)
+    ok = same_nan(tsd, os_["target"]) and same_nan(nsd, os_["n_states"]) and same_nan(std_, os_["status"])
+    ok = ok and all(same_nan(gs[k], og[k]) for k in ("param", "traj", "traj_len", "cost", "status", "iters", "row"))
+    assert ok, "SLP GPU result is not bit-identical to the checker"
+    print(f"smoke SLP   {qs.shape[1]} queries, {int(nsd.sum().item())} states: bit-identical to the checker; "
+          f"{int((gs['status'] == 0).sum().item())} converged")
     print(f"smoke ok: {eng.launches} kernel launches through libcrb.so")
     eng.close()

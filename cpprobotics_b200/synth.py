@@ -262,3 +262,81 @@ def mptg_inputs(n: int, seed: int = 0xC0FFEE, i0: int = 0):
     state[2] = np.where(corner == 4, np.float32(200.0), state[2])
     target[0] = np.where(corner == 5, np.float32(-4.0), target[0])
     return np.ascontiguousarray(state), np.ascontiguousarray(target), np.ascontiguousarray(param)
+
+
+# src/state_lattice_planner.cpp:157-210: the demo's three scenarios.  Its float constants are double expressions
+# narrowed to float (e.g. -45.0/180 * M_PI); lane_state_sample_test's int d = 10 becomes the float d parameter.
+_DEG = np.pi / 180.0
+SLP_DEMO = {
+    0: dict(nxy=5, nh=3, ns=0, d=20, qp=(-45.0 / 180 * np.pi, 45.0 / 180 * np.pi, -45.0 / 180 * np.pi,
+                                         45.0 / 180 * np.pi)),
+    1: dict(nxy=30, nh=2, ns=100, d=20, qp=(0.0, -45.0 / 180 * np.pi, 45.0 / 180 * np.pi, -20.0 / 180 * np.pi,
+                                            20.0 / 180 * np.pi)),
+    2: dict(nxy=5, nh=1, ns=0, d=0, qp=(10.0, 90.0 / 180.0 * np.pi, 3.0, 1.0, 10.0)),
+}
+
+
+def slp_inputs(n_q: int, kind: int, seed: int = 0xC0FFEE, i0: int = 0):
+    """(sampler fields dict(kind, nxy, nh, ns, d), qp [F, n_q] float32) for the state lattice planner's samplers
+    (kind 0 uniform, 1 biased, 2 lane), the demo's integers; query i a function of (seed, i0 + i) only.  Query 0 is
+    the demo's scenario for that kind; the others are random around it: polar angle ranges a_min in [-1.2, 0],
+    a_max in [0, 1.2], heading ranges p_min in [-0.6, 0], p_max in [0, 0.6], goal_angle in [-1, 1]; lanes with
+    l_center in [-15, 15], l_heading in [-pi, pi], l_width in [1, 6], v_width in [0.5, 2], d in [5, 20].  One query in
+    64 is a corner case, by index:
+      1  an angle outside the exact sinf / cosf range (a_min = -200, a_max = -150; l_heading = 130)
+      2  a zero-width range (a_max = a_min; v_width = l_width)
+      3  a NaN input (p_max; l_center)
+      4  reversed ranges (a_max < a_min, p_max < p_min; negative d); biased: goal_angle 10, so every cnav sample is
+         negative and cnav_max keeps its FLT_MIN start
+      5  inf inputs (a_max = +inf: NaN angles; l_width = inf: NaN offsets)"""
+    idx = np.arange(i0, i0 + n_q, dtype=np.uint64)
+    demo = SLP_DEMO[kind]
+    f = 4 if kind == 0 else 5
+    qp = np.empty((f, n_q), np.float64)
+    corner = idx % np.uint64(64)
+    if kind == 2:
+        qp[0] = uniform(seed, 140, idx, -15.0, 15.0)
+        qp[1] = uniform(seed, 141, idx, -np.pi, np.pi)
+        qp[2] = uniform(seed, 142, idx, 1.0, 6.0)
+        qp[3] = uniform(seed, 143, idx, 0.5, 2.0)
+        qp[4] = uniform(seed, 144, idx, 5.0, 20.0)
+        qp[1] = np.where(corner == 1, 130.0, qp[1])
+        qp[3] = np.where(corner == 2, qp[2], qp[3])
+        qp[0] = np.where(corner == 3, np.nan, qp[0])
+        qp[4] = np.where(corner == 4, -qp[4], qp[4])
+        qp[2] = np.where(corner == 5, np.inf, qp[2])
+    else:
+        o = f - 4
+        if o:
+            qp[0] = uniform(seed, 145, idx, -1.0, 1.0)
+            qp[0] = np.where(corner == 4, 10.0, qp[0])
+        qp[o] = uniform(seed, 146, idx, -1.2, 0.0)
+        qp[o + 1] = uniform(seed, 147, idx, 0.0, 1.2)
+        qp[o + 2] = uniform(seed, 148, idx, -0.6, 0.0)
+        qp[o + 3] = uniform(seed, 149, idx, 0.0, 0.6)
+        qp[o] = np.where(corner == 1, -200.0, qp[o])
+        qp[o + 1] = np.where(corner == 1, -150.0, qp[o + 1])
+        qp[o + 1] = np.where(corner == 2, qp[o], qp[o + 1])
+        qp[o + 3] = np.where(corner == 3, np.nan, qp[o + 3])
+        rev = corner == 4
+        qp[o], qp[o + 1] = np.where(rev, qp[o + 1], qp[o]), np.where(rev, qp[o], qp[o + 1])
+        qp[o + 2], qp[o + 3] = np.where(rev, qp[o + 3], qp[o + 2]), np.where(rev, qp[o + 2], qp[o + 3])
+        qp[o + 1] = np.where(corner == 5, np.inf, qp[o + 1])
+    qp[:, idx == 0] = np.asarray(demo["qp"], np.float64)[:, None]
+    fields = dict(kind=kind, nxy=demo["nxy"], nh=demo["nh"], ns=demo["ns"], d=demo["d"])
+    return fields, np.ascontiguousarray(qp.astype(np.float32))
+
+
+def slp_table(rows: int, seed: int = 0x51A7):
+    """A lookup table [rows, 6] float32 (x, y, yaw, s, km, kf) in lookuptable.csv's ranges, made without it: targets
+    x in [1, 30], y in [-8, 8], yaw in [-0.6, 0.6], s = |xy|, and the seeds km = kf = the curvature of the circle
+    through the origin (heading 0) and (x, y)."""
+    idx = np.arange(rows, dtype=np.uint64)
+    t = np.empty((rows, 6), np.float64)
+    t[:, 0] = uniform(seed, 150, idx, 1.0, 30.0)
+    t[:, 1] = uniform(seed, 151, idx, -8.0, 8.0)
+    t[:, 2] = uniform(seed, 152, idx, -0.6, 0.6)
+    t[:, 3] = np.hypot(t[:, 0], t[:, 1])
+    t[:, 4] = 2.0 * t[:, 1] / (t[:, 3] ** 2)
+    t[:, 5] = t[:, 4]
+    return np.ascontiguousarray(t.astype(np.float32))

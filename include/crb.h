@@ -24,6 +24,11 @@
  *                                         (MotionModel::generate_last_state, quadratic_interpolation,
  *                                          update of include/motion_model.h:59-150)
  *   crb_mptg_generate_trajectory_batched <- MotionModel::generate_trajectory()  include/motion_model.h:110-131
+ *   crb_slp_sample_states_batched       <- calc_uniform_polar_states() / calc_biased_polar_states() /
+ *                                          calc_lane_states()    src/state_lattice_planner.cpp:29-113
+ *   crb_slp_search_nearest_batched      <- search_nearest_one_from_lookuptable()  src/state_lattice_planner.cpp:115-135
+ *                                         (generate_path :137-155 is this search followed by
+ *                                          crb_mptg_optimize_batched with crb_slp_default_params)
  *   crb_stats_*                         <- (no reference counterpart) per-GPU summary statistics, the
  *                                          only thing that ever crosses NVLink (one all-gather).
  *
@@ -418,6 +423,70 @@ int crb_mptg_optimize_batched(crb_ctx* ctx, int64_t n, const float* state, const
 int crb_mptg_generate_trajectory_batched(crb_ctx* ctx, int64_t n, const float* state, const float* param,
                                          const crb_mptg_params* prm, int max_pts, float* traj,
                                          int32_t* traj_len, float* last, int32_t* status);
+
+/* ---- state lattice planner (src/state_lattice_planner.cpp) ------------------------------------------------ */
+/* The planner's own settings (:22-24, :144-148) for generate_path's optimizer: base_l = L 1.0, ds = DS 0.1,
+ * max_iter 100, cost_th 0.1f, h_step {0.5f, 0.02f, 0.02f}; *v = CONST_V 3.0, the speed of the start state
+ * (0, 0, 0, v).  generate_path(states, table, k0) is crb_slp_search_nearest_batched followed by
+ * crb_mptg_optimize_batched with these parameters and that start state. */
+void crb_slp_default_params(crb_mptg_params* p, float* v);
+
+/* Terminal-state samplers.  The batch shares one kind and one set of integers; every query has its own floats. */
+#define CRB_SLP_UNIFORM 0 /* calc_uniform_polar_states :47-56 */
+#define CRB_SLP_BIASED 1  /* calc_biased_polar_states :58-99 */
+#define CRB_SLP_LANE 2    /* calc_lane_states :101-113 */
+typedef struct crb_slp_sampler {
+  int32_t kind; /* CRB_SLP_* */
+  int32_t nxy;  /* position samples (all kinds) */
+  int32_t nh;   /* heading samples (UNIFORM, BIASED) */
+  int32_t ns;   /* biased sampler's angle resolution (BIASED) */
+  int32_t d;    /* distance to the terminal states (UNIFORM, BIASED; LANE takes a float d per query) */
+} crb_slp_sampler;
+/* Limits: 1 <= nxy <= CRB_SLP_MAX_NXY; for UNIFORM and BIASED also 1 <= nh <= CRB_SLP_MAX_NH; for BIASED also
+ * 0 <= ns <= CRB_SLP_MAX_NS; and states per query (below) <= CRB_SLP_MAX_STATES.  Otherwise CRB_ERR_INVALID_ARG. */
+#define CRB_SLP_MAX_NXY 4096
+#define CRB_SLP_MAX_NH 1024
+#define CRB_SLP_MAX_NS (1 << 20)
+#define CRB_SLP_MAX_STATES 65536
+/* S, the output slots per query: nxy * nh (UNIFORM), max(nxy - 1, 0) * nh (BIASED: the scan never matches its
+ * last position sample), nxy (LANE).  -1 (and the error string) for a sampler outside the limits. */
+int crb_slp_states_per_query(const crb_slp_sampler* s);
+
+/* Per-query status of crb_slp_sample_states_batched. */
+#define CRB_SLP_OK 0
+#define CRB_SLP_OUT_OF_RANGE 1 /* a finite sin / cos argument with |x| >= 120, outside the range where this
+                                  library's sinf / cosf are proven equal to glibc's: n_states = 0 */
+
+/* The samplers for n_q queries.
+ *   qp [F][n_q] per-query floats (SoA):
+ *     UNIFORM: F = 4: a_min, a_max, p_min, p_max
+ *     BIASED:  F = 5: goal_angle, a_min, a_max, p_min, p_max
+ *     LANE:    F = 5: l_center, l_heading, l_width, v_width, d
+ *   target [3][n_q * S] out: state j of query q (x, y, yaw) is column q * S + j, in the reference's order; the
+ *     slots from n_states[q] on are NaN
+ *   n_states [n_q] int32 out: states the reference returns (UNIFORM nxy * nh, LANE nxy, BIASED data-dependent:
+ *     the scan's back-step li = j - 1 can repeat a sample); status [n_q] int32 out (CRB_SLP_*), or NULL
+ * Bit-exact with the reference built for x86-64 with glibc 2.39: its float / double mixing expression by
+ * expression (DESIGN.md), glibc's sinf / cosf, the biased sampler's FLT_MIN start of cnav_max and sequential float
+ * sums.  With nxy = 1 the polar samplers' angle is 0 / 0 (NaN), as in the reference.  DEVICE pointers, NULL allowed
+ * when n_q = 0 (target also when S = 0).  Only enqueues on the context's stream. */
+int crb_slp_sample_states_batched(crb_ctx* ctx, int64_t n_q, const crb_slp_sampler* s, const float* qp,
+                                  float* target, int32_t* n_states, int32_t* status);
+
+/* search_nearest_one_from_lookuptable :115-135 for n targets.
+ *   target [3][n] (x, y, yaw); table [rows][6] (x, y, yaw, s, km, kf: lookuptable.csv's columns), rows >= 1
+ *   k0 [n] or NULL (= 0): generate_path's p.steering_sequence[0] = k0 (:141)
+ *   param [4][n] out, in crb_mptg_optimize_batched's layout: (sqrtf(x*x + y*y), k0, km, kf) of the nearest row
+ *   row [n] int32 out or NULL: that row's index
+ * The distance is sqrtf((dx*dx + dy*dy) + dyaw*dyaw) with no yaw wrap, and a row wins only when it is strictly
+ * nearer than the best so far, starting from FLT_MAX: the first of equally near rows wins and a NaN or inf distance
+ * never does.  When no row wins (a NaN target, e.g. the polar samplers' with nxy = 1; the reference then reads
+ * csv_file[-1]) row = -1 and param is NaN, so crb_mptg_optimize_batched stops that problem with
+ * CRB_MPTG_EMPTY_TRAJ (CRB_MPTG_MAX_ITER_REACHED with traj_len 0 when max_iter = 0).  DEVICE pointers (target,
+ * table, param may be NULL when n = 0: a no-op; rows is checked all the same).  Only enqueues on the context's
+ * stream. */
+int crb_slp_search_nearest_batched(crb_ctx* ctx, int64_t n, const float* target, const float* table, int rows,
+                                   const float* k0, float* param, int32_t* row);
 
 /* ---- multi-GPU: communicator owned by the context (NCCL, opened at run time) ---------------------- */
 /* The batch shards over GPUs by contiguous agent ranges (one crb_ctx per device, one host thread or process

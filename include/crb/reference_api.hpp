@@ -11,6 +11,8 @@
 //   solve_DARE / dlqr (4x4 and 5x5)               src/lqr_steer_control.cpp:75-96, lqr_speed_steer_control.cpp:85-106
 //   dwa_control(x, u, config, goal, ob), motion(x, u, dt)   src/dynamic_window_approach.cpp:148-155, :43-50
 //   MotionModel, TrajectoryOptimizer::optimizer_traj(...)    include/motion_model.h, include/trajectory_optimizer.h
+//   calc_{uniform_polar,biased_polar,lane}_states, search_nearest_one_from_lookuptable, generate_path
+//                                                            src/state_lattice_planner.cpp:47-155
 //
 // Eigen is not a dependency: crb::Mat<R,C> is a POD with the memory layout of
 // Eigen::Matrix<float,R,C> (column-major, contiguous, no padding), enough of its interface for the
@@ -513,6 +515,144 @@ class TrajectoryOptimizer {
     }
   }
 };
+
+// src/state_lattice_planner.cpp:25-155 (its Table typedef, include/motion_model.h:56's StateList).  The samplers run
+// one query through crb_slp_sample_states_batched; generate_path runs its whole list as one batch: one search launch
+// and one optimizer launch, with crb_slp_default_params' settings (the file's L, DS, CONST_V, cost_th_, h_step_ and
+// max_iter; no macro of those names is defined here).  A state whose search finds no row (the reference reads
+// csv_file[-1]) or whose optimization stops with a status other than CONVERGED / MAX_ITER_REACHED throws.
+using StateList = std::vector<TrajState>;
+typedef std::vector<std::vector<float>> Table;
+
+namespace detail {
+// qp [nf] | target [3 S] | n_states, status  (n_q = 1)
+inline StateList slp_sample(int kind, int nxy, int nh, int ns, int d, const float* qp, int nf) {
+  crb_ctx* ctx = crb::Session::get();
+  crb_slp_sampler s;
+  s.kind = kind; s.nxy = nxy; s.nh = nh; s.ns = ns; s.d = d;
+  const int S = crb_slp_states_per_query(&s);
+  crb::check(S < 0 ? S : CRB_OK, "crb_slp_states_per_query");
+  float* q = crb::Session::scratch(nf + 3 * (size_t)S + 2);
+  float *t = q + nf, *cnt = t + 3 * (size_t)S;
+  crb::check(crb_memcpy_h2d(ctx, q, qp, nf * sizeof(float)), "h2d");
+  crb::check(crb_slp_sample_states_batched(ctx, 1, &s, q, t, (int32_t*)cnt, (int32_t*)(cnt + 1)),
+             "crb_slp_sample_states_batched");
+  int32_t ks[2];
+  crb::check(crb_memcpy_d2h(ctx, ks, cnt, sizeof(ks)), "d2h");
+  if (ks[1] != CRB_SLP_OK) throw std::runtime_error("state lattice sampler: an angle is outside the exact sin/cos range");
+  std::vector<float> h(3 * (size_t)S);
+  if (S) crb::check(crb_memcpy_d2h(ctx, h.data(), t, h.size() * sizeof(float)), "d2h");
+  StateList states;
+  for (int k = 0; k < ks[0]; ++k) states.push_back(TrajState(h[k], h[S + k], h[2 * (size_t)S + k]));
+  return states;
+}
+inline std::vector<float> slp_flat_table(const Table& csv_file) {
+  std::vector<float> t;
+  t.reserve(6 * csv_file.size());
+  for (size_t r = 0; r < csv_file.size(); ++r) {
+    if (csv_file[r].size() < 6) throw std::runtime_error("lookup table: a row has fewer than 6 columns");
+    t.insert(t.end(), csv_file[r].begin(), csv_file[r].begin() + 6);
+  }
+  if (t.empty() || csv_file.size() > 0x7fffffffu) throw std::runtime_error("lookup table: bad number of rows");
+  return t;
+}
+}  // namespace detail
+
+// calc_uniform_polar_states :47-56
+inline StateList calc_uniform_polar_states(int nxy, int nh, int d, float a_min, float a_max, float p_min, float p_max) {
+  const float qp[4] = {a_min, a_max, p_min, p_max};
+  return detail::slp_sample(CRB_SLP_UNIFORM, nxy, nh, 0, d, qp, 4);
+}
+// calc_biased_polar_states :58-99
+inline StateList calc_biased_polar_states(float goal_angle, int ns, int nxy, int nh, int d, float a_min, float a_max,
+                                          float p_min, float p_max) {
+  const float qp[5] = {goal_angle, a_min, a_max, p_min, p_max};
+  return detail::slp_sample(CRB_SLP_BIASED, nxy, nh, ns, d, qp, 5);
+}
+// calc_lane_states :101-113
+inline StateList calc_lane_states(float l_center, float l_heading, float l_width, float v_width, float d, int nxy) {
+  const float qp[5] = {l_center, l_heading, l_width, v_width, d};
+  return detail::slp_sample(CRB_SLP_LANE, nxy, 1, 0, 0, qp, 5);
+}
+
+// search_nearest_one_from_lookuptable :115-135: (|xy|, {0, km, kf}) of the nearest row
+inline Parameter search_nearest_one_from_lookuptable(TrajState target, Table csv_file) {
+  crb_ctx* ctx = crb::Session::get();
+  const std::vector<float> tb = detail::slp_flat_table(csv_file);
+  // table [6 rows] | target [3] | param [4] | row [1]
+  float* dtb = crb::Session::scratch(tb.size() + 8);
+  float *dt = dtb + tb.size(), *dp = dt + 3;
+  const float t[3] = {target.x, target.y, target.yaw};
+  crb::check(crb_memcpy_h2d(ctx, dtb, tb.data(), tb.size() * sizeof(float)), "h2d");
+  crb::check(crb_memcpy_h2d(ctx, dt, t, sizeof(t)), "h2d");
+  crb::check(crb_slp_search_nearest_batched(ctx, 1, dt, dtb, (int)csv_file.size(), nullptr, dp, (int32_t*)(dp + 4)),
+             "crb_slp_search_nearest_batched");
+  float p[5];
+  crb::check(crb_memcpy_d2h(ctx, p, dp, sizeof(p)), "d2h");
+  int32_t row;
+  std::memcpy(&row, &p[4], sizeof(row));
+  if (row < 0) throw std::runtime_error("search_nearest_one_from_lookuptable: no row is nearer than FLT_MAX");
+  return Parameter(p[0], {{p[1], p[2], p[3]}});
+}
+
+// generate_path :137-155
+inline std::vector<Traj> generate_path(StateList states, Table csv_file, float k0 = 0.0) {
+  crb_ctx* ctx = crb::Session::get();
+  const std::vector<float> tb = detail::slp_flat_table(csv_file);
+  const size_t n = states.size();
+  std::vector<Traj> out(n);
+  if (n == 0) return out;
+  crb_mptg_params prm;
+  float v = 0.0f;
+  crb_slp_default_params(&prm, &v);
+  std::vector<float> h(8 * n, 0.0f);  // target [3][n] | k0 [n] | state [4][n]
+  for (size_t i = 0; i < n; ++i) {
+    h[i] = states[i].x;
+    h[n + i] = states[i].y;
+    h[2 * n + i] = states[i].yaw;
+    h[3 * n + i] = k0;
+    h[7 * n + i] = v;  // state (0, 0, 0, CONST_V)
+  }
+  int max_pts = 256;
+  for (;;) {
+    // target [3n] | k0 [n] | state [4n] | param [4n] | row, len, status [3n] | table | traj [3 max_pts n]
+    float* d = crb::Session::scratch(15 * n + tb.size() + 3 * (size_t)max_pts * n);
+    float *dk0 = d + 3 * n, *dst = dk0 + n, *dp = dst + 4 * n, *drow = dp + 4 * n, *dlen = drow + n,
+          *dstat = dlen + n, *dtb = dstat + n, *dtraj = dtb + tb.size();
+    crb::check(crb_memcpy_h2d(ctx, d, h.data(), 8 * n * sizeof(float)), "h2d");
+    crb::check(crb_memcpy_h2d(ctx, dtb, tb.data(), tb.size() * sizeof(float)), "h2d");
+    crb::check(crb_slp_search_nearest_batched(ctx, (int64_t)n, d, dtb, (int)csv_file.size(), dk0, dp,
+                                              (int32_t*)drow),
+               "crb_slp_search_nearest_batched");
+    crb::check(crb_mptg_optimize_batched(ctx, (int64_t)n, dst, d, dp, &prm, max_pts, dtraj, (int32_t*)dlen, nullptr,
+                                         (int32_t*)dstat, nullptr),
+               "crb_mptg_optimize_batched");
+    std::vector<int32_t> rls(3 * n);
+    crb::check(crb_memcpy_d2h(ctx, rls.data(), drow, rls.size() * sizeof(int32_t)), "d2h");
+    int longest = 0;
+    for (size_t i = 0; i < n; ++i) {
+      if (rls[i] < 0) throw std::runtime_error("generate_path: a state has no nearest lookup-table row");
+      const int st = rls[2 * n + i];
+      if (st != CRB_MPTG_CONVERGED && st != CRB_MPTG_MAX_ITER_REACHED)
+        throw std::runtime_error("generate_path: optimizer_traj stopped with status " + std::to_string(st));
+      if (rls[n + i] > longest) longest = rls[n + i];
+    }
+    if (longest > max_pts) {  // the same batch again with room for every whole trajectory
+      max_pts = longest;
+      continue;
+    }
+    std::vector<float> tr(3 * (size_t)max_pts * n);
+    crb::check(crb_memcpy_d2h(ctx, tr.data(), dtraj, tr.size() * sizeof(float)), "d2h");
+    for (size_t i = 0; i < n; ++i) {
+      Traj& t = out[i];
+      t.reserve((size_t)rls[n + i]);
+      for (int k = 0; k < rls[n + i]; ++k)
+        t.push_back(TrajState(tr[(3 * (size_t)k) * n + i], tr[(3 * (size_t)k + 1) * n + i],
+                              tr[(3 * (size_t)k + 2) * n + i]));
+    }
+    return out;
+  }
+}
 }  // namespace cpprobotics
 
 #endif  // CRB_REFERENCE_API_HPP_
