@@ -695,14 +695,33 @@ static int mpc_launch(crb_ctx* ctx, cudaStream_t st, int64_t count, int64_t ld, 
   return CRB_OK;
 }
 
+// The limits of crb.h (after crb_mpc_default_params), checked before any device work.  A NaN fails every comparison.
+static int mpc_check_params(const crb_mpc_params* prm) {
+  CRB_REQUIRE(prm != nullptr, "prm is NULL");
+  const float f[] = {prm->dt, prm->wb, prm->max_steer, prm->max_accel, prm->max_speed, prm->min_speed,
+                     prm->w_a, prm->w_delta, prm->w_da, prm->w_ddelta, prm->w_x, prm->w_y, prm->w_yaw, prm->w_v,
+                     prm->du_th, prm->j_tol};
+  for (float v : f) CRB_REQUIRE(isfinite(v), "every float parameter must be finite");
+  CRB_REQUIRE(prm->dt > 0.0f && prm->wb > 0.0f, "dt and wb must be positive");
+  // tan(max_steer) must exist; a steering bound below pi/2 also keeps update()'s tanf in crb_tanf_libm's range
+  CRB_REQUIRE(prm->max_steer > 0.0f && (double)prm->max_steer < 1.57079632679489661923,
+              "max_steer must be in (0, pi/2)");
+  CRB_REQUIRE(prm->max_accel >= 0.0f, "max_accel must be >= 0");
+  CRB_REQUIRE(prm->min_speed <= prm->max_speed, "min_speed must be <= max_speed");
+  const float w[] = {prm->w_a, prm->w_delta, prm->w_da, prm->w_ddelta, prm->w_x, prm->w_y, prm->w_yaw, prm->w_v};
+  for (float v : w) CRB_REQUIRE(v >= 0.0f, "cost weights must be >= 0");
+  CRB_REQUIRE(prm->du_th >= 0.0f && prm->j_tol >= 0.0f, "du_th and j_tol must be >= 0");
+  CRB_REQUIRE(prm->max_iter >= 0 && prm->max_ls >= 0, "max_iter / max_ls negative");
+  return CRB_OK;
+}
+
 static int mpc_check(crb_ctx* ctx, int64_t n, int T, const float* x0, const float* xref,
                      const crb_mpc_params* prm) {
   CRB_REQUIRE(ctx != nullptr, "ctx is NULL");
-  CRB_REQUIRE(prm != nullptr, "prm is NULL");
+  const int rc = mpc_check_params(prm);
+  if (rc) return rc;
   CRB_REQUIRE(n >= 0, "n < 0");
   CRB_REQUIRE(T >= 2 && T <= CRB_MPC_MAX_T, "T out of range [2, CRB_MPC_MAX_T]");
-  CRB_REQUIRE(prm->dt > 0.0f && prm->wb > 0.0f, "dt and wb must be positive");
-  CRB_REQUIRE(prm->max_iter >= 0 && prm->max_ls >= 0, "max_iter / max_ls negative");
   CRB_REQUIRE(n == 0 || (x0 && xref), "NULL array");
   return CRB_OK;
 }
@@ -859,7 +878,9 @@ crb_mpc_plant_update_kernel(int64_t n, float* __restrict__ state, const float* _
   crb_sincosf_libm(yaw, sy, cy);   // std::cos / std::sin of a float: the host libm's bits (crb_common.cuh)
   const float nx = (float)((double)x + (double)(v * cy) * DT);
   const float ny = (float)((double)y + (double)(v * sy) * DT);
-  const float nyaw = (float)((double)yaw + (double)v / WB * (double)tanf(delta) * DT);
+  // std::tan of a float: glibc's bits.  |delta| <= max_steer < pi/2 (crb.h limits), inside crb_tanf_libm's
+  // proven range; a NaN delta stays NaN
+  const float nyaw = (float)((double)yaw + (double)v / WB * (double)crb_tanf_libm(delta) * DT);
   float nv = (float)((double)v + (double)a * DT);
   if ((double)nv > MAX_SPEED) nv = (float)MAX_SPEED;
   if ((double)nv < MIN_SPEED) nv = (float)MIN_SPEED;
@@ -869,12 +890,12 @@ crb_mpc_plant_update_kernel(int64_t n, float* __restrict__ state, const float* _
 extern "C" int crb_mpc_plant_update_batched(crb_ctx* ctx, int64_t n, float* state, const float* u0,
                                             const crb_mpc_params* prm) {
   CRB_REQUIRE(ctx != nullptr, "ctx is NULL");
-  CRB_DEVICE_GUARD(ctx);   // ctx->device is current for this call, the caller's device is restored after it
-  CRB_REQUIRE(prm != nullptr, "prm is NULL");
+  const int rc = mpc_check_params(prm);
+  if (rc) return rc;
   CRB_REQUIRE(n >= 0, "n < 0");
-  CRB_REQUIRE(prm->dt > 0.0f && prm->wb > 0.0f, "dt and wb must be positive");
   if (n == 0) return CRB_OK;
   CRB_REQUIRE(state && u0, "NULL array");
+  CRB_DEVICE_GUARD(ctx);   // ctx->device is current for this call, the caller's device is restored after it
   crb_mpc_plant_update_kernel<<<crb_grid_for(n, 256), 256, 0, ctx->stream>>>(n, state, u0,
                                                                              mpc_plant_constants(prm));
   CRB_CUDA(cudaGetLastError());
@@ -925,12 +946,13 @@ extern "C" int crb_mpc_calc_ref_trajectory_batched(crb_ctx* ctx, int64_t n, int 
                                                    int32_t* target_ind, float* xref,
                                                    const crb_mpc_params* prm) {
   CRB_REQUIRE(ctx != nullptr, "ctx is NULL");
-  CRB_DEVICE_GUARD(ctx);   // ctx->device is current for this call, the caller's device is restored after it
   CRB_REQUIRE(n >= 0 && T >= 1 && T <= CRB_MPC_MAX_T, "n < 0 or T out of range");
   CRB_REQUIRE(ncourse >= 1 && dl > 0.0f, "empty course or dl <= 0");
-  CRB_REQUIRE(prm != nullptr && prm->dt > 0.0f, "prm is NULL or dt <= 0");
+  // the lookup uses only dt
+  CRB_REQUIRE(prm != nullptr && isfinite(prm->dt) && prm->dt > 0.0f, "prm is NULL or dt not finite and > 0");
   if (n == 0) return CRB_OK;
   CRB_REQUIRE(state && cx && cy && cyaw && sp && target_ind && xref, "NULL array");
+  CRB_DEVICE_GUARD(ctx);   // ctx->device is current for this call, the caller's device is restored after it
   crb_mpc_ref_traj_kernel<<<crb_grid_for(n, 256), 256, 0, ctx->stream>>>(
       n, T, state, cx, cy, cyaw, sp, ncourse, dl, target_ind, xref, mpc_plant_constants(prm).dt);
   CRB_CUDA(cudaGetLastError());

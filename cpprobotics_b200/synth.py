@@ -138,7 +138,8 @@ def mpc_states(n: int, i0: int = 0, seed: int = 0xC0FFEE, course=None):
 def mpc_xref_numpy(state, pind, T: int, course=None, dl: float = 1.0, dt: float = 0.2):
     """Vectorised restatement of calc_ref_trajectory / calc_nearest_index
     (src/model_predictive_control.cpp:107-170) used to synthesise the solver's xref input
-    [4T, n] (field 4t+k).  float32 arithmetic where the reference uses float."""
+    [4T, n] (field 4t+k).  float32 arithmetic where the reference uses float.  dt is the double DT of :149
+    (for a crb_mpc_params.dt other than the default, the value libcrb promotes it to: the float's own value)."""
     cx, cy, cyaw, sp = course if course is not None else mpc_course()
     n = state.shape[1]
     nc = len(cx)
@@ -156,7 +157,10 @@ def mpc_xref_numpy(state, pind, T: int, course=None, dl: float = 1.0, dt: float 
     for i in range(T):
         travel = (travel.astype(np.float64) + np.abs(state[3]).astype(np.float64) * dt).astype(np.float32)
         q = (travel / np.float32(dl)).astype(np.float32)
-        dind = np.where(q >= 0, np.floor(q + np.float32(0.5)), np.ceil(q - np.float32(0.5))).astype(np.int64)
+        # roundf (:150): half away from zero.  q >= 0 and q < 2^23, so floor(q) and q - floor(q) are exact;
+        # floor(q + 0.5f) is not (it rounds q = 0.49999997f up to 1)
+        r = np.floor(q)
+        dind = (r + (q - r >= np.float32(0.5))).astype(np.int64)
         j = np.minimum(ind + dind, nc - 1)
         xref[4 * i + 0] = cx[j]
         xref[4 * i + 1] = cy[j]

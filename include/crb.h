@@ -248,6 +248,11 @@ typedef struct crb_mpc_params {
 } crb_mpc_params;
 void crb_mpc_default_params(crb_mpc_params* p);
 
+/* Limits.  Every float parameter finite, dt > 0, wb > 0, 0 < max_steer < pi/2, max_accel >= 0,
+ * min_speed <= max_speed, the eight weights, du_th and j_tol >= 0, max_iter and max_ls >= 0; otherwise the solve and
+ * the plant step return CRB_ERR_INVALID_ARG before any device work.  calc_ref_trajectory uses (and checks) only dt.
+ * The defaults are inside these limits. */
+
 #define CRB_MPC_MAX_T 32
 /* Per-agent status word (the reference drops IPOPT's status, :338-339). */
 #define CRB_MPC_CONVERGED     0  /* sum|du| <= du_th */
@@ -286,6 +291,8 @@ int crb_mpc_solve_batched_hinted(crb_ctx* ctx, int64_t n, int T, const float* x0
  * step in double because its constants are double macros (:26-38): a parameter equal to the reference's
  * macro rounded to float is taken as the macro's double value (defaults are bit-identical to the
  * reference), any other value is promoted from float.  The same rule gives calc_ref_trajectory its DT.
+ * cos and sin of the yaw (|yaw| < 120) and tan of the clamped steering are restatements of x86-64 glibc's
+ * sinf / cosf (its FMA build) and tanf, so the step reproduces the reference's bits on such a host.
  * Replaces: update(State&, float a, float delta), src/model_predictive_control.cpp:69-81. */
 int crb_mpc_plant_update_batched(crb_ctx* ctx, int64_t n, float* state, const float* u0,
                                  const crb_mpc_params* prm);

@@ -627,10 +627,11 @@ void crb_oracle_mpc_solve_batched(int64_t n, int T, const float* x0, const float
 /* ---- update(): src/model_predictive_control.cpp:69-81 (plant step on the first control).
  * MAX_STEER, DT, WB, MAX_SPEED, MIN_SPEED are double macros: float operands promote to double and the
  * result narrows on assignment; std::cos/std::sin of a float are the float overloads; CppAD::tan of a
- * float resolves to std::tan(float). */
-void crb_oracle_plant_update(float st[4], float a, float delta) {
-  const double MAX_STEER = 45.0 / 180 * M_PI, DT = 0.2, WB = 2.5;
-  const double MAX_SPEED = 55.0 / 3.6, MIN_SPEED = -20.0 / 3.6;
+ * float resolves to std::tan(float).  k = {MAX_STEER, DT, WB, MAX_SPEED, MIN_SPEED}: the macros' values, or any
+ * other constants in double (libcrb's promotion rule, crb.h, is applied by the caller). */
+void crb_oracle_plant_update_k(float st[4], float a, float delta, const double k[5]) {
+  const double MAX_STEER = k[0], DT = k[1], WB = k[2];
+  const double MAX_SPEED = k[3], MIN_SPEED = k[4];
   if ((double)delta >= MAX_STEER) delta = (float)MAX_STEER;
   if ((double)delta <= -MAX_STEER) delta = (float)(-MAX_STEER);
   const float x = st[0], y = st[1], yaw = st[2], v = st[3];
@@ -640,6 +641,11 @@ void crb_oracle_plant_update(float st[4], float a, float delta) {
   st[3] = (float)((double)v + (double)a * DT);
   if ((double)st[3] > MAX_SPEED) st[3] = (float)MAX_SPEED;
   if ((double)st[3] < MIN_SPEED) st[3] = (float)MIN_SPEED;
+}
+
+void crb_oracle_plant_update(float st[4], float a, float delta) {
+  const double k[5] = {45.0 / 180 * M_PI, 0.2, 2.5, 55.0 / 3.6, -20.0 / 3.6};
+  crb_oracle_plant_update_k(st, a, delta, k);
 }
 
 /* ---- calc_nearest_index :107-127.  `ind` is a float in the reference (:109); the window is
@@ -661,11 +667,10 @@ int crb_oracle_calc_nearest_index(const float st[4], const float* cx, const floa
   return (int)ind;
 }
 
-/* ---- calc_ref_trajectory :130-170; xref out as [T][4] ------------------------------------------------ */
-void crb_oracle_calc_ref_trajectory(const float st[4], const float* cx, const float* cy,
-                                    const float* cyaw, const float* sp, int ncourse, float dl, int T,
-                                    int* target_ind, float* xref /*[T][4]*/) {
-  const double DT = 0.2;
+/* ---- calc_ref_trajectory :130-170; xref out as [T][4].  DT: the macro's 0.2, or any other step in double ---- */
+void crb_oracle_calc_ref_trajectory_dt(const float st[4], const float* cx, const float* cy,
+                                       const float* cyaw, const float* sp, int ncourse, float dl, int T,
+                                       int* target_ind, float* xref /*[T][4]*/, double DT) {
   for (int i = 0; i < 4 * T; ++i) xref[i] = 0.0f;                                  /* :133 */
   int ind = crb_oracle_calc_nearest_index(st, cx, cy, ncourse, *target_ind);       /* :138 */
   if (*target_ind >= ind) ind = *target_ind;                                       /* :139 */
@@ -681,4 +686,10 @@ void crb_oracle_calc_ref_trajectory(const float st[4], const float* cx, const fl
     xref[i * 4 + 3] = sp[j];
   }
   *target_ind = ind;                                                               /* :169 */
+}
+
+void crb_oracle_calc_ref_trajectory(const float st[4], const float* cx, const float* cy,
+                                    const float* cyaw, const float* sp, int ncourse, float dl, int T,
+                                    int* target_ind, float* xref /*[T][4]*/) {
+  crb_oracle_calc_ref_trajectory_dt(st, cx, cy, cyaw, sp, ncourse, dl, T, target_ind, xref, 0.2);
 }

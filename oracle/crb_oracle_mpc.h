@@ -33,12 +33,18 @@ void crb_oracle_mpc_solve_batched(int64_t n, int T, const float* x0, const float
                                   const float* u_init, const crb_oracle_mpc_params* p, float* sol,
                                   float* u0, float* cost, int32_t* status, int32_t* iters,
                                   int nthreads);
+/* update() with the reference's macros, and with k = {MAX_STEER, DT, WB, MAX_SPEED, MIN_SPEED} */
 void crb_oracle_plant_update(float st[4], float a, float delta);
+void crb_oracle_plant_update_k(float st[4], float a, float delta, const double k[5]);
 int crb_oracle_calc_nearest_index(const float st[4], const float* cx, const float* cy, int ncourse,
                                   int pind);
+/* calc_ref_trajectory() with the reference's DT, and with any DT */
 void crb_oracle_calc_ref_trajectory(const float st[4], const float* cx, const float* cy,
                                     const float* cyaw, const float* sp, int ncourse, float dl, int T,
                                     int* target_ind, float* xref);
+void crb_oracle_calc_ref_trajectory_dt(const float st[4], const float* cx, const float* cy,
+                                       const float* cyaw, const float* sp, int ncourse, float dl, int T,
+                                       int* target_ind, float* xref, double DT);
 #ifdef __cplusplus
 }
 #endif

@@ -252,10 +252,13 @@ def _mpc_lib():
             C.c_int64, C.c_int, f32p, f32p, C.c_void_p, C.POINTER(MpcParams), C.c_void_p, C.c_void_p,
             C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         L.crb_oracle_plant_update.argtypes = [f32p, C.c_float, C.c_float]
+        L.crb_oracle_plant_update_k.argtypes = [f32p, C.c_float, C.c_float, f64p]
         L.crb_oracle_calc_nearest_index.restype = C.c_int
         L.crb_oracle_calc_nearest_index.argtypes = [f32p, f32p, f32p, C.c_int, C.c_int]
         L.crb_oracle_calc_ref_trajectory.argtypes = [f32p, f32p, f32p, f32p, f32p, C.c_int, C.c_float,
                                                      C.c_int, C.POINTER(C.c_int), f32p]
+        L.crb_oracle_calc_ref_trajectory_dt.argtypes = [f32p, f32p, f32p, f32p, f32p, C.c_int, C.c_float,
+                                                        C.c_int, C.POINTER(C.c_int), f32p, C.c_double]
         L._mpc_ready = True
     return L
 
@@ -288,9 +291,27 @@ def mpc_solve_batched(x0, xref, T, params=None, u_init=None, nthreads=0):
     return dict(sol=sol, u0=u0, cost=cost, status=status, iters=iters)
 
 
-def plant_update(state, a, delta):
+# update()'s double macros (src/model_predictive_control.cpp:26-38) in crb_mpc_params' field names
+PLANT_MACROS = dict(max_steer=45.0 / 180 * np.pi, dt=0.2, wb=2.5, max_speed=55.0 / 3.6, min_speed=-20.0 / 3.6)
+
+
+def plant_constant(params, name):
+    """libcrb's promotion rule (include/crb.h): a float parameter equal to the reference's macro rounded to
+    float stands for the macro's double value; any other value is promoted from float."""
+    v = np.float32(getattr(params, name))
+    ref = PLANT_MACROS[name]
+    return ref if v == np.float32(ref) else float(v)
+
+
+def plant_update(state, a, delta, params=None):
+    """update() :69-81 on one state [4]; params (MpcParams) gives max_steer, dt, wb, max_speed and min_speed,
+    None = the reference's macros."""
     st = np.ascontiguousarray(state, np.float32).copy()
-    _mpc_lib().crb_oracle_plant_update(st, float(a), float(delta))
+    if params is None:
+        _mpc_lib().crb_oracle_plant_update(st, float(a), float(delta))
+    else:
+        k = np.array([plant_constant(params, f) for f in ("max_steer", "dt", "wb", "max_speed", "min_speed")])
+        _mpc_lib().crb_oracle_plant_update_k(st, float(a), float(delta), k)
     return st
 
 
@@ -300,12 +321,15 @@ def calc_nearest_index(state, cx, cy, pind):
         np.ascontiguousarray(cy, np.float32), len(cx), int(pind)))
 
 
-def calc_ref_trajectory(state, cx, cy, cyaw, sp, dl, T, target_ind):
-    """Returns (xref [T,4], new target_ind)."""
+def calc_ref_trajectory(state, cx, cy, cyaw, sp, dl, T, target_ind, params=None):
+    """Returns (xref [T,4], new target_ind).  params (MpcParams) gives dt, None = the reference's DT."""
     ti = C.c_int(int(target_ind))
     xref = np.zeros((T, 4), np.float32)
-    _mpc_lib().crb_oracle_calc_ref_trajectory(
-        np.ascontiguousarray(state, np.float32), np.ascontiguousarray(cx, np.float32),
-        np.ascontiguousarray(cy, np.float32), np.ascontiguousarray(cyaw, np.float32),
-        np.ascontiguousarray(sp, np.float32), len(cx), float(dl), int(T), C.byref(ti), xref)
+    args = (np.ascontiguousarray(state, np.float32), np.ascontiguousarray(cx, np.float32),
+            np.ascontiguousarray(cy, np.float32), np.ascontiguousarray(cyaw, np.float32),
+            np.ascontiguousarray(sp, np.float32), len(cx), float(dl), int(T), C.byref(ti), xref)
+    if params is None:
+        _mpc_lib().crb_oracle_calc_ref_trajectory(*args)
+    else:
+        _mpc_lib().crb_oracle_calc_ref_trajectory_dt(*args, plant_constant(params, "dt"))
     return xref, ti.value

@@ -13,6 +13,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import mpc_cases as MC
 from cpprobotics_b200 import synth
 from oracle import oracle as O
 
@@ -59,10 +60,10 @@ def run_sim(L, st, xref, T, prm, S, seed, u_init=None, hint=None):
     return out
 
 
-def case(n, T, seed=0xC0FFEE):
+def case(n, T, seed=0xC0FFEE, dt=0.2):
     course = synth.mpc_course()
     st, pind = synth.mpc_states(n, seed=seed, course=course)
-    xref, _ = synth.mpc_xref_numpy(st, pind, T, course=course)
+    xref, _ = synth.mpc_xref_numpy(st, pind, T, course=course, dt=dt)
     return st, xref
 
 
@@ -81,6 +82,22 @@ def test_task_machine_is_bit_exact_for_any_schedule(sim, n, T, S, seed):
     same(got, want)
     # every problem was refilled once; sweeps were really regrouped (more than one task of each kind)
     assert got["tasks"].min() >= 1
+
+
+@pytest.mark.parametrize("S", [64, 17])
+@pytest.mark.parametrize("T", [7, 20])
+@pytest.mark.parametrize("name", ["W", "B", "S"])
+def test_task_machine_is_bit_exact_at_non_default_constants(sim, name, T, S):
+    """The parameter sets of tests/mpc_cases.py: every weight distinct (W), other model and bounds with the speed
+    bound active (B), a slow vehicle (S).  (The simulator fills the kernel's parameter block itself; the GPU tests
+    in test_mpc_constants.py check libcrb's own fill.)"""
+    over = MC.SETS[name]
+    st, xref = case(300, T, seed=T + S, dt=O.plant_constant(O.mpc_params(**over), "dt"))
+    prm = O.mpc_params(**over)
+    want = O.mpc_solve_batched(st, xref, T, prm)
+    got = run_sim(sim, st, xref, T, prm, S, seed=T * S)
+    same(got, want)
+    assert (want["status"] == 0).all() and got["tasks"].min() >= 1
 
 
 @pytest.mark.parametrize("kind", ["iters", "random", "constant", "negative_and_huge", "one_long"])
