@@ -162,6 +162,7 @@ PROTOTYPES = {
     "crb_stats_reduce": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p]),
     "crb_probe_fp32_peak": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),
+    "crb_probe_ekf_pattern": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "crb_comm_nccl_version": (C.c_int, []),
     "crb_comm_get_unique_id": (C.c_int, [C.c_void_p]),
     "crb_comm_init_rank": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),

@@ -99,40 +99,80 @@ __device__ __forceinline__ void ekf_step(float (&x)[4], float (&P)[16], float z0
   }
 }
 
+// V consecutive floats of one field: one 4-byte (V = 1) or 8-byte (V = 2) streaming access.
+template <int V>
+__device__ __forceinline__ void ld_agents(const float* p, float (&v)[V]) {
+  if constexpr (V == 1) {
+    v[0] = ld_stream(p);
+  } else {
+    const float2 t = __ldcs(reinterpret_cast<const float2*>(p));
+    v[0] = t.x;
+    v[1] = t.y;
+  }
+}
+template <int V>
+__device__ __forceinline__ void st_agents(float* p, const float (&v)[V]) {
+  if constexpr (V == 1) st_stream(p, v[0]);
+  else __stcs(reinterpret_cast<float2*>(p), make_float2(v[0], v[1]));
+}
+
 // count agents, leading dimension ld (>= count) for x/P, ld_zu for z/u (they may live in a staging
-// buffer with a different pitch).
-template <int BLOCK, int MINB>
+// buffer with a different pitch).  Each thread filters V consecutive agents; V = 2 needs count, ld and ld_zu
+// even and 8-byte aligned arrays (ekf_launch checks), and then a warp access is 256 contiguous bytes of one
+// field: half the memory instructions per byte, and the two agents' algebra is independent work for the
+// scheduler while their loads are in flight.
+template <int BLOCK, int MINB, int V>
 __global__ void __launch_bounds__(BLOCK, MINB)
 crb_ekf_step_kernel(int64_t count, int64_t ld, float* __restrict__ x, float* __restrict__ P,
                     const float* __restrict__ z, const float* __restrict__ u, int64_t ld_zu,
                     int n_steps, EkfArgs a) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t i = V * ((int64_t)blockIdx.x * blockDim.x + threadIdx.x);
   if (i >= count) return;
   crb_pdl_launch_dependents();   // the next launch may start scheduling its CTAs behind ours
   crb_pdl_wait();   // the previous launch on this stream (e.g. the preceding filter step) is complete
-  float xs[4], Ps[16];
+  float xs[4][V], Ps[16][V], z0[V], z1[V], u0[V], u1[V];
 #pragma unroll
-  for (int f = 0; f < 4; ++f) xs[f] = ld_stream(x + f * ld + i);
+  for (int f = 0; f < 4; ++f) ld_agents<V>(x + f * ld + i, xs[f]);
 #pragma unroll
-  for (int f = 0; f < 16; ++f) Ps[f] = ld_stream(P + f * ld + i);
-  float z0 = ld_stream(z + 0 * ld_zu + i), z1 = ld_stream(z + 1 * ld_zu + i);
-  float u0 = ld_stream(u + 0 * ld_zu + i), u1 = ld_stream(u + 1 * ld_zu + i);
+  for (int f = 0; f < 16; ++f) ld_agents<V>(P + f * ld + i, Ps[f]);
+  ld_agents<V>(z + 0 * ld_zu + i, z0);
+  ld_agents<V>(z + 1 * ld_zu + i, z1);
+  ld_agents<V>(u + 0 * ld_zu + i, u0);
+  ld_agents<V>(u + 1 * ld_zu + i, u1);
   for (int s = 0; s < n_steps; ++s) {
-    float nz0 = 0.f, nz1 = 0.f, nu0 = 0.f, nu1 = 0.f;
+    float nz0[V] = {}, nz1[V] = {}, nu0[V] = {}, nu1[V] = {};
     if (s + 1 < n_steps) {  // prefetch the next step's observation/control under this step's math
       const int64_t o = (int64_t)(s + 1) * 2;
-      nz0 = ld_stream(z + (o + 0) * ld_zu + i);
-      nz1 = ld_stream(z + (o + 1) * ld_zu + i);
-      nu0 = ld_stream(u + (o + 0) * ld_zu + i);
-      nu1 = ld_stream(u + (o + 1) * ld_zu + i);
+      ld_agents<V>(z + (o + 0) * ld_zu + i, nz0);
+      ld_agents<V>(z + (o + 1) * ld_zu + i, nz1);
+      ld_agents<V>(u + (o + 0) * ld_zu + i, nu0);
+      ld_agents<V>(u + (o + 1) * ld_zu + i, nu1);
     }
-    ekf_step(xs, Ps, z0, z1, u0, u1, a);
-    z0 = nz0; z1 = nz1; u0 = nu0; u1 = nu1;
+#pragma unroll
+    for (int k = 0; k < V; ++k) {
+      float xk[4], Pk[16];
+#pragma unroll
+      for (int f = 0; f < 4; ++f) xk[f] = xs[f][k];
+#pragma unroll
+      for (int f = 0; f < 16; ++f) Pk[f] = Ps[f][k];
+      ekf_step(xk, Pk, z0[k], z1[k], u0[k], u1[k], a);
+#pragma unroll
+      for (int f = 0; f < 4; ++f) xs[f][k] = xk[f];
+#pragma unroll
+      for (int f = 0; f < 16; ++f) Ps[f][k] = Pk[f];
+      z0[k] = nz0[k]; z1[k] = nz1[k]; u0[k] = nu0[k]; u1[k] = nu1[k];
+    }
   }
+  // The store addresses are recomputed after the math instead of reusing the load addresses: keeping ~20
+  // 64-bit field addresses live across ekf_step costs 80 registers and a 24-byte spill on the hot path.  The
+  // empty asm hides that ld and i are the values the loads used.  Offsets stay 64-bit: 19 * ld + i passes 2^31
+  // at about 1.1e8 agents.
+  int64_t lds = ld, is = i;
+  asm volatile("" : "+l"(lds), "+l"(is));
 #pragma unroll
-  for (int f = 0; f < 4; ++f) st_stream(x + f * ld + i, xs[f]);
+  for (int f = 0; f < 4; ++f) st_agents<V>(x + f * lds + is, xs[f]);
 #pragma unroll
-  for (int f = 0; f < 16; ++f) st_stream(P + f * ld + i, Ps[f]);
+  for (int f = 0; f < 16; ++f) st_agents<V>(P + f * lds + is, Ps[f]);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -304,10 +344,12 @@ static int ekf_launch(crb_ctx* ctx, cudaStream_t st, int64_t count, int64_t ld, 
   a.dt = prm->dt;
   memcpy(a.Q, prm->Q, sizeof(a.Q));
   memcpy(a.R, prm->R, sizeof(a.R));
-  // Launch shape: 256-thread CTAs, 3 resident per SM (85 registers): 24 warps x 24 independent 128-byte loads
-  // in flight per SM cover H100's HBM latency.  At 4 per SM (64 registers) the kernel spills on sm_90a: measured
-  // on an H100 SXM (400 W limit), 2^20 agents, 13.0 G updates/s vs 15.0 G at 3 per SM.  CRB_EKF_VARIANT selects
-  // alternatives for A/B measurements.
+  // Launch shape: two agents per thread in 128-thread CTAs, 4 resident per SM, whenever the arrays allow 8-byte
+  // accesses; otherwise one agent per thread in 256-thread CTAs, 3 per SM.  Either way every SM has ~24 KB of
+  // independent reads in flight per 256 agents, which covers H100's HBM latency.  Measured at 2^20 agents, 30
+  // graph-captured launches over 3 buffer sets, on two H100 80GB HBM3 boxes (700 W limit): the two-agent form runs
+  // 4.6 % and 6.4 % faster than the one-agent form, and 4, 2 or 6 CTAs per SM make no difference (DESIGN.md 3).
+  // CRB_EKF_VARIANT selects alternatives for A/B measurements.
   static int variant = -1;
   if (variant < 0) {
     const char* e = getenv("CRB_EKF_VARIANT");
@@ -316,26 +358,33 @@ static int ekf_launch(crb_ctx* ctx, cudaStream_t st, int64_t count, int64_t ld, 
   // bulk copies need 16-byte aligned, 16-byte multiple row segments
   const bool tma_ok = n_steps == 1 && (ld % 4) == 0 && (ld_zu % 4) == 0 && (count % 4) == 0 &&
                       (((uintptr_t)x | (uintptr_t)P | (uintptr_t)z | (uintptr_t)u) & 15) == 0;
+  // two agents per thread: every row segment a thread touches is 8-byte aligned
+  const bool pair_ok = (count % 2) == 0 && (ld % 2) == 0 && (ld_zu % 2) == 0 &&
+                       (((uintptr_t)x | (uintptr_t)P | (uintptr_t)z | (uintptr_t)u) & 7) == 0;
   if (tma_ok && variant == 4) return ekf_tma_launch<128, 3>(ctx, st, count, ld, x, P, z, u, ld_zu, a);
   if (tma_ok && variant == 5) return ekf_tma_launch<128, 2>(ctx, st, count, ld, x, P, z, u, ld_zu, a);
   if (tma_ok && variant == 6) return ekf_tma_launch<256, 2>(ctx, st, count, ld, x, P, z, u, ld_zu, a);
   if (tma_ok && variant == 7) return ekf_tma_launch<256, 3>(ctx, st, count, ld, x, P, z, u, ld_zu, a);
   switch (variant) {
     case 1:
-      crb_ekf_step_kernel<256, 4><<<crb_grid_for(count, 256), 256, 0, st>>>(count, ld, x, P, z, u,
+      crb_ekf_step_kernel<256, 4, 1><<<crb_grid_for(count, 256), 256, 0, st>>>(count, ld, x, P, z, u,
                                                                             ld_zu, n_steps, a);
       break;
     case 2:
-      crb_ekf_step_kernel<128, 8><<<crb_grid_for(count, 128), 128, 0, st>>>(count, ld, x, P, z, u,
+      crb_ekf_step_kernel<128, 8, 1><<<crb_grid_for(count, 128), 128, 0, st>>>(count, ld, x, P, z, u,
                                                                             ld_zu, n_steps, a);
       break;
     case 3:
-      crb_ekf_step_kernel<512, 2><<<crb_grid_for(count, 512), 512, 0, st>>>(count, ld, x, P, z, u,
+      crb_ekf_step_kernel<512, 2, 1><<<crb_grid_for(count, 512), 512, 0, st>>>(count, ld, x, P, z, u,
                                                                             ld_zu, n_steps, a);
       break;
     default:
-      CRB_CUDA(crb_launch_pdl(crb_ekf_step_kernel<256, 3>, (unsigned)crb_grid_for(count, 256), 256u, st,
-                              count, ld, x, P, z, u, ld_zu, n_steps, a));
+      if (pair_ok)
+        CRB_CUDA(crb_launch_pdl(crb_ekf_step_kernel<128, 4, 2>, (unsigned)crb_grid_for(count / 2, 128), 128u, st,
+                                count, ld, x, P, z, u, ld_zu, n_steps, a));
+      else
+        CRB_CUDA(crb_launch_pdl(crb_ekf_step_kernel<256, 3, 1>, (unsigned)crb_grid_for(count, 256), 256u, st,
+                                count, ld, x, P, z, u, ld_zu, n_steps, a));
   }
   CRB_CUDA(cudaGetLastError());
   ctx->launches++;

@@ -47,3 +47,48 @@ extern "C" int crb_probe_fp32_peak(crb_ctx* ctx, double* tflops_out) {
   *tflops_out = best;
   return CRB_OK;
 }
+
+// crb_probe_ekf_pattern: the access pattern of the EKF step's default form (crb_ekf_step_kernel<128, 4, 2> in
+// crb_ekf.cu: two agents per thread, 8-byte streaming loads and stores of the same 24 / 20 SoA fields, PDL, same
+// launch shape) with trivial arithmetic, the ceiling for that pattern (scripts/ekf_ceiling.py).  Every state
+// field gets (z0 + z1) + (u0 + u1) of its agent added, in place.
+__global__ void __launch_bounds__(128, 4)
+crb_probe_ekf_pattern_kernel(int64_t count, float* __restrict__ x, float* __restrict__ P,
+                             const float* __restrict__ z, const float* __restrict__ u) {
+  const int64_t i = 2 * ((int64_t)blockIdx.x * blockDim.x + threadIdx.x);
+  if (i >= count) return;
+  const int64_t ld = count;
+  crb_pdl_launch_dependents();
+  crb_pdl_wait();
+  float2 xs[4], Ps[16];
+#pragma unroll
+  for (int f = 0; f < 4; ++f) xs[f] = __ldcs(reinterpret_cast<const float2*>(x + f * ld + i));
+#pragma unroll
+  for (int f = 0; f < 16; ++f) Ps[f] = __ldcs(reinterpret_cast<const float2*>(P + f * ld + i));
+  const float2 z0 = __ldcs(reinterpret_cast<const float2*>(z + i));
+  const float2 z1 = __ldcs(reinterpret_cast<const float2*>(z + ld + i));
+  const float2 u0 = __ldcs(reinterpret_cast<const float2*>(u + i));
+  const float2 u1 = __ldcs(reinterpret_cast<const float2*>(u + ld + i));
+  const float sx = (z0.x + z1.x) + (u0.x + u1.x), sy = (z0.y + z1.y) + (u0.y + u1.y);
+#pragma unroll
+  for (int f = 0; f < 4; ++f)
+    __stcs(reinterpret_cast<float2*>(x + f * ld + i), make_float2(xs[f].x + sx, xs[f].y + sy));
+#pragma unroll
+  for (int f = 0; f < 16; ++f)
+    __stcs(reinterpret_cast<float2*>(P + f * ld + i), make_float2(Ps[f].x + sx, Ps[f].y + sy));
+}
+
+extern "C" int crb_probe_ekf_pattern(crb_ctx* ctx, int64_t n, float* x, float* P, const float* z,
+                                     const float* u) {
+  CRB_REQUIRE(ctx != nullptr, "ctx is NULL");
+  CRB_DEVICE_GUARD(ctx);
+  CRB_REQUIRE(n >= 0 && n % 2 == 0, "n < 0 or odd");
+  if (n == 0) return CRB_OK;
+  CRB_REQUIRE(x && P && z && u, "NULL array");
+  CRB_REQUIRE((((uintptr_t)x | (uintptr_t)P | (uintptr_t)z | (uintptr_t)u) & 7) == 0,
+              "arrays not 8-byte aligned");
+  CRB_CUDA(crb_launch_pdl(crb_probe_ekf_pattern_kernel, (unsigned)crb_grid_for(n / 2, 128), 128u, ctx->stream, n,
+                          x, P, z, u));
+  ctx->launches++;
+  return CRB_OK;
+}

@@ -610,6 +610,16 @@ class Engine:
         check(self.lib.crb_probe_fp32_peak(self.ctx, C.byref(v)), "crb_probe_fp32_peak")
         return float(v.value)
 
+    def probe_ekf_pattern(self, x, P, z, u) -> None:
+        """One launch of the EKF step's access pattern with trivial arithmetic (crb_probe.cu), in place on
+        x [4,n] and P [16,n]; z, u [2,n].  CUDA tensors."""
+        n = int(x.shape[-1])
+        _shape(x, 4, n, "x"); _shape(P, 16, n, "P"); _shape(z, 2, n, "z"); _shape(u, 2, n, "u")
+        check(self.lib.crb_probe_ekf_pattern(
+            self.ctx, n, _ptr(x, np.float32, device=True, name="x"), _ptr(P, np.float32, device=True, name="P"),
+            _ptr(z, np.float32, device=True, name="z"), _ptr(u, np.float32, device=True, name="u")),
+            "crb_probe_ekf_pattern")
+
     # ---- stats ------------------------------------------------------------------------------------
     def stats_reduce(self, values, status=None, iters=None, i0: int = 0, out=None):
         """Per-GPU summary of a per-agent f32 array -> float64 CUDA tensor of CRB_STATS_LEN."""

@@ -531,6 +531,12 @@ int crb_stats_reduce(crb_ctx* ctx, int64_t n, int64_t i0, const float* values,
 /* Non-tensor binary32 FMA rate of the context's device at its current clocks, in TFLOP/s (best of 5 launches of
  * a register-only FFMA kernel, synchronous).  The denominator of the MPC / LQR roofline fractions. */
 int crb_probe_fp32_peak(crb_ctx* ctx, double* tflops_out);
+/* One launch, enqueued on the context's stream, of a kernel with the memory access pattern of
+ * crb_ekf_step_batched (same arrays, layout, access width and launch shape) and trivial arithmetic: every field
+ * of x and P gets (z[0] + z[1]) + (u[0] + u[1]) of its agent added, in place (device pointers, n_steps = 1; n
+ * even and the arrays 8-byte aligned, as the EKF step's two-agent form needs).  Timed next to
+ * the EKF step it is the bandwidth ceiling of that access pattern (scripts/ekf_ceiling.py). */
+int crb_probe_ekf_pattern(crb_ctx* ctx, int64_t n, float* x, float* P, const float* z, const float* u);
 
 #ifdef __cplusplus
 }

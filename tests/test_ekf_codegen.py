@@ -1,0 +1,59 @@
+"""EKF step code generation and the access-pattern probe.
+CPU: every EKF kernel the launcher can select compiles for sm_90a, with the build's flags, without spilling to
+local memory.  H100: the two-agent form of the step (even n, 8-byte aligned arrays) gives the same bits as the
+one-agent form, over several steps per launch; crb_probe_ekf_pattern does what include/crb.h says it does."""
+import os
+import subprocess
+
+import numpy as np
+import pytest
+
+import __graft_entry__ as G
+from cpprobotics_b200 import synth
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def test_ekf_kernels_do_not_spill(tmp_path):
+    if not os.path.exists(G.NVCC):
+        pytest.skip("no nvcc")
+    out = subprocess.run([G.NVCC] + G.NVCC_FLAGS + ["-c", os.path.join(G.CSRC, "crb_ekf.cu"),
+                                                    "-o", str(tmp_path / "ekf.o")],
+                         capture_output=True, text=True, check=True).stderr
+    blocks = out.split("Compiling entry function")[1:]
+    kernels = {b.splitlines()[0].split("'")[1]: b for b in blocks if "crb_ekf_step" in b.splitlines()[0]}
+    # the direct kernel at <128,4,2> and <256,3,1> (default), <256,4,1>, <128,8,1>, <512,2,1>, and the TMA-staged
+    # one at 4 shapes
+    assert len(kernels) == 9, sorted(kernels)
+    for name, b in kernels.items():
+        assert "0 bytes spill stores, 0 bytes spill loads" in b, (name, b)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("n_steps", [1, 3])
+def test_ekf_two_agent_form_is_bitwise_the_one_agent_form(engine, n_steps):
+    """n = 20_001 is odd, so its launch takes the one-agent kernel; its first 20_000 agents run again as an even
+    batch, which takes the two-agent kernel.  Agents are independent, so the bits must agree."""
+    import torch
+    n = 20_001
+    x, P, z, u = synth.ekf_inputs(n, n_steps=n_steps)
+    odd = [torch.from_numpy(a).cuda() for a in (x, P, z, u)]
+    even = [torch.from_numpy(np.ascontiguousarray(a[:, : n - 1])).cuda() for a in (x, P, z, u)]
+    engine.ekf_estimation(*odd, n_steps=n_steps)
+    engine.ekf_estimation(*even, n_steps=n_steps)
+    torch.cuda.synchronize()
+    assert np.array_equal(odd[0].cpu().numpy()[:, : n - 1], even[0].cpu().numpy())
+    assert np.array_equal(odd[1].cpu().numpy()[:, : n - 1], even[1].cpu().numpy())
+
+
+@pytest.mark.gpu
+def test_ekf_pattern_probe_adds_the_agent_sum(engine):
+    import torch
+    n = 100_002
+    x, P, z, u = synth.ekf_inputs(n)
+    t = [torch.from_numpy(a).cuda() for a in (x, P, z, u)]
+    engine.probe_ekf_pattern(*t)
+    torch.cuda.synchronize()
+    s = (z[0] + z[1]) + (u[0] + u[1])
+    assert np.array_equal(t[0].cpu().numpy(), x + s) and np.array_equal(t[1].cpu().numpy(), P + s)
+    assert np.array_equal(t[2].cpu().numpy(), z) and np.array_equal(t[3].cpu().numpy(), u)
