@@ -174,42 +174,24 @@ __device__ __forceinline__ void st_stream(float* p, float v) { __stcs(p, v); }
 // sincosf.h, s_sincosf_data.c).  On x86-64 hosts with FMA (every server CPU of the last decade) glibc's ifunc
 // picks the build of those files compiled with -mfma, in which each a + b * c of the source is ONE fused
 // operation: that is what is restated here with explicit fma(), operation for operation, and the GPU's FP64
-// pipe (IEEE DFMA / DMUL) reproduces it bit for bit.  Checked against the host libm on 3.2e8 floats in
-// |y| < 120 (oracle/crb_oracle.c:crb_oracle_libm_sincosf, tests/test_oracle_ekf.py): sin AND cos identical on
-// every one of them.  (On a host without FMA, glibc's plain build differs from this on 2e-8 of the inputs, by
-// one ulp.)  |y| >= 120 (glibc's table-driven reduce_large) is not restated: CUDA's sincosf is used there (no
-// BASELINE workload comes near it).  17 FP64 operations + 3 conversions per call.
-static __device__ __noinline__ float2 crb_sincosf_large(float y) {  // by value: no address-taken locals at the call site
-  float s, c;
-  sincosf(y, &s, &c);
-  return make_float2(s, c);
-}
+// pipe (IEEE DFMA / DMUL) reproduces it bit for bit.  |y| >= 120 takes glibc's reduce_large: an exact 2.62
+// fixed-point remainder from three 32x32-bit integer products with a window of 2/pi, converted to binary64 and
+// scaled by pi/2^62, then the same polynomial; integer and binary64 work only, so it is reproduced bit for bit
+// too.  The C restatement (oracle/crb_oracle.c:crb_oracle_libm_sincosf) equals the host libm, sin AND cos, on
+// every finite float with |y| >= 120 and on a dense sample below (tests/test_oracle_ekf.py), and this function
+// equals the C restatement on all 2^32 bit patterns on the device (tests/test_ekf_edges.py).  (On a host without
+// FMA, glibc's plain build differs from this on 2e-8 of the inputs, by one ulp.)  Inf and NaN give NaN.  17 FP64
+// operations + 3 conversions per call below 120.
 // x with the sign flipped when neg != 0 (x * -1.0 without occupying the FP64 pipe)
 __device__ __forceinline__ double crb_flip(double x, int neg) {
   return __hiloint2double(__double2hiint(x) ^ (neg ? (int)0x80000000 : 0), __double2loint(x));
 }
-__device__ __forceinline__ void crb_sincosf_libm(float y, float& sn, float& cs) {
-  const unsigned top = (__float_as_uint(y) >> 20) & 0x7ffu;
-  if (top >= 0x42fu) {  // |y| >= 120, inf, nan: out of line (CUDA's Payne-Hanek path is long)
-    const float2 sc = crb_sincosf_large(y);
-    sn = sc.x;
-    cs = sc.y;
-    return;
-  }
-  double x = (double)y;
-  int n = 0;
-  if (top >= 0x3f4u) {  // |y| >= pi/4 (abstop12(0x1.921FB6p-1f) = 0x3f4): reduce_fast
-    const double r = x * 0x1.45F306DC9C883p+23;
-    n = ((int)r + 0x800000) >> 24;
-    x = fma(-(double)n, 0x1.921FB54442D18p0, x);
-  } else if (top < 0x398u) {  // |y| < 2^-12
-    sn = y;
-    cs = 1.0f;
-    return;
-  }
+// sinf_poly for both results on the reduced argument x (|x| <= pi/4): m picks the signs (sign table and the
+// negated cosine table), n the polynomial (sinf takes the sine polynomial for even n, cosf for odd n)
+__device__ __forceinline__ void crb_sincosf_poly(double x, int n, int m, float& sn, float& cs) {
   const double x2 = x * x;
-  const int neg_s = (n + 1) & 2;  // sign[n & 3] = {1, -1, -1, 1}
-  const int neg_c = n & 2;        // second table entry: cosine coefficients negated
+  const int neg_s = (m + 1) & 2;  // sign[m & 3] = {1, -1, -1, 1}
+  const int neg_c = m & 2;        // second table entry: cosine coefficients negated
   const double xs = crb_flip(x, neg_s);
   // sine polynomial on xs (its coefficients are the same in both table entries)
   const double x3 = xs * x2;
@@ -229,6 +211,53 @@ __device__ __forceinline__ void crb_sincosf_libm(float y, float& sn, float& cs) 
   // sinf uses the sine polynomial for even n, cosf for odd n (and vice versa)
   sn = (n & 1) ? pc : ps;
   cs = (n & 1) ? ps : pc;
+}
+// 2/pi in 8-bit steps (glibc's __inv_pio4): word k holds bits [8k - 24, 8k + 8) of its binary fraction
+static __device__ __constant__ const uint32_t crb_inv_pio4[24] = {
+    0xa2,       0xa2f9,     0xa2f983,   0xa2f9836e, 0xf9836e4e, 0x836e4e44, 0x6e4e4415, 0x4e441529,
+    0x441529fc, 0x1529fc27, 0x29fc2757, 0xfc2757d1, 0x2757d1f5, 0x57d1f534, 0xd1f534dd, 0xf534ddc0,
+    0x34ddc0db, 0xddc0db62, 0xc0db6295, 0xdb629599, 0x6295993c, 0x95993c43, 0x993c4390, 0x3c439041};
+// glibc's reduce_large for |y| >= 120, out of line so that the hot paths (whose arguments stay far below 120) keep
+// their registers: |y| = (n + r / 2^62) * pi/2 in exact 2.62 fixed point from the 24-bit significand and a 96-bit
+// window of 2/pi chosen by the exponent.  Returns r * pi/2^62 (|.| <= pi/4) with n in .y's low word and the sign
+// quadrant n + signbit(y) in its high word; inf and nan return y - y (nan), which the polynomial passes on.
+static __device__ __noinline__ double2 crb_sincosf_reduce_large(float y) {  // by value: no address-taken locals
+  uint32_t xi = __float_as_uint(y);
+  if ((xi & 0x7fffffffu) >= 0x7f800000u) return make_double2((double)__fsub_rn(y, y), 0.0);
+  const uint32_t* arr = &crb_inv_pio4[(xi >> 26) & 15];
+  const int sign = (int)(xi >> 31);
+  xi = ((xi & 0xffffffu) | 0x800000u) << ((xi >> 23) & 7);
+  uint64_t res0 = (uint64_t)(xi * arr[0]);  // only the low 32 bits of the top product matter
+  const uint64_t res1 = (uint64_t)xi * arr[4];
+  const uint64_t res2 = (uint64_t)xi * arr[8];
+  res0 = ((res2 >> 32) | (res0 << 32)) + res1;
+  const uint64_t n = (res0 + (1ull << 61)) >> 62;
+  res0 -= n << 62;
+  const double x = __dmul_rn(__ll2double_rn((long long)res0), 0x1.921FB54442D18p-62);
+  return make_double2(x, __hiloint2double((int)n + sign, (int)n));
+}
+__device__ __forceinline__ void crb_sincosf_libm(float y, float& sn, float& cs) {
+  const unsigned top = (__float_as_uint(y) >> 20) & 0x7ffu;
+  double x = (double)y;
+  int n = 0, m;
+  if (top >= 0x42fu) {  // |y| >= 120, inf, nan
+    const double2 r = crb_sincosf_reduce_large(y);
+    x = r.x;
+    n = __double2loint(r.y);
+    m = __double2hiint(r.y);
+  } else {
+    if (top >= 0x3f4u) {  // |y| >= pi/4 (abstop12(0x1.921FB6p-1f) = 0x3f4): reduce_fast
+      const double r = x * 0x1.45F306DC9C883p+23;
+      n = ((int)r + 0x800000) >> 24;
+      x = fma(-(double)n, 0x1.921FB54442D18p0, x);
+    } else if (top < 0x398u) {  // |y| < 2^-12
+      sn = y;
+      cs = 1.0f;
+      return;
+    }
+    m = n;
+  }
+  crb_sincosf_poly(x, n, m, sn, cs);
 }
 
 // ---- tanf with the HOST libm's bits ---------------------------------------------------------------------

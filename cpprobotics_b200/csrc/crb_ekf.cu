@@ -11,12 +11,15 @@
 // back to back (independent, ~96 B in flight per thread) and the 4x4 algebra lives in registers.
 //
 // Arithmetic: the kernel reproduces the dense Eigen evaluation of the reference entry for entry.
-// jF is identity plus four entries and jH is a row selector; multiplying by an exact 0/1 and adding
-// an exact 0 is exact in IEEE arithmetic, so only the non-trivial terms are evaluated, in the same
-// (sequential-k) order and with separate multiply and add (this TU is compiled with -fmad=false; the
-// kernel is memory-bound, FMUL+FADD instead of FFMA costs nothing).  With that, results differ from
-// the CPU restatement only where glibc's FMA build of sinf/cosf rounds differently from the plain binary64
-// evaluation in crb_sincosf_libm (2e-8 of the inputs).
+// jF is identity plus four entries and jH is a row selector; for finite operands, multiplying by an exact
+// 0/1 and adding the resulting zero leaves a nonzero sum unchanged, so only the non-trivial terms are
+// evaluated, in the same (sequential-k) order and with separate multiply and add (this TU is compiled with
+// -fmad=false; the kernel is memory-bound, FMUL+FADD instead of FFMA costs nothing).  sin / cos carry the
+// host libm's bits at every argument (crb_sincosf_libm), so every result is bit-identical to the CPU
+// restatement on a host whose glibc runs its FMA build, with two exceptions the skipped terms cause: an
+// exact zero may have the other sign (a dense sum adds +0 terms, turning -0 into +0), and in an agent with
+// an infinite input the dense 0 * inf makes NaN of every entry, also of those this kernel computes without
+// that input (tests/test_ekf_edges.py).
 #include <stdint.h>
 #include <stdlib.h>
 

@@ -573,40 +573,70 @@ void crb_oracle_dlqr_batched(int64_t n, int nx, int nu, const float* A, const fl
 
 
 /* ---- glibc's sinf / cosf, restated (what the CUDA kernels' crb_sincosf_libm executes) -------------------
- * glibc >= 2.28: sysdeps/ieee754/flt-32/s_sinf.c, s_cosf.c, sincosf.h (reduce_fast, sinf_poly),
- * s_sincosf_data.c (__sincosf_table).  Third-party code that is not under /root/reference: the reference
- * reaches it through std::sin / std::cos on floats (src/extended_kalman_filter.cpp:29-33, :41-45;
- * src/particle_filter.cpp:33-37).  Everything is binary64 multiply / add / fused multiply-add with one final
- * rounding to float, so the GPU's FP64 pipe can reproduce it.  Pinned by tests/test_oracle_ekf.py against THIS host's libm (the
- * oracle's EKF / PF restatements keep calling libm itself, like the reference).  |y| >= 120 (reduce_large) is
- * not restated: libm is called. */
+ * glibc >= 2.28: sysdeps/ieee754/flt-32/s_sinf.c, s_cosf.c, sincosf.h (reduce_fast, reduce_large, sinf_poly),
+ * s_sincosf_data.c (__sincosf_table).  Third-party code that the reference reaches through std::sin / std::cos on
+ * floats (src/extended_kalman_filter.cpp:29-33, :41-45; src/particle_filter.cpp:33-37).  Every finite argument is
+ * restated, libm is never called: below 120 binary64 multiply / add / fused multiply-add with one final rounding to
+ * float, from 120 on the same polynomial after an exact integer reduction.  The GPU reproduces both.  Pinned by
+ * tests/test_oracle_ekf.py against THIS host's libm on every finite float with |y| >= 120 and a dense sample below
+ * (the oracle's EKF / PF restatements keep calling libm itself, like the reference).  Inf and NaN give NaN. */
 static uint32_t ls_abstop12(float x) {
   uint32_t u;
   memcpy(&u, &x, 4);
   return (u >> 20) & 0x7ff;
 }
+
+/* 2/pi in 8-bit steps: word k holds bits [8k - 24, 8k + 8) of its binary fraction (k < 3: the leading bits only).
+ * tests/test_oracle_ekf.py regenerates the words from Machin's formula. */
+const uint32_t crb_oracle_inv_pio4[24] = {
+    0xa2,       0xa2f9,     0xa2f983,   0xa2f9836e, 0xf9836e4e, 0x836e4e44, 0x6e4e4415, 0x4e441529,
+    0x441529fc, 0x1529fc27, 0x29fc2757, 0xfc2757d1, 0x2757d1f5, 0x57d1f534, 0xd1f534dd, 0xf534ddc0,
+    0x34ddc0db, 0xddc0db62, 0xc0db6295, 0xdb629599, 0x6295993c, 0x95993c43, 0x993c4390, 0x3c439041};
+
+/* reduce_large: |y| = (n + r / 2^62) * pi/2 computed exactly in 2.62 fixed point from the 24-bit significand and a
+ * 96-bit window of 2/pi chosen by the exponent (the sign bit is ignored).  Returns r * pi/2^62, |result| <= pi/4. */
+static double ls_reduce_large(uint32_t xi, int* np) {
+  const uint32_t* arr = &crb_oracle_inv_pio4[(xi >> 26) & 15];
+  const int shift = (xi >> 23) & 7;
+  xi = ((xi & 0xffffff) | 0x800000) << shift;
+  uint64_t res0 = (uint32_t)(xi * arr[0]); /* only the low 32 bits of the top product matter */
+  const uint64_t res1 = (uint64_t)xi * arr[4];
+  const uint64_t res2 = (uint64_t)xi * arr[8];
+  res0 = (res2 >> 32) | (res0 << 32);
+  res0 += res1;
+  const uint64_t n = (res0 + (1ULL << 61)) >> 62;
+  res0 -= n << 62;
+  *np = (int)n;
+  return (double)(int64_t)res0 * 0x1.921FB54442D18p-62;
+}
+
 void crb_oracle_libm_sincosf(float y, float* sn, float* cs) {
   /* the -mfma build of glibc's sources (what the ifunc selects on hosts with FMA): every a + b * c is fused */
   const uint32_t top = ls_abstop12(y);
-  if (top >= 0x42f) { /* |y| >= 120, inf, nan */
-    *sn = sinf(y);
-    *cs = cosf(y);
+  double x = (double)y;
+  int n = 0, m = 0; /* m: the quadrant that picks the signs, n: the one that picks the polynomial */
+  if (top >= 0x7f8) { /* inf, nan */
+    *sn = *cs = y - y;
     return;
   }
-  double x = (double)y;
-  int n = 0;
-  if (top >= 0x3f4) { /* |y| >= pi/4: reduce_fast, hpi_inv prescaled by 2^24 */
+  if (top >= 0x42f) { /* |y| >= 120: reduce_large, the argument's sign joins the quadrant */
+    uint32_t xi;
+    memcpy(&xi, &y, 4);
+    x = ls_reduce_large(xi, &n);
+    m = n + (int)(xi >> 31);
+  } else if (top >= 0x3f4) { /* |y| >= pi/4: reduce_fast, hpi_inv prescaled by 2^24 */
     const double r = x * 0x1.45F306DC9C883p+23;
     n = ((int32_t)r + 0x800000) >> 24;
     x = fma(-(double)n, 0x1.921FB54442D18p0, x);
+    m = n;
   } else if (top < 0x398) { /* |y| < 2^-12 */
     *sn = y;
     *cs = 1.0f;
     return;
   }
   const double x2 = x * x;
-  const double sgn = ((n + 1) & 2) ? -1.0 : 1.0; /* sign[n & 3] = {1, -1, -1, 1} */
-  const double q = (n & 2) ? -1.0 : 1.0;         /* __sincosf_table[1]: cosine coefficients negated */
+  const double sgn = ((m + 1) & 2) ? -1.0 : 1.0; /* sign[m & 3] = {1, -1, -1, 1} */
+  const double q = (m & 2) ? -1.0 : 1.0;         /* __sincosf_table[1]: cosine coefficients negated */
   const double xs = x * sgn;
   const double x3 = xs * x2;
   const double s1 = fma(x2, -0x1.994eb3774cf24p-13, 0x1.1107605230bc4p-7);
@@ -627,7 +657,10 @@ void crb_oracle_libm_sincosf(float y, float* sn, float* cs) {
  * the restatement and the host libm disagree; out[0] = sin mismatches, out[1] = cos mismatches */
 void crb_oracle_libm_sincosf_census(uint32_t lo_bits, uint32_t hi_bits, uint32_t step, int64_t* out) {
   int64_t bs = 0, bc = 0;
-  for (uint64_t u = lo_bits; u < hi_bits; u += step) {
+#ifdef _OPENMP
+#pragma omp parallel for reduction(+ : bs, bc) schedule(static, 1 << 14)
+#endif
+  for (int64_t u = lo_bits; u < (int64_t)hi_bits; u += step) {
     const uint32_t b = (uint32_t)u;
     float f;
     memcpy(&f, &b, 4);
@@ -643,4 +676,27 @@ void crb_oracle_libm_sincosf_census(uint32_t lo_bits, uint32_t hi_bits, uint32_t
   }
   out[0] = bs;
   out[1] = bc;
+}
+
+/* the device's sin / cos of every float in [lo_bits, hi_bits), both signs (got[4k + 2sg] = sin and got[4k + 2sg + 1]
+ * = cos of bit pattern lo_bits + k with sign sg), against the restatement; NaN matches NaN.  Returns the number of
+ * arguments where either differs. */
+int64_t crb_oracle_libm_sincosf_check(uint32_t lo_bits, uint32_t hi_bits, const float* got) {
+  int64_t bad = 0;
+#ifdef _OPENMP
+#pragma omp parallel for reduction(+ : bad) schedule(static, 1 << 16)
+#endif
+  for (int64_t u = lo_bits; u < (int64_t)hi_bits; ++u) {
+    for (int sg = 0; sg < 2; ++sg) {
+      const uint32_t b = (uint32_t)u | (sg ? 0x80000000u : 0u);
+      float y, ms, mc;
+      memcpy(&y, &b, 4);
+      crb_oracle_libm_sincosf(y, &ms, &mc);
+      const float* g = got + 4 * (u - (int64_t)lo_bits) + 2 * sg;
+      const int s_ok = memcmp(&g[0], &ms, 4) == 0 || (isnan(g[0]) && isnan(ms));
+      const int c_ok = memcmp(&g[1], &mc, 4) == 0 || (isnan(g[1]) && isnan(mc));
+      bad += !(s_ok && c_ok);
+    }
+  }
+  return bad;
 }

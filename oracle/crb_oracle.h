@@ -74,9 +74,11 @@ int64_t crb_oracle_check_const_division(float d, uint32_t lo_bits, uint32_t hi_b
 int64_t crb_oracle_check_ff_product(double pre, uint32_t lo_bits, uint32_t hi_bits);
 int64_t crb_oracle_check_resample_id_rcp(int64_t n_max, const int64_t* ns, int n_ns, int64_t* evaluated);
 
-/* glibc's sinf / cosf restated (binary64 polynomial, what the kernels' crb_sincosf_libm executes) */
+/* glibc's sinf / cosf restated for every argument (what the kernels' crb_sincosf_libm executes) */
+extern const uint32_t crb_oracle_inv_pio4[24];
 void crb_oracle_libm_sincosf(float y, float* sn, float* cs);
 void crb_oracle_libm_sincosf_census(uint32_t lo_bits, uint32_t hi_bits, uint32_t step, int64_t* out);
+int64_t crb_oracle_libm_sincosf_check(uint32_t lo_bits, uint32_t hi_bits, const float* got);
 #ifdef __cplusplus
 }
 #endif

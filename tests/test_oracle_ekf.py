@@ -165,7 +165,55 @@ def test_restated_glibc_sincosf_carries_this_hosts_libm_bits():
     L.crb_oracle_libm_sincosf_census(int(lo), int(hi), 1, out.ctypes.data)
     assert out[0] <= 4 and out[1] <= 4, out
     s, c = C.c_float(), C.c_float()
-    for y, ws, wc in [(0.0, 0.0, 1.0), (1e-5, 1e-5, 1.0), (np.inf, np.nan, np.nan)]:
+    for y, ws, wc in [(0.0, 0.0, 1.0), (1e-5, 1e-5, 1.0), (np.inf, np.nan, np.nan), (-np.inf, np.nan, np.nan),
+                      (np.nan, np.nan, np.nan)]:
         L.crb_oracle_libm_sincosf(C.c_float(y), C.byref(s), C.byref(c))
         assert (np.isnan(s.value) and np.isnan(ws)) or s.value == np.float32(ws)
         assert (np.isnan(c.value) and np.isnan(wc)) or c.value == np.float32(wc)
+
+
+def test_restated_sincosf_beyond_120_is_this_hosts_libm_on_every_float():
+    """From |y| = 120 on, glibc reduces with reduce_large (integer products with a window of 2/pi) instead of the
+    binary64 multiply-subtract; the restatement does the same, and must give this host's sinf and cosf on every one
+    of the 2,032,140,288 finite floats with |y| >= 120, both signs (about 5 s on 8 threads).  On a host without FMA,
+    glibc's plain build of the shared polynomial differs by an ulp on a few arguments in 1e8."""
+    import ctypes as C
+    L = O.lib()
+    L.crb_oracle_libm_sincosf_census.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]
+    out = np.zeros(2, np.int64)
+    L.crb_oracle_libm_sincosf_census(0x42F00000, 0x7F800000, 1, out.ctypes.data)
+    n = 2 * (0x7F800000 - 0x42F00000)
+    assert n == 2_032_140_288
+    has_fma = " fma " in open("/proc/cpuinfo").read()
+    assert (out == 0).all() if has_fma else (out[0] <= 2e-7 * n and out[1] <= 2e-7 * n), out
+
+
+def _two_over_pi_words():
+    """glibc's __inv_pio4 from first principles: pi by Machin's formula in integers, then word k = the bits
+    [8k - 24, 8k + 8) of the binary fraction of 2/pi."""
+    prec = 320                                   # bits; the words need 200
+    one = 1 << (prec + 16)
+
+    def arctan_inv(q):                           # arctan(1/q) * one
+        s, t, k, sign = 0, one // q, 1, 1
+        while t:
+            s += sign * (t // k)
+            t //= q * q
+            k += 2
+            sign = -sign
+        return s
+    pi = 16 * arctan_inv(5) - 4 * arctan_inv(239)   # pi * one, good to ~prec bits
+    frac = (2 * one << prec) // pi                  # 2/pi * 2^prec
+    return [(frac >> (prec - 8 * (k + 1))) & 0xFFFFFFFF for k in range(24)]
+
+
+def test_reduce_large_table_is_two_over_pi():
+    """The 2/pi words of the restated reduce_large, in the checker and in the kernels' header, regenerated here."""
+    import ctypes as C
+    import re
+    want = _two_over_pi_words()
+    assert want[:6] == [0xa2, 0xa2f9, 0xa2f983, 0xa2f9836e, 0xf9836e4e, 0x836e4e44]
+    assert list((C.c_uint32 * 24).in_dll(O.lib(), "crb_oracle_inv_pio4")) == want
+    src = open(os.path.join(os.path.dirname(GOLD), "..", "cpprobotics_b200", "csrc", "crb_common.cuh")).read()
+    body = re.search(r"crb_inv_pio4\[24\] = \{([^}]*)\}", src).group(1)
+    assert [int(w, 16) for w in re.findall(r"0x[0-9a-f]+", body)] == want

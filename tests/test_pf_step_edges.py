@@ -26,15 +26,16 @@ def _assert_pf_parity(px_got, pw_got, px_want, pw_want, lm, sigma2=0.01):
     """Per-particle relative 1e-5 on w.
 
     The kernels evaluate sin/cos with glibc's own binary64 algorithm (crb_sincosf_libm), so the predicted
-    positions carry the HOST libm's bits: they must be IDENTICAL to the oracle's, except on the ~2e-8 of the
-    arguments where glibc's FMA build rounds an intermediate differently (then 1 ulp).  On every particle with
+    positions carry the HOST libm's bits: they must be IDENTICAL to the oracle's where glibc runs its FMA build (the
+    one restated); without FMA its sinf / cosf round differently on ~2e-8 of the arguments (then 1 ulp).  On every particle with
     identical positions the weight must agree to 1e-5 RELATIVE (w > 1e-30; the kernel's single fused
     exponential differs from the reference's eight rounded factors by <= ~1e-6).  The few particles whose
     position is an ulp off get the condition-number gate (one ulp of position is 3e-5 of w per landmark)."""
     same = (px_got == px_want).all(axis=0)
     n = same.size
     n_off = int((~same).sum())
-    assert n_off <= max(2, int(4e-6 * n)), f"{n_off} of {n} predicted positions differ from the host libm path"
+    fma_host = " fma " in open("/proc/cpuinfo").read()
+    assert n_off <= (0 if fma_host else max(2, int(4e-6 * n))), f"{n_off} of {n} predicted positions differ from the host libm path"
     assert np.abs(px_got - px_want).max() <= 1e-6 * max(1.0, np.abs(px_want).max())
     big = same & (pw_want > 1e-30)
     rel = np.abs(pw_got[big].astype(np.float64) - pw_want[big]) / pw_want[big]
