@@ -39,6 +39,15 @@ CRB_SLP_MAX_NS = 1 << 20
 CRB_SLP_MAX_STATES = 65536
 CRB_SLP_OK = 0
 CRB_SLP_OUT_OF_RANGE = 1
+CRB_GRID_MAX_SIDE = 32768
+CRB_GRID_MAX_CELLS = 1 << 24
+CRB_GRID_WS_BUDGET = 1 << 32
+CRB_GRID_ASTAR = 0
+CRB_GRID_DIJKSTRA = 1
+CRB_GRID_FOUND = 0
+CRB_GRID_NO_PATH = 1
+CRB_GRID_START_OUTSIDE = 2
+CRB_GRID_BAD_POINT = 3
 
 c_f32p = C.POINTER(C.c_float)
 c_i32p = C.POINTER(C.c_int32)
@@ -76,6 +85,10 @@ class MptgParams(C.Structure):
 
 class SlpSampler(C.Structure):
     _fields_ = [("kind", C.c_int32), ("nxy", C.c_int32), ("nh", C.c_int32), ("ns", C.c_int32), ("d", C.c_int32)]
+
+
+class GridBox(C.Structure):
+    _fields_ = [("min_x", C.c_int32), ("min_y", C.c_int32), ("max_x", C.c_int32), ("max_y", C.c_int32)]
 
 
 # name -> (restype, argtypes); every symbol include/crb.h declares
@@ -159,6 +172,13 @@ PROTOTYPES = {
                                                 C.c_void_p, C.c_void_p, C.c_void_p]),
     "crb_slp_search_nearest_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int,
                                                  C.c_void_p, C.c_void_p, C.c_void_p]),
+    "crb_grid_box_of_obstacles": (C.c_int, [C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.POINTER(GridBox)]),
+    "crb_grid_obstacle_map": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_float,
+                                        C.POINTER(GridBox), C.c_void_p]),
+    "crb_grid_plan_batched": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(GridBox), C.c_void_p, C.c_float, C.c_int64,
+                                        C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p]),
+    "crb_grid_plan_slots": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(GridBox), C.c_int64, C.POINTER(C.c_int64)]),
     "crb_stats_reduce": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p]),
     "crb_probe_fp32_peak": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),

@@ -27,6 +27,9 @@ struct crb_ctx {
   // MPC solver workspace (two trajectory buffers + gains per problem) for the device-pointer entry
   void* mpc_ws;
   size_t mpc_ws_cap;
+  // grid planner workspace (query counter + one search slot per lane, crb_grid.cu), grown on demand
+  void* grid_ws;
+  size_t grid_ws_cap;
   void* host_scratch;  // small pinned buffer for reduction results
   // per-device function attributes already set for this context's device (a second context on another
   // device in the same process must set them again, so these are not process-global latches)

@@ -1,0 +1,460 @@
+// crb_grid.cu — grid A* and Dijkstra for many start / goal queries on one obstacle map, for sm_90a.
+//
+// Replaces calc_obstacle_map, a_star_planning and dijkstra_star_planning of src/a_star.cpp and src/dijkstra.cpp
+// (the two files differ in about 12 lines: the key, and A*'s path_cost relaxation).  Bit-exact with the reference
+// built for x86-64: every float and double operation is an explicitly rounded intrinsic, so the TU's -fmad setting
+// does not matter, and the priority queue is the libstdc++ binary heap restated step by step (push: sift-up while
+// the parent's key is greater; pop: the last entry is saved, the hole walks down to a leaf taking the right child
+// unless its key is greater than the left one's, the lone left child of an even-sized heap is taken, and the saved
+// entry sifts back up).  Ties are everywhere on a grid, and which parent a cell keeps is decided by that order.
+//
+// Mapping.
+//   crb_grid_map_kernel: one thread per cell; the obstacles are rounded to cells once per block, a tile at a time, in
+//     shared memory, and every thread of the block tests its cell against the tile.
+//   crb_grid_plan_kernel: one thread per query, running the reference's search serially (the pop order is the
+//     result, so there is nothing to split inside a query).  The kernel is persistent: each lane owns one workspace
+//     slot and takes its next query from an atomic counter, so a lane whose query ends early starts another instead
+//     of waiting for the rest of its warp.  A slot holds
+//       heap  [8 * cells + 1] 8-byte entries: float key, cell << 3 | move (every visited cell pushes at most 8)
+//       g     [cells] float, A*'s path_cost (FLT_MAX = never reached)
+//       state [cells] uint8: bit 7 visited, bit 3 the start, bits 0-2 the move that reached the cell from its parent
+//     and the parent of a cell is cell - offset[move], so no pointer or parent array is kept.
+#include <float.h>
+
+#include "crb_common.cuh"
+
+#define GRID_MAP_BLOCK 256
+#define GRID_PLAN_BLOCK 128
+
+namespace {
+
+// get_motion_model :99-108, in its order; the diagonal cost is (float)std::sqrt(2)
+__constant__ int c_mx[8] = {1, 0, -1, 0, -1, -1, 1, 1};
+__constant__ int c_my[8] = {0, 1, 0, -1, -1, 1, -1, 1};
+constexpr float kDiag = 1.41421354f;
+
+__device__ __forceinline__ float grid_nan() { return __int_as_float(0x7fc00000); }
+
+struct Entry {  // one heap element; 8-byte aligned so that an entry moves in one load and one store
+  float key;
+  uint32_t cd;  // cell << 3 | move
+};
+static_assert(sizeof(Entry) == 8, "heap entry is 8 bytes");
+
+// comp(a, b) of the reference's priority_queue: a->key > b->key
+__device__ __forceinline__ void heap_sift_up(Entry* h, int64_t hole, int64_t top, Entry v) {
+  int64_t parent = (hole - 1) / 2;
+  while (hole > top && h[parent].key > v.key) {
+    h[hole] = h[parent];
+    hole = parent;
+    parent = (hole - 1) / 2;
+  }
+  h[hole] = v;
+}
+
+__device__ __forceinline__ void heap_push(Entry* h, int64_t& len, Entry v) {
+  heap_sift_up(h, len, 0, v);
+  ++len;
+}
+
+// pop_heap + pop_back: returns the top, len shrinks by one
+__device__ __forceinline__ Entry heap_pop(Entry* h, int64_t& len) {
+  const Entry top = h[0];
+  --len;
+  if (len > 0) {
+    const Entry v = h[len];
+    int64_t hole = 0, child = 0;
+    while (child < (len - 1) / 2) {
+      child = 2 * (child + 1);
+      if (h[child].key > h[child - 1].key) --child;
+      h[hole] = h[child];
+      hole = child;
+    }
+    if ((len & 1) == 0 && child == (len - 2) / 2) {
+      child = 2 * (child + 1);
+      h[hole] = h[child - 1];
+      hole = child - 1;
+    }
+    heap_sift_up(h, hole, 0, v);
+  }
+  return top;
+}
+
+// (int)std::round(p / reso) with p / reso a float quotient and roundf; false when the result is not a finite value
+// inside the int range (the reference's conversion is undefined there)
+__device__ __forceinline__ bool grid_cell_f(float p, float reso, int& c) {
+  const float r = roundf(__fdiv_rn(p, reso));
+  if (!(r >= -2147483648.0f && r < 2147483648.0f)) return false;
+  c = __float2int_rz(r);
+  return true;
+}
+
+// (int)std::round(o * 1.0 / reso), in double
+__device__ __forceinline__ bool grid_cell_d(float o, float reso, int& c) {
+  const double r = round(__ddiv_rn((double)o, (double)reso));
+  if (!(r >= -2147483648.0 && r < 2147483648.0)) return false;
+  c = __double2int_rz(r);
+  return true;
+}
+
+}  // namespace
+
+__global__ void __launch_bounds__(GRID_MAP_BLOCK)
+crb_grid_map_kernel(int64_t n_obs, const float* __restrict__ ox, const float* __restrict__ oy, float reso, float thr,
+                    crb_grid_box box, int64_t cells, uint8_t* __restrict__ map) {
+  __shared__ int2 s_ob[GRID_MAP_BLOCK];
+  __shared__ int s_ok[GRID_MAP_BLOCK];
+  const int64_t c = (int64_t)blockIdx.x * GRID_MAP_BLOCK + threadIdx.x;
+  const int64_t H = (int64_t)box.max_y - box.min_y;
+  const int64_t x = c < cells ? box.min_x + c / H : 0, y = c < cells ? box.min_y + c % H : 0;
+  bool blocked = false;
+  for (int64_t k0 = 0; k0 < n_obs; k0 += GRID_MAP_BLOCK) {
+    const int64_t k = k0 + threadIdx.x;
+    int ix = 0, iy = 0;
+    const bool ok = k < n_obs && grid_cell_d(ox[k], reso, ix) && grid_cell_d(oy[k], reso, iy);
+    __syncthreads();  // the previous tile is no longer read
+    s_ob[threadIdx.x] = make_int2(ix, iy);
+    s_ok[threadIdx.x] = ok;
+    __syncthreads();
+    const int m = n_obs - k0 < GRID_MAP_BLOCK ? (int)(n_obs - k0) : GRID_MAP_BLOCK;
+    for (int j = 0; j < m && !blocked; ++j) {
+      if (!s_ok[j]) continue;
+      // std::sqrt(std::pow(ox - x, 2) + std::pow(oy - y, 2)) in double, narrowed to the float d; the squares of
+      // integer differences are exact
+      const double dx = (double)(s_ob[j].x - x), dy = (double)(s_ob[j].y - y);
+      const float d = __double2float_rn(__dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy))));
+      blocked = d <= thr;
+    }
+  }
+  if (c < cells) map[c] = blocked ? 1 : 0;
+}
+
+struct GridPlanArgs {
+  crb_grid_box box;
+  const uint8_t* map;
+  float reso;
+  int64_t n;
+  const float* sg;
+  int max_pts;
+  float* path;
+  int32_t* path_len;
+  float* cost;
+  int32_t* n_visited;
+  int32_t* status;
+  unsigned long long* counter;
+  char* ws;
+  size_t slot_bytes;
+  int64_t slots;
+  int64_t heap_off, g_off, state_off;  // byte offsets inside a slot
+};
+
+template <int ALGO>
+__global__ void __launch_bounds__(GRID_PLAN_BLOCK) crb_grid_plan_kernel(const GridPlanArgs a) {
+  const int64_t lane = (int64_t)blockIdx.x * GRID_PLAN_BLOCK + threadIdx.x;
+  if (lane >= a.slots) return;
+  char* slot = a.ws + lane * a.slot_bytes;
+  Entry* heap = (Entry*)(slot + a.heap_off);
+  float* g = (float*)(slot + a.g_off);
+  uint8_t* st = (uint8_t*)(slot + a.state_off);
+  const int64_t n = a.n;
+  const int W = a.box.max_x - a.box.min_x, H = a.box.max_y - a.box.min_y;
+  const int64_t cells = (int64_t)W * H;
+  for (;;) {
+    const int64_t q = (int64_t)atomicAdd(a.counter, 1ull);
+    if (q >= n) return;
+    int sx, sy, gx, gy;
+    int32_t status = CRB_GRID_NO_PATH, nvis = 0, plen = 0;
+    float cost = grid_nan();
+    if (!(grid_cell_f(a.sg[q], a.reso, sx) && grid_cell_f(a.sg[n + q], a.reso, sy) &&
+          grid_cell_f(a.sg[2 * n + q], a.reso, gx) && grid_cell_f(a.sg[3 * n + q], a.reso, gy))) {
+      status = CRB_GRID_BAD_POINT;
+    } else {
+      // box-relative cells (64-bit: a cell far outside the box must not wrap into it)
+      const int64_t rsx = (int64_t)sx - a.box.min_x, rsy = (int64_t)sy - a.box.min_y;
+      const int64_t rgx = (int64_t)gx - a.box.min_x, rgy = (int64_t)gy - a.box.min_y;
+      if (rsx < 0 || rsx >= W || rsy < 0 || rsy >= H) {
+        status = CRB_GRID_START_OUTSIDE;
+      } else {
+        const bool goal_in = rgx >= 0 && rgx < W && rgy >= 0 && rgy < H;
+        const int64_t goal_cell = goal_in ? rgx * H + rgy : -1;
+        // fresh cell state (and path costs) for this query, 16 bytes per store
+        {
+          uint4* s4 = (uint4*)st;
+          const int64_t n4 = (cells + 15) / 16;
+          for (int64_t i = 0; i < n4; ++i) s4[i] = make_uint4(0u, 0u, 0u, 0u);
+          if (ALGO == CRB_GRID_ASTAR) {
+            const uint32_t fm = __float_as_uint(FLT_MAX);
+            uint4* g4 = (uint4*)g;
+            const int64_t m4 = (cells + 3) / 4;
+            for (int64_t i = 0; i < m4; ++i) g4[i] = make_uint4(fm, fm, fm, fm);
+          }
+        }
+        const int64_t start = rsx * H + rsy;
+        if (ALGO == CRB_GRID_ASTAR) g[start] = 0.0f;
+        int64_t len = 0;
+        heap_push(heap, len, Entry{0.0f, (uint32_t)start << 3});
+        bool first = true;
+        while (len > 0) {
+          const Entry e = heap_pop(heap, len);
+          const int64_t cell = e.cd >> 3;
+          if (st[cell] & 0x80) continue;  // a duplicate of a visited cell
+          st[cell] = first ? 0x88 : (uint8_t)(0x80 | (e.cd & 7));
+          first = false;
+          ++nvis;
+          if (cell == goal_cell) {
+            status = CRB_GRID_FOUND;
+            cost = e.key;
+            break;
+          }
+          const int cx = (int)(cell / H), cy = (int)(cell - (int64_t)cx * H);
+          float gc = 0.0f, h = 0.0f;
+          if (ALGO == CRB_GRID_ASTAR) {
+            gc = g[cell];
+            // calc_heristic(ngoal, node): w * std::sqrt(pow(dx, 2) + pow(dy, 2)) in double (w = 1), narrowed
+            const double dx = (double)(rgx - cx), dy = (double)(rgy - cy);
+            h = __double2float_rn(__dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy))));
+          }
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int nx = cx + c_mx[i], ny = cy + c_my[i];
+            if (nx < 0 || nx >= W || ny < 0 || ny >= H) continue;  // verify_node: the box
+            const int64_t nc = (int64_t)nx * H + ny;
+            if (__ldg(a.map + nc)) continue;                        // verify_node: the map
+            if (st[nc] & 0x80) continue;                            // visited
+            const float step = i < 4 ? 1.0f : kDiag;
+            if (ALGO == CRB_GRID_ASTAR) {
+              const float ng = __fadd_rn(gc, step);
+              if (ng < g[nc]) {
+                g[nc] = ng;
+                heap_push(heap, len, Entry{__fadd_rn(ng, h), ((uint32_t)nc << 3) | (uint32_t)i});
+              }
+            } else {
+              heap_push(heap, len, Entry{__fadd_rn(e.key, step), ((uint32_t)nc << 3) | (uint32_t)i});
+            }
+          }
+        }
+        if (status == CRB_GRID_FOUND) {
+          // calc_final_path: the goal, then parent after parent down to the start
+          int64_t c = goal_cell;
+          for (;;) {
+            if (a.path && plen < a.max_pts) {
+              const int x = (int)(c / H), y = (int)(c - (c / H) * H);
+              a.path[(2 * (int64_t)plen) * n + q] = __fmul_rn(__int2float_rn(x + a.box.min_x), a.reso);
+              a.path[(2 * (int64_t)plen + 1) * n + q] = __fmul_rn(__int2float_rn(y + a.box.min_y), a.reso);
+            }
+            ++plen;
+            const uint8_t s = st[c];
+            if (s & 0x08) break;
+            c -= (int64_t)c_mx[s & 7] * H + c_my[s & 7];
+          }
+        }
+      }
+    }
+    if (status != CRB_GRID_FOUND) plen = 0;
+    if (a.path_len) a.path_len[q] = plen;
+    if (a.cost) a.cost[q] = cost;
+    if (a.n_visited) a.n_visited[q] = status == CRB_GRID_NO_PATH || status == CRB_GRID_FOUND ? nvis : 0;
+    if (a.status) a.status[q] = status;
+  }
+}
+
+namespace {
+
+// W, H and W * H of a box inside the limits, or false after setting the error string
+bool grid_box_dims(const crb_grid_box* b, const char* fn, int64_t& W, int64_t& H) {
+  if (b == nullptr) {
+    crb_set_error("%s: invalid argument: box is NULL", fn);
+    return false;
+  }
+  W = (int64_t)b->max_x - b->min_x;
+  H = (int64_t)b->max_y - b->min_y;
+  if (W < 1 || H < 1) {
+    crb_set_error("%s: invalid argument: the box is empty", fn);
+    return false;
+  }
+  if (W > CRB_GRID_MAX_SIDE || H > CRB_GRID_MAX_SIDE || W * H > CRB_GRID_MAX_CELLS) {
+    crb_set_error("%s: invalid argument: the box exceeds CRB_GRID_MAX_SIDE or CRB_GRID_MAX_CELLS", fn);
+    return false;
+  }
+  return true;
+}
+
+bool grid_reso_ok(float reso) { return isfinite(reso) && reso > 0.0f; }
+
+int grid_require_device(const char* fn) {
+  int count = 0;
+  const cudaError_t e = cudaGetDeviceCount(&count);
+  if (e != cudaSuccess || count == 0) {
+    cudaGetLastError();
+    crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", fn);
+    return CRB_ERR_NO_DEVICE;
+  }
+  return CRB_OK;
+}
+
+size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// slot layout: heap | g (A* only) | state, each 256-byte aligned
+void grid_slot_layout(int algo, int64_t cells, int64_t& heap_off, int64_t& g_off, int64_t& state_off,
+                      size_t& slot_bytes) {
+  heap_off = 0;
+  g_off = (int64_t)align_up((size_t)(8 * cells + 1) * sizeof(Entry), 256);
+  state_off = g_off + (algo == CRB_GRID_ASTAR ? (int64_t)align_up((size_t)cells * sizeof(float), 256) : 0);
+  slot_bytes = align_up((size_t)state_off + (size_t)cells, 256);
+}
+
+int grid_slots(crb_ctx* ctx, int algo, int64_t cells, int64_t n, int64_t& slots, size_t& slot_bytes,
+               int64_t* offs) {
+  int per_sm = 0;
+  CRB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(
+      &per_sm, algo == CRB_GRID_ASTAR ? (const void*)crb_grid_plan_kernel<CRB_GRID_ASTAR>
+                                      : (const void*)crb_grid_plan_kernel<CRB_GRID_DIJKSTRA>,
+      GRID_PLAN_BLOCK, 0));
+  int64_t ho, go, so;
+  grid_slot_layout(algo, cells, ho, go, so, slot_bytes);
+  const int64_t resident = (int64_t)(per_sm > 0 ? per_sm : 1) * GRID_PLAN_BLOCK * ctx->sm_count;
+  int64_t by_budget = (int64_t)(CRB_GRID_WS_BUDGET / slot_bytes);
+  if (by_budget < 1) by_budget = 1;
+  slots = n < resident ? n : resident;
+  if (slots > by_budget) slots = by_budget;
+  if (slots < 1) slots = 1;
+  if (offs) {
+    offs[0] = ho;
+    offs[1] = go;
+    offs[2] = so;
+  }
+  return CRB_OK;
+}
+
+}  // namespace
+
+// Grow-only planner workspace of the context (the first 256 bytes hold the query counter).
+static int grid_ws_reserve(crb_ctx* ctx, size_t bytes) {
+  if (ctx->grid_ws_cap >= bytes) return CRB_OK;
+  if (ctx->grid_ws) {
+    CRB_CUDA(cudaStreamSynchronize(ctx->stream));
+    CRB_CUDA(cudaFree(ctx->grid_ws));
+    ctx->grid_ws = nullptr;
+    ctx->grid_ws_cap = 0;
+  }
+  const cudaError_t e = cudaMalloc(&ctx->grid_ws, bytes);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    ctx->grid_ws = nullptr;
+    crb_set_error("crb_grid_plan_batched: cudaMalloc of %zu workspace bytes: %s", bytes, cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? CRB_ERR_ALLOC : CRB_ERR_CUDA;
+  }
+  ctx->grid_ws_cap = bytes;
+  return CRB_OK;
+}
+
+extern "C" {
+
+int crb_grid_box_of_obstacles(int64_t n_obs, const float* ox, const float* oy, float reso, crb_grid_box* box) {
+  CRB_REQUIRE(n_obs >= 1, "n_obs must be >= 1");
+  CRB_REQUIRE(ox && oy && box, "ox, oy or box is NULL");
+  CRB_REQUIRE(grid_reso_ok(reso), "reso must be finite and > 0");
+  int mnx = INT32_MAX, mxx = INT32_MIN, mny = INT32_MAX, mxy = INT32_MIN;
+  for (int64_t k = 0; k < n_obs; ++k) {
+    const double rx = round((double)ox[k] * 1.0 / (double)reso), ry = round((double)oy[k] * 1.0 / (double)reso);
+    CRB_REQUIRE(rx >= -2147483648.0 && rx < 2147483648.0 && ry >= -2147483648.0 && ry < 2147483648.0,
+                "an obstacle is non-finite or rounds outside the int range");
+    const int x = (int)rx, y = (int)ry;
+    mnx = x < mnx ? x : mnx;
+    mxx = x > mxx ? x : mxx;
+    mny = y < mny ? y : mny;
+    mxy = y > mxy ? y : mxy;
+  }
+  box->min_x = mnx;
+  box->min_y = mny;
+  box->max_x = mxx;
+  box->max_y = mxy;
+  return CRB_OK;
+}
+
+int crb_grid_obstacle_map(crb_ctx* ctx, int64_t n_obs, const float* ox, const float* oy, float reso, float rr,
+                          const crb_grid_box* box, uint8_t* map) {
+  CRB_REQUIRE(ctx != nullptr, "ctx is NULL");
+  CRB_REQUIRE(n_obs >= 0, "n_obs must be >= 0");
+  CRB_REQUIRE(grid_reso_ok(reso), "reso must be finite and > 0");
+  CRB_REQUIRE(isfinite(rr), "rr must be finite");
+  int64_t W, H;
+  if (!grid_box_dims(box, __func__, W, H)) return CRB_ERR_INVALID_ARG;
+  CRB_REQUIRE(map != nullptr && (n_obs == 0 || (ox && oy)), "ox, oy or map is NULL");
+  const int rc = grid_require_device(__func__);
+  if (rc != CRB_OK) return rc;
+  CRB_DEVICE_GUARD(ctx);
+  const int64_t cells = W * H;
+  // vr / reso: the float quotient the reference compares with
+  const float thr = rr / reso;
+  crb_grid_map_kernel<<<crb_grid_for(cells, GRID_MAP_BLOCK), GRID_MAP_BLOCK, 0, ctx->stream>>>(
+      n_obs, ox, oy, reso, thr, *box, cells, map);
+  CRB_CUDA(cudaGetLastError());
+  ctx->launches++;
+  return CRB_OK;
+}
+
+int crb_grid_plan_slots(crb_ctx* ctx, int algo, const crb_grid_box* box, int64_t n, int64_t* slots) {
+  CRB_REQUIRE(ctx != nullptr && slots != nullptr, "ctx or slots is NULL");
+  CRB_REQUIRE(algo == CRB_GRID_ASTAR || algo == CRB_GRID_DIJKSTRA, "algo must be CRB_GRID_ASTAR or CRB_GRID_DIJKSTRA");
+  CRB_REQUIRE(n >= 0, "n must be >= 0");
+  int64_t W, H;
+  if (!grid_box_dims(box, __func__, W, H)) return CRB_ERR_INVALID_ARG;
+  const int rc = grid_require_device(__func__);
+  if (rc != CRB_OK) return rc;
+  CRB_DEVICE_GUARD(ctx);
+  size_t sb;
+  return grid_slots(ctx, algo, W * H, n, *slots, sb, nullptr);
+}
+
+int crb_grid_plan_batched(crb_ctx* ctx, int algo, const crb_grid_box* box, const uint8_t* map, float reso, int64_t n,
+                          const float* sg, int max_pts, float* path, int32_t* path_len, float* cost,
+                          int32_t* n_visited, int32_t* status) {
+  CRB_REQUIRE(ctx != nullptr, "ctx is NULL");
+  CRB_REQUIRE(algo == CRB_GRID_ASTAR || algo == CRB_GRID_DIJKSTRA, "algo must be CRB_GRID_ASTAR or CRB_GRID_DIJKSTRA");
+  CRB_REQUIRE(grid_reso_ok(reso), "reso must be finite and > 0");
+  CRB_REQUIRE(n >= 0 && n <= INT64_MAX / 4, "n out of range");
+  CRB_REQUIRE(max_pts >= 0, "max_pts must be >= 0");
+  CRB_REQUIRE(n <= INT64_MAX / 2 / (max_pts > 0 ? max_pts : 1), "n * max_pts out of range");
+  int64_t W, H;
+  if (!grid_box_dims(box, __func__, W, H)) return CRB_ERR_INVALID_ARG;
+  CRB_REQUIRE(n == 0 || (map && sg), "map or sg is NULL");
+  CRB_REQUIRE(n == 0 || max_pts == 0 || path, "path is NULL with max_pts > 0");
+  const int rc = grid_require_device(__func__);
+  if (rc != CRB_OK) return rc;
+  if (n == 0) return CRB_OK;
+  CRB_DEVICE_GUARD(ctx);
+  GridPlanArgs a;
+  a.box = *box;
+  a.map = map;
+  a.reso = reso;
+  a.n = n;
+  a.sg = sg;
+  a.max_pts = max_pts;
+  a.path = max_pts > 0 ? path : nullptr;
+  a.path_len = path_len;
+  a.cost = cost;
+  a.n_visited = n_visited;
+  a.status = status;
+  int64_t offs[3];
+  int r = grid_slots(ctx, algo, W * H, n, a.slots, a.slot_bytes, offs);
+  if (r != CRB_OK) return r;
+  a.heap_off = offs[0];
+  a.g_off = offs[1];
+  a.state_off = offs[2];
+  r = grid_ws_reserve(ctx, 256 + (size_t)a.slots * a.slot_bytes);
+  if (r != CRB_OK) return r;
+  a.counter = (unsigned long long*)ctx->grid_ws;
+  a.ws = (char*)ctx->grid_ws + 256;
+  CRB_CUDA(cudaMemsetAsync(a.counter, 0, sizeof(unsigned long long), ctx->stream));
+  const int blocks = crb_grid_for(a.slots, GRID_PLAN_BLOCK);
+  if (algo == CRB_GRID_ASTAR)
+    crb_grid_plan_kernel<CRB_GRID_ASTAR><<<blocks, GRID_PLAN_BLOCK, 0, ctx->stream>>>(a);
+  else
+    crb_grid_plan_kernel<CRB_GRID_DIJKSTRA><<<blocks, GRID_PLAN_BLOCK, 0, ctx->stream>>>(a);
+  CRB_CUDA(cudaGetLastError());
+  ctx->launches++;
+  return CRB_OK;
+}
+
+}  // extern "C"

@@ -16,6 +16,9 @@ Method names follow the reference functions they replace:
   Engine.slp_search_nearest  <- search_nearest_one_from_lookuptable()            src/state_lattice_planner.cpp:115-135
   Engine.slp_generate_path   <- generate_path()                                  src/state_lattice_planner.cpp:137-155
   slp_load_table             <- main()'s CSVIterator + std::stod reading         src/state_lattice_planner.cpp:214-226
+  grid_box_of_obstacles      <- a_star_planning() / dijkstra_star_planning() :115-140 (obstacle cells, the box)
+  Engine.grid_obstacle_map   <- calc_obstacle_map()                              src/a_star.cpp:48-78
+  Engine.grid_plan           <- a_star_planning() / dijkstra_star_planning()     src/a_star.cpp:110-244, src/dijkstra.cpp
 
 All arrays are SoA field-major float32 (`[fields, n]`, C-contiguous); see include/crb.h.  Methods
 without a suffix take CUDA tensors (torch is only the device allocator / stream owner); `*_host`
@@ -31,7 +34,7 @@ from typing import Optional
 import numpy as np
 
 from . import _lib
-from ._lib import DwaParams, EkfParams, MpcParams, MptgParams, PfParams, check, load_library
+from ._lib import DwaParams, EkfParams, GridBox, MpcParams, MptgParams, PfParams, check, load_library
 
 try:  # torch is the device-memory / stream / distributed plumbing, never the compute path
     import torch
@@ -75,6 +78,19 @@ def slp_default_params():
     p, v = MptgParams(), C.c_float(0.0)
     load_library().crb_slp_default_params(C.byref(p), C.byref(v))
     return p, float(v.value)
+
+
+def grid_box_of_obstacles(ox, oy, reso: float) -> GridBox:
+    """The box of cells [min, max) of an obstacle list, as the planners compute it (src/a_star.cpp:115-140): every
+    obstacle rounded as (int)round(o * 1.0 / reso) in double.  ox, oy host arrays (float32); no device needed."""
+    x = np.ascontiguousarray(ox, np.float32)
+    y = np.ascontiguousarray(oy, np.float32)
+    if x.shape != y.shape or x.ndim != 1:
+        raise ValueError(f"ox, oy: expected two 1-D arrays of one length, got {x.shape} and {y.shape}")
+    b = GridBox()
+    check(load_library().crb_grid_box_of_obstacles(x.size, x.ctypes.data, y.ctypes.data, float(reso), C.byref(b)),
+          "crb_grid_box_of_obstacles")
+    return b
 
 
 _libc = None
@@ -123,7 +139,8 @@ def _ptr(a, dtype, *, device: Optional[bool], name: str) -> int:
     if a is None:
         return None
     if torch is not None and isinstance(a, torch.Tensor):
-        want = {np.float32: torch.float32, np.int32: torch.int32, np.float64: torch.float64}[dtype]
+        want = {np.float32: torch.float32, np.int32: torch.int32, np.float64: torch.float64,
+                np.uint8: torch.uint8}[dtype]
         if a.dtype != want:
             raise TypeError(f"{name}: expected {want}, got {a.dtype}")
         if not a.is_contiguous():
@@ -565,6 +582,70 @@ class Engine:
         self.mptg_optimize(state, target, param, params if params is not None else p0, traj=traj, traj_len=traj_len,
                            cost=cost, status=status, iters=iters)
         return dict(param=param, traj=traj, traj_len=traj_len, cost=cost, status=status, iters=iters, row=row)
+
+    # ---- grid A* / Dijkstra ------------------------------------------------------------------------------------
+    @staticmethod
+    def grid_box_of_obstacles(ox, oy, reso: float) -> GridBox:
+        """The planners' box of cells from host obstacle arrays (see grid_box_of_obstacles)."""
+        return grid_box_of_obstacles(ox, oy, reso)
+
+    @staticmethod
+    def _grid_dims(box: GridBox):
+        return int(box.max_x) - int(box.min_x), int(box.max_y) - int(box.min_y)
+
+    def grid_obstacle_map(self, ox, oy, reso: float, rr: float, box: GridBox, map=None):
+        """calc_obstacle_map() :48-78 for the box: ox, oy [n_obs] CUDA float32.  Returns map [W, H] uint8 (1 =
+        blocked; cell (x, y) at [x - min_x, y - min_y]), allocated when not given.  Only enqueues."""
+        n = int(ox.shape[-1])
+        _shape(ox, 1, n, "ox"); _shape(oy, 1, n, "oy")
+        W, H = self._grid_dims(box)
+        if map is None:
+            map = torch.empty((max(W, 0), max(H, 0)), dtype=torch.uint8, device=ox.device)
+        elif tuple(map.shape) != (W, H):
+            raise ValueError(f"map: expected shape ({W}, {H}), got {tuple(map.shape)}")
+        check(self.lib.crb_grid_obstacle_map(
+            self.ctx, n, _ptr(ox, np.float32, device=True, name="ox"), _ptr(oy, np.float32, device=True, name="oy"),
+            float(reso), float(rr), C.byref(box), _ptr(map, np.uint8, device=True, name="map")),
+            "crb_grid_obstacle_map")
+        return map
+
+    def grid_plan_slots(self, algo: int, box: GridBox, n: int) -> int:
+        """The number of searches grid_plan runs at once for n queries on this box."""
+        s = C.c_int64(0)
+        check(self.lib.crb_grid_plan_slots(self.ctx, int(algo), C.byref(box), int(n), C.byref(s)),
+              "crb_grid_plan_slots")
+        return int(s.value)
+
+    def grid_plan(self, algo: int, box: GridBox, map, reso: float, sg, max_pts: int = 0, path=None, path_len=None,
+                  cost=None, n_visited=None, status=None):
+        """a_star_planning() (algo CRB_GRID_ASTAR) or dijkstra_star_planning() (CRB_GRID_DIJKSTRA) for n queries on
+        one map: map [W, H] uint8 (grid_obstacle_map's), sg [4, n] float32 (sx, sy, gx, gy).  Returns dict(path
+        [2*max_pts, n] (point k's x, y in rows 2k, 2k+1, the goal first; NaN past path_len; None when max_pts = 0),
+        path_len, cost, n_visited, status (CRB_GRID_*)), allocating what is not given.  CUDA tensors; only enqueues
+        (the first call at a larger workspace allocates it)."""
+        n = int(sg.shape[-1])
+        _shape(sg, 4, n, "sg")
+        W, H = self._grid_dims(box)
+        if tuple(map.shape) not in ((W, H), (W * H,)):
+            raise ValueError(f"map: expected shape ({W}, {H}), got {tuple(map.shape)}")
+        dev = sg.device
+        if path is None and max_pts > 0:
+            path = torch.full((2 * max_pts, n), float("nan"), dtype=torch.float32, device=dev)
+        if path is not None:
+            _shape(path, 2 * max_pts, n, "path")
+        i32 = lambda a: a if a is not None else torch.empty(n, dtype=torch.int32, device=dev)  # noqa: E731
+        path_len, n_visited, status = i32(path_len), i32(n_visited), i32(status)
+        if cost is None:
+            cost = torch.empty(n, dtype=torch.float32, device=dev)
+        for a, name in ((path_len, "path_len"), (cost, "cost"), (n_visited, "n_visited"), (status, "status")):
+            _shape(a, 1, n, name)
+        check(self.lib.crb_grid_plan_batched(
+            self.ctx, int(algo), C.byref(box), _ptr(map, np.uint8, device=True, name="map"), float(reso), n,
+            _ptr(sg, np.float32, device=True, name="sg"), int(max_pts),
+            _ptr(path, np.float32, device=True, name="path"), _ptr(path_len, np.int32, device=True, name="path_len"),
+            _ptr(cost, np.float32, device=True, name="cost"), _ptr(n_visited, np.int32, device=True, name="n_visited"),
+            _ptr(status, np.int32, device=True, name="status")), "crb_grid_plan_batched")
+        return dict(path=path, path_len=path_len, cost=cost, n_visited=n_visited, status=status)
 
     # ---- multi-GPU: the communicator lives in libcrb (crb_comm.cu), not in torch --------------------
     @staticmethod

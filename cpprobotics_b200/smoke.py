@@ -160,5 +160,24 @@ def run() -> None:
     assert ok, "SLP GPU result is not bit-identical to the checker"
     print(f"smoke SLP   {qs.shape[1]} queries, {int(nsd.sum().item())} states: bit-identical to the checker; "
           f"{int((gs['status'] == 0).sum().item())} converged")
+    # grid A* / Dijkstra: the demo's map and 65 queries on it per planner, as the checker
+    from oracle import grid as OG  # checker only
+    from ._lib import GridBox
+    gox, goy = synth.grid_demo_obstacles()
+    gd = synth.GRID_DEMO
+    gb = OG.box_of_obstacles(gox, goy, gd["reso"])
+    gm = OG.obstacle_map(gox, goy, gd["reso"], gd["rr"], gb)
+    gsg = synth.grid_inputs(65, gb, gm, gd["reso"])
+    box = GridBox(*[int(v) for v in gb])
+    gmd = eng.grid_obstacle_map(torch.from_numpy(gox).to(dev), torch.from_numpy(goy).to(dev), gd["reso"], gd["rr"], box)
+    for algo in (OG.ASTAR, OG.DIJKSTRA):
+        gr = eng.grid_plan(algo, box, gmd, gd["reso"], torch.from_numpy(gsg).to(dev), max_pts=128)
+        torch.cuda.synchronize()
+        go = OG.plan(algo, gb, gm, gd["reso"], gsg, max_pts=128)
+        ok = same_nan(gmd, gm) and all(same_nan(gr[k], go[k]) for k in ("path", "path_len", "cost", "n_visited",
+                                                                          "status"))
+        assert ok, "grid planner GPU result is not bit-identical to the checker"
+        print(f"smoke GRID  {'A*' if algo == OG.ASTAR else 'Dijkstra'} 65 queries on the demo map: bit-identical to "
+              f"the checker; {int((gr['status'] == 0).sum().item())} found")
     print(f"smoke ok: {eng.launches} kernel launches through libcrb.so")
     eng.close()

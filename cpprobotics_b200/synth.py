@@ -344,3 +344,75 @@ def slp_table(rows: int, seed: int = 0x51A7):
     t[:, 4] = 2.0 * t[:, 1] / (t[:, 3] ** 2)
     t[:, 5] = t[:, 4]
     return np.ascontiguousarray(t.astype(np.float32))
+
+
+# src/a_star.cpp / src/dijkstra.cpp:247-286: the demo's walls (float loop counters, 60.0 - i narrowed to float), start
+# (10, 10), goal (50, 50), grid_size 1, robot_size 1.  The box is [0, 60) x [0, 60): 60 x 60 cells.
+GRID_DEMO = dict(sx=10.0, sy=10.0, gx=50.0, gy=50.0, reso=1.0, rr=1.0)
+
+
+def grid_demo_obstacles():
+    """(ox, oy) float32 in the demo's push_back order."""
+    ox, oy = [], []
+    for i in range(60):
+        ox.append(i); oy.append(60.0)
+    for i in range(60):
+        ox.append(60.0); oy.append(i)
+    for i in range(61):
+        ox.append(i); oy.append(60.0)
+    for i in range(61):
+        ox.append(0.0); oy.append(i)
+    for i in range(40):
+        ox.append(20.0); oy.append(i)
+    for i in range(40):
+        ox.append(40.0); oy.append(60.0 - i)
+    return np.float32(ox), np.float32(oy)
+
+
+def grid_scatter_obstacles(side: int, reso: float = 1.0, per_cell: float = 1.0 / 40, seed: int = 0x6A1D):
+    """(ox, oy) float32: obstacles at the corners (0, 0) and (side, side), which make the box [0, side)^2 cells, and
+    round(side^2 * per_cell) obstacles scattered uniformly over it (coordinates in metres, cell * reso)."""
+    k = int(round(side * side * per_cell))
+    idx = np.arange(k, dtype=np.uint64)
+    x = uniform(seed, 170, idx, 0.0, side * reso)
+    y = uniform(seed, 171, idx, 0.0, side * reso)
+    ox = np.concatenate([[0.0, side * reso], x]).astype(np.float32)
+    oy = np.concatenate([[0.0, side * reso], y]).astype(np.float32)
+    return ox, oy
+
+
+def grid_inputs(n: int, box, grid_map, reso: float, seed: int = 0xC0FFEE, i0: int = 0):
+    """sg [4, n] float32 (sx, sy, gx, gy) for the grid planners on one map (box (min_x, min_y, max_x, max_y), grid_map
+    [W, H], nonzero = blocked); query i a function of (seed, i0 + i) and the map only.  Start and goal are free cells,
+    given in metres with a jitter of up to 0.45 cell that the planners' rounding removes.  One query in 64 is a corner
+    case, by index:
+      1  the goal on a blocked cell (unreachable)      2  the start outside the box
+      3  a NaN goal                                      4  start == goal
+      5  the goal outside the box                        6  the start on a blocked cell (the reference expands it)"""
+    idx = np.arange(i0, i0 + n, dtype=np.uint64)
+    m = np.asarray(grid_map)
+    W, H = m.shape
+    free = np.flatnonzero(m.reshape(-1) == 0)
+    blocked = np.flatnonzero(m.reshape(-1) != 0)
+    if free.size == 0:
+        raise ValueError("the map has no free cell")
+
+    def pick(cells, stream):
+        k = np.minimum((u01(seed, stream, idx) * cells.size).astype(np.int64), cells.size - 1)
+        c = cells[k]
+        return c // H + int(box[0]), c % H + int(box[1])
+
+    sx, sy = pick(free, 180)
+    gx, gy = pick(free, 181)
+    corner = idx % np.uint64(64)
+    if blocked.size:
+        bx, by = pick(blocked, 182)
+        gx, gy = np.where(corner == 1, bx, gx), np.where(corner == 1, by, gy)
+        sx, sy = np.where(corner == 6, bx, sx), np.where(corner == 6, by, sy)
+    sx = np.where(corner == 2, int(box[0]) - 3, sx)
+    gx, gy = np.where(corner == 4, sx, gx), np.where(corner == 4, sy, gy)
+    gy = np.where(corner == 5, int(box[3]) + 2, gy)
+    jit = [uniform(seed, 183 + j, idx, -0.45, 0.45) for j in range(4)]
+    sg = np.stack([(sx + jit[0]) * reso, (sy + jit[1]) * reso, (gx + jit[2]) * reso, (gy + jit[3]) * reso])
+    sg[2] = np.where(corner == 3, np.nan, sg[2])
+    return np.ascontiguousarray(sg.astype(np.float32))

@@ -29,6 +29,10 @@
  *   crb_slp_search_nearest_batched      <- search_nearest_one_from_lookuptable()  src/state_lattice_planner.cpp:115-135
  *                                         (generate_path :137-155 is this search followed by
  *                                          crb_mptg_optimize_batched with crb_slp_default_params)
+ *   crb_grid_box_of_obstacles           <- a_star_planning() / dijkstra_star_planning() :115-140 (cells, box)
+ *   crb_grid_obstacle_map               <- calc_obstacle_map()   src/a_star.cpp:48-78, src/dijkstra.cpp
+ *   crb_grid_plan_batched               <- a_star_planning()     src/a_star.cpp:110-244 (with calc_final_path
+ *                                          :31-45), dijkstra_star_planning()  src/dijkstra.cpp
  *   crb_stats_*                         <- (no reference counterpart) per-GPU summary statistics, the
  *                                          only thing that ever crosses NVLink (one all-gather).
  *
@@ -494,6 +498,80 @@ int crb_slp_sample_states_batched(crb_ctx* ctx, int64_t n_q, const crb_slp_sampl
  * stream. */
 int crb_slp_search_nearest_batched(crb_ctx* ctx, int64_t n, const float* target, const float* table, int rows,
                                    const float* k0, float* param, int32_t* row);
+
+/* ---- grid A* and Dijkstra (src/a_star.cpp, src/dijkstra.cpp) ------------------------------------------------ */
+/* Many start / goal queries on one obstacle map.  The two files share one skeleton: obstacles rounded to cells, a
+ * box of cells [min, max) on each axis, calc_obstacle_map :48-78, then a best-first search over the eight moves of
+ * get_motion_model :99-108 with a std::priority_queue ordered by `left->key > right->key`.  Bit-exact with the
+ * reference built for x86-64: the same float / double expressions, and the same pop order, ties included (the
+ * libstdc++ binary heap's push / pop / adjust steps are restated, DESIGN.md).
+ *
+ * Scope.  The reference is defined only for a square box and, for A*, a box with min_x = min_y = 0 (it allocates
+ * obmap (ywidth, xwidth) but indexes it [x][y], and indexes A*'s path_cost without the box offset), a start inside
+ * the box and a reachable goal (otherwise it calls top() on an empty queue).  This library indexes every per-cell
+ * array relative to the box, (x - min_x, y - min_y), which inside that domain is the same computation, and defines
+ * the rest with the statuses below. */
+typedef struct crb_grid_box {
+  int32_t min_x, min_y, max_x, max_y; /* cells [min_x, max_x) x [min_y, max_y) */
+} crb_grid_box;
+/* Box limits: both sides in [1, CRB_GRID_MAX_SIDE] and W * H <= CRB_GRID_MAX_CELLS (W = max_x - min_x,
+ * H = max_y - min_y), so every squared cell distance inside the box is exact in double and a cell index with a
+ * 3-bit move fits in 32 bits.  Otherwise CRB_ERR_INVALID_ARG. */
+#define CRB_GRID_MAX_SIDE 32768
+#define CRB_GRID_MAX_CELLS (1 << 24)
+/* Device workspace the planner may hold: slots = min(n, resident threads, CRB_GRID_WS_BUDGET / bytes per slot), at
+ * least 1, where a slot is a search's cell state (1 byte per cell), A*'s path costs (4 bytes per cell) and its heap
+ * (8 bytes per entry, 8 * W * H + 1 entries: every visited cell pushes at most 8). */
+#define CRB_GRID_WS_BUDGET ((size_t)1 << 32)
+
+/* The reference's :115-140 on host arrays (no device needed): every obstacle rounded as (int)round(o * 1.0 / reso)
+ * in double, box = (min over x, min over y, max over x, max over y).  As in the reference the extreme obstacle
+ * column and row lie outside the box (verify_node rejects x >= max_x).  CRB_ERR_INVALID_ARG when n_obs < 1, reso
+ * is not finite and > 0, or an obstacle is non-finite or rounds outside the int range. */
+int crb_grid_box_of_obstacles(int64_t n_obs, const float* ox, const float* oy, float reso, crb_grid_box* box);
+
+/* calc_obstacle_map :48-78: map [W*H] uint8 out, 1 = blocked, cell (x, y) at (x - min_x) * H + (y - min_y).  A
+ * cell is blocked when some obstacle k has (float)sqrt(pow(ox_k - x, 2) + pow(oy_k - y, 2)) <= rr / reso, the root
+ * in double and the threshold a float quotient; obstacles are rounded as in crb_grid_box_of_obstacles (one that
+ * rounds to a non-finite value or outside the int range blocks nothing).  ox, oy [n_obs], map: DEVICE pointers;
+ * reso finite and > 0, rr finite.  Only enqueues on the context's stream. */
+int crb_grid_obstacle_map(crb_ctx* ctx, int64_t n_obs, const float* ox, const float* oy, float reso, float rr,
+                          const crb_grid_box* box, uint8_t* map);
+
+#define CRB_GRID_ASTAR 0    /* a_star_planning :110-244 */
+#define CRB_GRID_DIJKSTRA 1 /* dijkstra_star_planning */
+
+/* Per-query status of crb_grid_plan_batched. */
+#define CRB_GRID_FOUND 0         /* the goal cell was popped */
+#define CRB_GRID_NO_PATH 1       /* the open set emptied first (goal unreachable, blocked or outside the box) */
+#define CRB_GRID_START_OUTSIDE 2 /* the start cell lies outside the box */
+#define CRB_GRID_BAD_POINT 3     /* start or goal is non-finite, or round(p / reso) leaves the int range */
+
+/* a_star_planning / dijkstra_star_planning for n queries on one map (the map of crb_grid_obstacle_map, or any
+ * uint8 map in its layout, nonzero = blocked).
+ *   sg [4][n] in: (sx, sy, gx, gy); cells are (int)roundf(p / reso), a float quotient
+ *   optional outputs, NULL = not written:
+ *     path [2*max_pts][n]  field 2k + j = component j (x, y) of point k: calc_final_path :31-45, the goal cell first,
+ *                          then its parents down to the start, each (float)cell * reso with no box offset; only the
+ *                          first min(path_len, max_pts) points are written, the rest is left as it is
+ *     path_len [n]         int32: the full number of points (1 when start == goal)
+ *     cost [n]             the popped goal entry's key: A* (path_cost[parent] + step) + h(parent), Dijkstra the sum
+ *                          of the steps
+ *     n_visited [n]        int32: cells popped while unvisited (start and goal included)
+ *     status [n]           int32: CRB_GRID_*; other than FOUND: path_len 0, cost NaN (n_visited counts the cells the
+ *                          search visited, 0 for START_OUTSIDE and BAD_POINT)
+ * The reference's quirks are kept: A*'s heuristic is taken at the expanded node, not the new one; A* pushes only on
+ * a strict decrease of path_cost and Dijkstra pushes every valid unvisited neighbour; duplicates stay in the heap and
+ * are dropped when popped; a start on an obstacle is expanded.
+ * One thread per query (a search is serial: its pop order is the result); persistent lanes take queries from an
+ * atomic counter.  The slots' workspace is a grow-only buffer of the context: the first call at a larger
+ * W * H * slots allocates (and synchronises the stream), so it cannot be captured in a CUDA graph; later calls only
+ * enqueue (a memset and one kernel) and can.  DEVICE pointers, NULL allowed when n = 0. */
+int crb_grid_plan_batched(crb_ctx* ctx, int algo, const crb_grid_box* box, const uint8_t* map, float reso, int64_t n,
+                          const float* sg, int max_pts, float* path, int32_t* path_len, float* cost,
+                          int32_t* n_visited, int32_t* status);
+/* The number of slots (concurrent searches) crb_grid_plan_batched uses for these arguments. */
+int crb_grid_plan_slots(crb_ctx* ctx, int algo, const crb_grid_box* box, int64_t n, int64_t* slots);
 
 /* ---- multi-GPU: communicator owned by the context (NCCL, opened at run time) ---------------------- */
 /* The batch shards over GPUs by contiguous agent ranges (one crb_ctx per device, one host thread or process

@@ -13,6 +13,8 @@
 //   MotionModel, TrajectoryOptimizer::optimizer_traj(...)    include/motion_model.h, include/trajectory_optimizer.h
 //   calc_{uniform_polar,biased_polar,lane}_states, search_nearest_one_from_lookuptable, generate_path
 //                                                            src/state_lattice_planner.cpp:47-155
+//   a_star_planning(sx, sy, gx, gy, ox, oy, reso, rr), dijkstra_star_planning(...)
+//                                                            src/a_star.cpp:110-244, src/dijkstra.cpp
 //
 // Eigen is not a dependency: crb::Mat<R,C> is a POD with the memory layout of
 // Eigen::Matrix<float,R,C> (column-major, contiguous, no padding), enough of its interface for the
@@ -24,6 +26,7 @@
 #ifndef CRB_REFERENCE_API_HPP_
 #define CRB_REFERENCE_API_HPP_
 
+#include <algorithm>
 #include <array>
 #include <cmath>
 #include <cstring>
@@ -652,6 +655,101 @@ inline std::vector<Traj> generate_path(StateList states, Table csv_file, float k
     }
     return out;
   }
+}
+}  // namespace cpprobotics
+
+// src/a_star.cpp:110-244 and src/dijkstra.cpp.  The reference's planners return nothing and draw; these return what
+// its calc_final_path :31-45 computes, {rx, ry}: the goal first, then parent after parent down to the start, each
+// cell * reso.  The batched overloads plan every (sx[i], sy[i], gx[i], gy[i]) on the one map of ox / oy in one
+// launch and return one {rx, ry} per query.  A query the reference does not define (an unreachable goal, a start
+// outside the box or a non-finite point: crb.h's CRB_GRID_* statuses) throws.
+namespace cpprobotics {
+namespace detail {
+inline std::vector<std::vector<std::vector<float>>> grid_plan(int algo, const std::vector<float>& sx,
+                                                              const std::vector<float>& sy,
+                                                              const std::vector<float>& gx,
+                                                              const std::vector<float>& gy,
+                                                              const std::vector<float>& ox,
+                                                              const std::vector<float>& oy, float reso, float rr) {
+  crb_ctx* ctx = crb::Session::get();
+  const size_t n = sx.size();
+  if (sy.size() != n || gx.size() != n || gy.size() != n) throw std::runtime_error("grid planner: sx, sy, gx, gy differ in length");
+  if (ox.size() != oy.size()) throw std::runtime_error("grid planner: ox and oy differ in length");
+  crb_grid_box box;
+  crb::check(crb_grid_box_of_obstacles((int64_t)ox.size(), ox.data(), oy.data(), reso, &box),
+             "crb_grid_box_of_obstacles");
+  std::vector<std::vector<std::vector<float>>> out(n);
+  if (n == 0) return out;
+  const size_t no = ox.size(), cells = (size_t)((int64_t)box.max_x - box.min_x) * (size_t)((int64_t)box.max_y - box.min_y);
+  std::vector<float> h(2 * no + 4 * n);  // ox | oy | sg [4][n]
+  std::copy(ox.begin(), ox.end(), h.begin());
+  std::copy(oy.begin(), oy.end(), h.begin() + no);
+  for (size_t i = 0; i < n; ++i) {
+    h[2 * no + i] = sx[i];
+    h[2 * no + n + i] = sy[i];
+    h[2 * no + 2 * n + i] = gx[i];
+    h[2 * no + 3 * n + i] = gy[i];
+  }
+  int max_pts = 256;
+  for (;;) {
+    // ox, oy, sg | len, status [2n] | map [cells bytes] | path [2 max_pts n]
+    const size_t map_f = (cells + 3) / 4;
+    float* d = crb::Session::scratch(h.size() + 2 * n + map_f + 2 * (size_t)max_pts * n);
+    float *dsg = d + 2 * no, *dls = dsg + 4 * n, *dmap = dls + 2 * n, *dpath = dmap + map_f;
+    crb::check(crb_memcpy_h2d(ctx, d, h.data(), h.size() * sizeof(float)), "h2d");
+    crb::check(crb_grid_obstacle_map(ctx, (int64_t)no, d, d + no, reso, rr, &box, (uint8_t*)dmap),
+               "crb_grid_obstacle_map");
+    crb::check(crb_grid_plan_batched(ctx, algo, &box, (const uint8_t*)dmap, reso, (int64_t)n, dsg, max_pts, dpath,
+                                     (int32_t*)dls, nullptr, nullptr, (int32_t*)(dls + n)),
+               "crb_grid_plan_batched");
+    std::vector<int32_t> ls(2 * n);
+    crb::check(crb_memcpy_d2h(ctx, ls.data(), dls, ls.size() * sizeof(int32_t)), "d2h");
+    int longest = 0;
+    for (size_t i = 0; i < n; ++i) {
+      if (ls[n + i] != CRB_GRID_FOUND)
+        throw std::runtime_error("grid planner: no path (status " + std::to_string(ls[n + i]) + ")");
+      if (ls[i] > longest) longest = ls[i];
+    }
+    if (longest > max_pts) {  // again with room for every whole path
+      max_pts = longest;
+      continue;
+    }
+    std::vector<float> p(2 * (size_t)max_pts * n);
+    crb::check(crb_memcpy_d2h(ctx, p.data(), dpath, p.size() * sizeof(float)), "d2h");
+    for (size_t i = 0; i < n; ++i) {
+      std::vector<float> rx, ry;
+      for (int k = 0; k < ls[i]; ++k) {
+        rx.push_back(p[(2 * (size_t)k) * n + i]);
+        ry.push_back(p[(2 * (size_t)k + 1) * n + i]);
+      }
+      out[i] = {rx, ry};
+    }
+    return out;
+  }
+}
+}  // namespace detail
+
+inline std::vector<std::vector<float>> a_star_planning(float sx, float sy, float gx, float gy, std::vector<float> ox_,
+                                                       std::vector<float> oy_, float reso, float rr) {
+  return detail::grid_plan(CRB_GRID_ASTAR, {sx}, {sy}, {gx}, {gy}, ox_, oy_, reso, rr)[0];
+}
+inline std::vector<std::vector<float>> dijkstra_star_planning(float sx, float sy, float gx, float gy,
+                                                              std::vector<float> ox_, std::vector<float> oy_,
+                                                              float reso, float rr) {
+  return detail::grid_plan(CRB_GRID_DIJKSTRA, {sx}, {sy}, {gx}, {gy}, ox_, oy_, reso, rr)[0];
+}
+inline std::vector<std::vector<std::vector<float>>> a_star_planning(std::vector<float> sx, std::vector<float> sy,
+                                                                    std::vector<float> gx, std::vector<float> gy,
+                                                                    std::vector<float> ox_, std::vector<float> oy_,
+                                                                    float reso, float rr) {
+  return detail::grid_plan(CRB_GRID_ASTAR, sx, sy, gx, gy, ox_, oy_, reso, rr);
+}
+inline std::vector<std::vector<std::vector<float>>> dijkstra_star_planning(std::vector<float> sx, std::vector<float> sy,
+                                                                           std::vector<float> gx, std::vector<float> gy,
+                                                                           std::vector<float> ox_,
+                                                                           std::vector<float> oy_, float reso,
+                                                                           float rr) {
+  return detail::grid_plan(CRB_GRID_DIJKSTRA, sx, sy, gx, gy, ox_, oy_, reso, rr);
 }
 }  // namespace cpprobotics
 
