@@ -5,12 +5,12 @@ is the thin Python host layer the tests and the bench use to reach it.  There is
 importing works anywhere (so the build can be checked without a GPU), computing needs an H100.
 """
 from ._lib import (CrbError, DwaParams, EkfParams, GridBox, MpcParams, MptgParams, PfParams,  # noqa: F401
-                   SlpSampler, load_library)
+                   RrtParams, SlpSampler, load_library)
 from .engine import (Engine, dwa_default_params, ekf_default_params, grid_box_of_obstacles,  # noqa: F401
-                     mpc_default_params, mptg_default_params, pf_default_params, slp_default_params,
-                     slp_load_table)
+                     mpc_default_params, mptg_default_params, pf_default_params, rrt_default_params,
+                     slp_default_params, slp_load_table)
 
 __all__ = ["Engine", "CrbError", "EkfParams", "PfParams", "MpcParams", "DwaParams", "MptgParams", "SlpSampler",
-           "GridBox", "load_library", "grid_box_of_obstacles",
+           "GridBox", "RrtParams", "load_library", "grid_box_of_obstacles",
            "ekf_default_params", "pf_default_params", "mpc_default_params", "dwa_default_params",
-           "mptg_default_params", "slp_default_params", "slp_load_table"]
+           "mptg_default_params", "slp_default_params", "slp_load_table", "rrt_default_params"]

@@ -48,6 +48,10 @@ CRB_GRID_FOUND = 0
 CRB_GRID_NO_PATH = 1
 CRB_GRID_START_OUTSIDE = 2
 CRB_GRID_BAD_POINT = 3
+CRB_RRT_MAX_ITER = 16384
+CRB_RRT_FOUND = 0
+CRB_RRT_MAX_ITER_REACHED = 1
+CRB_RRT_BAD_INPUT = 2
 
 c_f32p = C.POINTER(C.c_float)
 c_i32p = C.POINTER(C.c_int32)
@@ -89,6 +93,11 @@ class SlpSampler(C.Structure):
 
 class GridBox(C.Structure):
     _fields_ = [("min_x", C.c_int32), ("min_y", C.c_int32), ("max_x", C.c_int32), ("max_y", C.c_int32)]
+
+
+class RrtParams(C.Structure):
+    _fields_ = [("rand_min", C.c_float), ("rand_max", C.c_float), ("expand_dis", C.c_float),
+                ("goal_sample_rate", C.c_int32), ("max_iter", C.c_int32)]
 
 
 # name -> (restype, argtypes); every symbol include/crb.h declares
@@ -179,6 +188,10 @@ PROTOTYPES = {
                                         C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p]),
     "crb_grid_plan_slots": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(GridBox), C.c_int64, C.POINTER(C.c_int64)]),
+    "crb_rrt_default_params": (None, [C.POINTER(RrtParams)]),
+    "crb_rrt_plan_batched": (C.c_int, [C.c_void_p, C.POINTER(RrtParams), C.c_void_p, C.c_int32, C.c_int64, C.c_void_p,
+                                       C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "crb_stats_reduce": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p]),
     "crb_probe_fp32_peak": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),

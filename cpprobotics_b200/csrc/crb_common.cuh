@@ -30,6 +30,7 @@ struct crb_ctx {
   // grid planner workspace (query counter + one search slot per lane, crb_grid.cu), grown on demand
   void* grid_ws;
   size_t grid_ws_cap;
+  void* rrt_counter;  // RRT query counter (crb_rrt.cu), allocated on first use
   void* host_scratch;  // small pinned buffer for reduction results
   // per-device function attributes already set for this context's device (a second context on another
   // device in the same process must set them again, so these are not process-global latches)
@@ -340,4 +341,89 @@ __device__ __forceinline__ float crb_tanf_libm(float x) {
   const float y0 = __double2float_rn(d);
   const float y1 = __double2float_rn(__dsub_rn(d, (double)y0));
   return crb_tanf_kernel(y0, y1, 1 - ((n & 1) << 1));
+}
+
+// ---- atan2f with the HOST libm's bits -------------------------------------------------------------------
+// The reference calls std::atan2 on floats (include/rrt.h:113), i.e. glibc's atan2f.  glibc 2.39 computes it with
+// fdlibm's binary32 e_atan2f.c on top of __atanf (s_atanf.c) (Sun Microsystems, freely redistributable), in float
+// only; it is not (float)atan2((double)y, (double)x).  Restated operation for operation with explicitly rounded
+// intrinsics, so it does not depend on the TU's -fmad setting.  The C twin (oracle/crb_oracle_rrt.c) equals the host
+// atanf on every non-negative float and the host atan2f on dense pairs and every sign / zero / inf / NaN case
+// (tests/test_rrt.py); this equals the C twin on the device.
+static __device__ __noinline__ float crb_atanf_libm(float x) {  // __atanf
+  const int hx = __float_as_int(x);
+  const int ix = hx & 0x7fffffff;
+  int id;
+  if (ix >= 0x4c000000) {  // |x| >= 2^25
+    if (ix > 0x7f800000) return __fadd_rn(x, x);
+    return hx > 0 ? __fadd_rn(1.5707962513e+00f, 7.5497894159e-08f) : __fsub_rn(-1.5707962513e+00f, 7.5497894159e-08f);
+  }
+  if (ix < 0x3ee00000) {              // |x| < 0.4375
+    if (ix < 0x31000000) return x;    // |x| < 2^-29
+    id = -1;
+  } else {
+    x = fabsf(x);
+    if (ix < 0x3f980000) {      // |x| < 1.1875
+      if (ix < 0x3f300000) {    // 7/16 <= |x| < 11/16
+        id = 0;
+        x = __fdiv_rn(__fsub_rn(__fmul_rn(2.0f, x), 1.0f), __fadd_rn(2.0f, x));
+      } else {                  // 11/16 <= |x| < 19/16
+        id = 1;
+        x = __fdiv_rn(__fsub_rn(x, 1.0f), __fadd_rn(x, 1.0f));
+      }
+    } else if (ix < 0x401c0000) {  // |x| < 2.4375
+      id = 2;
+      x = __fdiv_rn(__fsub_rn(x, 1.5f), __fadd_rn(1.0f, __fmul_rn(1.5f, x)));
+    } else {                       // 2.4375 <= |x| < 2^25
+      id = 3;
+      x = __fdiv_rn(-1.0f, x);
+    }
+  }
+  const float z = __fmul_rn(x, x);
+  const float w = __fmul_rn(z, z);
+  const float s1 = __fmul_rn(z, __fadd_rn(3.3333334327e-01f, __fmul_rn(w, __fadd_rn(1.4285714924e-01f,
+                   __fmul_rn(w, __fadd_rn(9.0908870101e-02f, __fmul_rn(w, __fadd_rn(6.6610731184e-02f,
+                   __fmul_rn(w, __fadd_rn(4.9768779427e-02f, __fmul_rn(w, 1.6285819933e-02f)))))))))));
+  const float s2 = __fmul_rn(w, __fadd_rn(-2.0000000298e-01f, __fmul_rn(w, __fadd_rn(-1.1111110449e-01f,
+                   __fmul_rn(w, __fadd_rn(-7.6918758452e-02f, __fmul_rn(w, __fadd_rn(-5.8335702866e-02f,
+                   __fmul_rn(w, -3.6531571299e-02f)))))))));
+  if (id < 0) return __fsub_rn(x, __fmul_rn(x, __fadd_rn(s1, s2)));
+  // atanhi[id], atanlo[id] (selects, not an indexed array: no local memory)
+  const float hi = id == 0 ? 4.6364760399e-01f : id == 1 ? 7.8539812565e-01f : id == 2 ? 9.8279368877e-01f
+                                                                                       : 1.5707962513e+00f;
+  const float lo = id == 0 ? 5.0121582440e-09f : id == 1 ? 3.7748947079e-08f : id == 2 ? 3.4473217170e-08f
+                                                                                       : 7.5497894159e-08f;
+  const float r = __fsub_rn(hi, __fsub_rn(__fsub_rn(__fmul_rn(x, __fadd_rn(s1, s2)), lo), x));
+  return hx < 0 ? -r : r;
+}
+__device__ __forceinline__ float crb_atan2f_libm(float y, float x) {
+  const float tiny = 1.0e-30f, pi_o_4 = 7.8539818525e-01f, pi_o_2 = 1.5707963705e+00f, pi = 3.1415927410e+00f,
+              pi_lo = -8.7422776573e-08f;
+  const int hx = __float_as_int(x), ix = hx & 0x7fffffff;
+  const int hy = __float_as_int(y), iy = hy & 0x7fffffff;
+  if (ix > 0x7f800000 || iy > 0x7f800000) return __fadd_rn(x, y);  // NaN
+  if (hx == 0x3f800000) return crb_atanf_libm(y);                   // x = 1
+  const int m = ((hy >> 31) & 1) | ((hx >> 30) & 2);                 // 2 * sign(x) + sign(y)
+  const float pi_t = __fadd_rn(pi, tiny), pi_o_2_t = __fadd_rn(pi_o_2, tiny);
+  if (iy == 0) return m < 2 ? y : (m == 2 ? pi_t : __fsub_rn(-pi, tiny));
+  if (ix == 0) return hy < 0 ? __fsub_rn(-pi_o_2, tiny) : pi_o_2_t;
+  if (ix == 0x7f800000) {
+    if (iy == 0x7f800000) {
+      const float a = m < 2 ? pi_o_4 : __fmul_rn(3.0f, pi_o_4);
+      return (m & 1) ? __fsub_rn(-a, tiny) : __fadd_rn(a, tiny);
+    }
+    return m == 0 ? 0.0f : m == 1 ? -0.0f : m == 2 ? pi_t : __fsub_rn(-pi, tiny);
+  }
+  if (iy == 0x7f800000) return hy < 0 ? __fsub_rn(-pi_o_2, tiny) : pi_o_2_t;
+  const int k = (iy - ix) >> 23;
+  float z;
+  if (k > 60) z = __fadd_rn(pi_o_2, __fmul_rn(0.5f, pi_lo));  // |y / x| > 2^60
+  else if (hx < 0 && k < -60) z = 0.0f;                       // |y| / x < -2^60
+  else z = crb_atanf_libm(fabsf(__fdiv_rn(y, x)));
+  switch (m) {
+    case 0: return z;
+    case 1: return -z;
+    case 2: return __fsub_rn(pi, __fsub_rn(z, pi_lo));
+    default: return __fsub_rn(__fsub_rn(z, pi_lo), pi);
+  }
 }

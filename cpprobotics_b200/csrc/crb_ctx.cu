@@ -82,6 +82,7 @@ int crb_destroy(crb_ctx* ctx) {
   if (ctx->scratch) cudaFree(ctx->scratch);
   if (ctx->mpc_ws) cudaFree(ctx->mpc_ws);
   if (ctx->grid_ws) cudaFree(ctx->grid_ws);
+  if (ctx->rrt_counter) cudaFree(ctx->rrt_counter);
   if (ctx->host_scratch) cudaFreeHost(ctx->host_scratch);
   if (ctx->ev_start) cudaEventDestroy(ctx->ev_start);
   if (ctx->ev_stop) cudaEventDestroy(ctx->ev_stop);

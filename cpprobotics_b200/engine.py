@@ -19,6 +19,7 @@ Method names follow the reference functions they replace:
   grid_box_of_obstacles      <- a_star_planning() / dijkstra_star_planning() :115-140 (obstacle cells, the box)
   Engine.grid_obstacle_map   <- calc_obstacle_map()                              src/a_star.cpp:48-78
   Engine.grid_plan           <- a_star_planning() / dijkstra_star_planning()     src/a_star.cpp:110-244, src/dijkstra.cpp
+  Engine.rrt_plan            <- RRT::planning()                                  include/rrt.h:75-159
 
 All arrays are SoA field-major float32 (`[fields, n]`, C-contiguous); see include/crb.h.  Methods
 without a suffix take CUDA tensors (torch is only the device allocator / stream owner); `*_host`
@@ -34,7 +35,7 @@ from typing import Optional
 import numpy as np
 
 from . import _lib
-from ._lib import DwaParams, EkfParams, GridBox, MpcParams, MptgParams, PfParams, check, load_library
+from ._lib import DwaParams, EkfParams, GridBox, MpcParams, MptgParams, PfParams, RrtParams, check, load_library
 
 try:  # torch is the device-memory / stream / distributed plumbing, never the compute path
     import torch
@@ -78,6 +79,13 @@ def slp_default_params():
     p, v = MptgParams(), C.c_float(0.0)
     load_library().crb_slp_default_params(C.byref(p), C.byref(v))
     return p, float(v.value)
+
+
+def rrt_default_params() -> RrtParams:
+    """RRT's constructor defaults (expand_dis 1.0, goal_sample_rate 5, max_iter 500) and the demo's rand_area {-2, 15}."""
+    p = RrtParams()
+    load_library().crb_rrt_default_params(C.byref(p))
+    return p
 
 
 def grid_box_of_obstacles(ox, oy, reso: float) -> GridBox:
@@ -646,6 +654,56 @@ class Engine:
             _ptr(cost, np.float32, device=True, name="cost"), _ptr(n_visited, np.int32, device=True, name="n_visited"),
             _ptr(status, np.int32, device=True, name="status")), "crb_grid_plan_batched")
         return dict(path=path, path_len=path_len, cost=cost, n_visited=n_visited, status=status)
+
+    # ---- RRT ----------------------------------------------------------------------------------------------------
+    @staticmethod
+    def rrt_default_params() -> RrtParams:
+        return rrt_default_params()
+
+    def rrt_plan(self, ob, se, seed, params: Optional[RrtParams] = None, max_pts: int = 0, max_nodes: int = 0,
+                 path=None, path_len=None, tree=None, parent=None, n_nodes=None, n_iter=None, status=None):
+        """RRT::planning() for n seeded queries on one obstacle list: ob [n_ob, 3] float32 rows (x, y, r), se [4, n]
+        float32 (sx, sy, gx, gy), seed [n] int32 or uint32 bits (goal_gen.seed(seed[i])).  Returns dict(path [2*max_pts,
+        n] (point k's x, y in rows 2k, 2k+1, the goal first, the start last; NaN past path_len), path_len, tree
+        [2*max_nodes, n] (node k's x, y in rows 2k, 2k+1; NaN past n_nodes), parent [max_nodes, n] (-1 for the start
+        and past n_nodes), n_nodes, n_iter, status (CRB_RRT_*)), allocating what is not given (path / tree / parent
+        None when their capacity is 0).  CUDA tensors; only enqueues (the first call on an Engine allocates the query
+        counter)."""
+        n = int(se.shape[-1])
+        _shape(se, 4, n, "se")
+        _shape(seed, 1, n, "seed")
+        if ob.dim() != 2 or int(ob.shape[1]) != 3:
+            raise ValueError(f"ob: expected shape (n_ob, 3), got {tuple(ob.shape)}")
+        if seed.dtype not in (torch.int32, torch.uint32):
+            raise TypeError(f"seed: expected int32 or uint32, got {seed.dtype}")
+        if not seed.is_cuda or not seed.is_contiguous():
+            raise ValueError("seed: expected a contiguous CUDA tensor")
+        prm = params if params is not None else rrt_default_params()
+        dev = se.device
+        full = lambda rows, v, dt: torch.full((rows, n), v, dtype=dt, device=dev)  # noqa: E731
+        if path is None and max_pts > 0:
+            path = full(2 * max_pts, float("nan"), torch.float32)
+        if tree is None and max_nodes > 0:
+            tree = full(2 * max_nodes, float("nan"), torch.float32)
+        if parent is None and max_nodes > 0:
+            parent = full(max_nodes, -1, torch.int32)
+        for a, rows, name in ((path, 2 * max_pts, "path"), (tree, 2 * max_nodes, "tree"), (parent, max_nodes, "parent")):
+            if a is not None:
+                _shape(a, rows, n, name)
+        i32 = lambda a: a if a is not None else torch.empty(n, dtype=torch.int32, device=dev)  # noqa: E731
+        path_len, n_nodes, n_iter, status = i32(path_len), i32(n_nodes), i32(n_iter), i32(status)
+        for a, name in ((path_len, "path_len"), (n_nodes, "n_nodes"), (n_iter, "n_iter"), (status, "status")):
+            _shape(a, 1, n, name)
+        check(self.lib.crb_rrt_plan_batched(
+            self.ctx, C.byref(prm), _ptr(ob, np.float32, device=True, name="ob"), int(ob.shape[0]), n,
+            _ptr(se, np.float32, device=True, name="se"), seed.data_ptr(), int(max_pts),
+            _ptr(path, np.float32, device=True, name="path"), _ptr(path_len, np.int32, device=True, name="path_len"),
+            int(max_nodes), _ptr(tree, np.float32, device=True, name="tree"),
+            _ptr(parent, np.int32, device=True, name="parent"), _ptr(n_nodes, np.int32, device=True, name="n_nodes"),
+            _ptr(n_iter, np.int32, device=True, name="n_iter"), _ptr(status, np.int32, device=True, name="status")),
+            "crb_rrt_plan_batched")
+        return dict(path=path, path_len=path_len, tree=tree, parent=parent, n_nodes=n_nodes, n_iter=n_iter,
+                    status=status)
 
     # ---- multi-GPU: the communicator lives in libcrb (crb_comm.cu), not in torch --------------------
     @staticmethod

@@ -179,5 +179,22 @@ def run() -> None:
         assert ok, "grid planner GPU result is not bit-identical to the checker"
         print(f"smoke GRID  {'A*' if algo == OG.ASTAR else 'Dijkstra'} 65 queries on the demo map: bit-identical to "
               f"the checker; {int((gr['status'] == 0).sum().item())} found")
+    # RRT: the demo's obstacles and 65 seeded queries on them, every output as the checker
+    from oracle import rrt as OR  # checker only
+    rd = synth.RRT_DEMO
+    rob = synth.rrt_demo_obstacles()
+    rse, rseed = synth.rrt_inputs(65, rob, rd["rand_min"], rd["rand_max"])
+    rp = eng.rrt_default_params()
+    rp.expand_dis, rp.max_iter = rd["expand_dis"], 4096
+    rr = eng.rrt_plan(torch.from_numpy(rob).to(dev), torch.from_numpy(rse).to(dev),
+                      torch.from_numpy(rseed.view(np.int32)).to(dev), rp, max_pts=64, max_nodes=512)
+    torch.cuda.synchronize()
+    ro = OR.plan(dict(rand_min=rp.rand_min, rand_max=rp.rand_max, expand_dis=rp.expand_dis,
+                      goal_sample_rate=rp.goal_sample_rate, max_iter=rp.max_iter), rob, rse, rseed, max_pts=64,
+                 max_nodes=512)
+    ok = all(same_nan(rr[k], ro[k]) for k in ("path", "path_len", "tree", "parent", "n_nodes", "n_iter", "status"))
+    assert ok, "RRT GPU result is not bit-identical to the checker"
+    print(f"smoke RRT   65 queries on the demo map: bit-identical to the checker; "
+          f"{int((rr['status'] == 0).sum().item())} found")
     print(f"smoke ok: {eng.launches} kernel launches through libcrb.so")
     eng.close()

@@ -416,3 +416,50 @@ def grid_inputs(n: int, box, grid_map, reso: float, seed: int = 0xC0FFEE, i0: in
     sg = np.stack([(sx + jit[0]) * reso, (sy + jit[1]) * reso, (gx + jit[2]) * reso, (gy + jit[3]) * reso])
     sg[2] = np.where(corner == 3, np.nan, sg[2])
     return np.ascontiguousarray(sg.astype(np.float32))
+
+
+# src/rrt.cpp: the demo's six circular obstacles (x, y, r), start (0, 0), goal (6, 9), rand_area {-2, 15}, expand_dis 0.5
+# (RRT's other constructor arguments take their defaults: goal_sample_rate 5).
+RRT_DEMO = dict(sx=0.0, sy=0.0, gx=6.0, gy=9.0, rand_min=-2.0, rand_max=15.0, expand_dis=0.5)
+
+
+def rrt_demo_obstacles():
+    """ob [6, 3] float32 rows (x, y, r) in the demo's order."""
+    return np.float32([[5, 5, 1], [3, 6, 2], [3, 8, 2], [3, 10, 2], [7, 5, 2], [9, 5, 2]])
+
+
+def rrt_scatter_obstacles(k: int, lo: float, hi: float, r_min: float = 0.3, r_max: float = 1.2, seed: int = 0x5A77):
+    """ob [k, 3] float32: k circles with centres uniform over [lo, hi)^2 and radii uniform in [r_min, r_max)."""
+    idx = np.arange(k, dtype=np.uint64)
+    return np.ascontiguousarray(np.stack([uniform(seed, 190, idx, lo, hi), uniform(seed, 191, idx, lo, hi),
+                                          uniform(seed, 192, idx, r_min, r_max)], axis=1).astype(np.float32))
+
+
+def rrt_inputs(n: int, ob, lo: float, hi: float, seed: int = 0xC0FFEE, i0: int = 0):
+    """(se [4, n] float32 (sx, sy, gx, gy), seed [n] uint32) for RRT queries on one map ob [k, 3]: query i a function of
+    (seed, i0 + i) and the map only.  Start and goal are uniform over [lo, hi)^2 outside every obstacle (a point inside
+    one is redrawn from the next of 16 streams; after 16 tries it is kept).  One query in 64 is a corner case, by index:
+      1  start == goal          2  the start inside an obstacle (the reference never checks it)"""
+    o = np.asarray(ob, np.float32).reshape(-1, 3)
+    idx = np.arange(i0, i0 + n, dtype=np.uint64)
+
+    def point(stream):
+        px, py = uniform(seed, stream, idx, lo, hi).astype(np.float32), uniform(seed, stream + 1, idx, lo, hi).astype(np.float32)
+        for t in range(1, 16):
+            inside = ((px[:, None] - o[:, 0]) ** 2 + (py[:, None] - o[:, 1]) ** 2 <= o[:, 2] ** 2).any(axis=1) \
+                if o.size else np.zeros(n, bool)
+            if not inside.any():
+                break
+            px = np.where(inside, uniform(seed, stream + 2 * t, idx, lo, hi), px).astype(np.float32)
+            py = np.where(inside, uniform(seed, stream + 2 * t + 1, idx, lo, hi), py).astype(np.float32)
+        return px, py
+
+    sx, sy = point(200)
+    gx, gy = point(240)
+    corner = idx % np.uint64(64)
+    gx, gy = np.where(corner == 1, sx, gx), np.where(corner == 1, sy, gy)
+    if o.size:
+        sx, sy = np.where(corner == 2, o[0, 0], sx), np.where(corner == 2, o[0, 1], sy)
+    se = np.ascontiguousarray(np.stack([sx, sy, gx, gy]).astype(np.float32))
+    seeds = (splitmix64(idx ^ np.uint64(seed)) >> np.uint64(32)).astype(np.uint32)
+    return se, seeds

@@ -33,6 +33,8 @@
  *   crb_grid_obstacle_map               <- calc_obstacle_map()   src/a_star.cpp:48-78, src/dijkstra.cpp
  *   crb_grid_plan_batched               <- a_star_planning()     src/a_star.cpp:110-244 (with calc_final_path
  *                                          :31-45), dijkstra_star_planning()  src/dijkstra.cpp
+ *   crb_rrt_plan_batched                <- RRT::planning()       include/rrt.h:75-159 (GetNearestNode :161-174,
+ *                                          CollisionCheck :176-181)
  *   crb_stats_*                         <- (no reference counterpart) per-GPU summary statistics, the
  *                                          only thing that ever crosses NVLink (one all-gather).
  *
@@ -572,6 +574,64 @@ int crb_grid_plan_batched(crb_ctx* ctx, int algo, const crb_grid_box* box, const
                           int32_t* n_visited, int32_t* status);
 /* The number of slots (concurrent searches) crb_grid_plan_batched uses for these arguments. */
 int crb_grid_plan_slots(crb_ctx* ctx, int algo, const crb_grid_box* box, int64_t n, int64_t* slots);
+
+/* ---- RRT (include/rrt.h) ----------------------------------------------------------------------------------------- */
+/* Many seeded start / goal queries on one obstacle list.  RRT::planning :75-159 loops until a new node lies within
+ * expand_dis of the goal: goal_gen, a std::mt19937, draws goal_dis (uniform_int_distribution<int>(0, 100)) and, when
+ * that exceeds goal_sample_rate, a random point (rand_x, then rand_y, both area_dis(goal_gen), a
+ * uniform_real_distribution<float>(rand_min, rand_max)), otherwise the goal; GetNearestNode :161-174 picks the first
+ * node with the least (float)(pow(dx, 2) + pow(dy, 2)); the new node lies expand_dis from it towards the sample, at
+ * atan2f / cosf / sinf; CollisionCheck :176-181 rejects it when its point lies inside an obstacle (the draws are
+ * spent, no node is added).  Bit-exact with the reference built for x86-64 with GCC 13 / libstdc++ and glibc 2.39:
+ * the generator and both distributions as libstdc++ computes them, glibc's atan2f / cosf / sinf, the double pow /
+ * sqrt, float arithmetic without contraction (DESIGN.md).  goal_gen is seeded from std::random_device in the
+ * reference; here query i is the reference after goal_gen.seed(seed[i]). */
+typedef struct crb_rrt_params {
+  float rand_min, rand_max; /* rand_area {min, max}: the area random points are drawn from */
+  float expand_dis;         /* distance from the nearest node to a new node, and the goal tolerance */
+  int32_t goal_sample_rate; /* the goal is the sample when goal_dis(goal_gen) <= goal_sample_rate (0..100) */
+  int32_t max_iter;         /* loop passes per query, rejected ones included (the reference has no cap) */
+} crb_rrt_params;
+/* RRT's constructor defaults expand_dis 1.0, goal_sample_rate 5 and max_iter 500 (the reference ignores its
+ * max_iter; here it is the cap).  rand_area has no default in the reference: the demo's {-2, 15} (src/rrt.cpp) is
+ * filled in. */
+void crb_rrt_default_params(crb_rrt_params* p);
+/* Limits: rand_min <= rand_max, both finite, expand_dis finite, 1 <= max_iter <= CRB_RRT_MAX_ITER; otherwise
+ * CRB_ERR_INVALID_ARG before any device work.  A query keeps its nodes (8 bytes each) and parents (2 bytes each) in
+ * shared memory with the generator's state (2496 bytes): at CRB_RRT_MAX_ITER that is 166 KB, within one H100 SM's
+ * 227 KB for a block. */
+#define CRB_RRT_MAX_ITER 16384
+
+/* Per-query status of crb_rrt_plan_batched. */
+#define CRB_RRT_FOUND 0     /* a node was accepted within expand_dis of the goal */
+#define CRB_RRT_MAX_ITER_REACHED 1 /* max_iter passes without reaching the goal (the reference keeps looping) */
+#define CRB_RRT_BAD_INPUT 2        /* a non-finite start, goal or obstacle value, or a nearest-node search with no winner
+                                      (every distance NaN or >= FLT_MAX: the reference reads node_list[-1]) */
+
+/* RRT::planning for n queries.
+ *   prm: shared by the batch (host pointer)
+ *   ob [n_ob][3] rows (x, y, r): circles shared by the batch (n_ob >= 0; NULL allowed when n_ob = 0)
+ *   se [4][n] (sx, sy, gx, gy), seed [n] uint32 (goal_gen.seed(seed[q]))
+ *   optional outputs, NULL = not written:
+ *     path [2*max_pts][n]  field 2k + j = component j (x, y) of point k of planning()'s result: the goal, then the last
+ *                          node and its parents down to, but not including, the start, then the start; only the first
+ *                          min(path_len, max_pts) points are written, the rest is left as it is
+ *     path_len [n]         int32: the full number of points (0 unless FOUND)
+ *     tree [2*max_nodes][n], parent [max_nodes][n]
+ *                          node_list in insertion order (node 0 is the start) and each node's parent as an index (-1
+ *                          for the start); the first min(n_nodes, max_nodes) nodes are written, also for
+ *                          MAX_ITER_REACHED
+ *     n_nodes [n]          int32: nodes in node_list (0 for a BAD_INPUT found before the loop)
+ *     n_iter [n]           int32: loop passes made, rejected ones included
+ *     status [n]           int32: CRB_RRT_*
+ * One warp per query: the lanes split the nearest-node scan and the obstacle test, and twist the generator together;
+ * persistent warps take queries from an atomic counter.  The first call on a context allocates that counter (4 bytes
+ * of device memory, kept until crb_destroy), so it cannot be captured in a CUDA graph; later calls only enqueue (a
+ * memset and one kernel) and can.  DEVICE pointers (ob, se, seed may be NULL when n = 0: a no-op). */
+int crb_rrt_plan_batched(crb_ctx* ctx, const crb_rrt_params* prm, const float* ob, int32_t n_ob, int64_t n,
+                         const float* se, const uint32_t* seed, int32_t max_pts, float* path, int32_t* path_len,
+                         int32_t max_nodes, float* tree, int32_t* parent, int32_t* n_nodes, int32_t* n_iter,
+                         int32_t* status);
 
 /* ---- multi-GPU: communicator owned by the context (NCCL, opened at run time) ---------------------- */
 /* The batch shards over GPUs by contiguous agent ranges (one crb_ctx per device, one host thread or process

@@ -15,6 +15,7 @@
 //                                                            src/state_lattice_planner.cpp:47-155
 //   a_star_planning(sx, sy, gx, gy, ox, oy, reso, rr), dijkstra_star_planning(...)
 //                                                            src/a_star.cpp:110-244, src/dijkstra.cpp
+//   Node, RRT(start, end, ob_list, rand_area, expand_dis, ...).planning()   include/rrt.h:21-159
 //
 // Eigen is not a dependency: crb::Mat<R,C> is a POD with the memory layout of
 // Eigen::Matrix<float,R,C> (column-major, contiguous, no padding), enough of its interface for the
@@ -29,7 +30,9 @@
 #include <algorithm>
 #include <array>
 #include <cmath>
+#include <cstdint>
 #include <cstring>
+#include <memory>
 #include <random>
 #include <stdexcept>
 #include <string>
@@ -751,6 +754,122 @@ inline std::vector<std::vector<std::vector<float>>> dijkstra_star_planning(std::
                                                                            float rr) {
   return detail::grid_plan(CRB_GRID_DIJKSTRA, sx, sy, gx, gy, ox_, oy_, reso, rr);
 }
+}  // namespace cpprobotics
+
+// include/rrt.h:21-159.  Node has the reference's members and constructor.  RRT has its constructor (path_resolution is
+// kept and unused, as there) and planning() returns what the reference's does: end, then the last node and its parents
+// down to, not including, the start, then start, each node's parent the next element (end's and start's stay NULL).
+// goal_gen is seeded from std::random_device as in the reference; seed(s) makes the next planning() call the
+// reference's after goal_gen.seed(s).  The reference loops until it finds a path and ignores max_iter; here max_iter
+// is raised to CRB_RRT_MAX_ITER and a query that is not FOUND within it (crb.h's CRB_RRT_* statuses) throws.  The
+// batched overload plans every (starts[i], ends[i]) with goal_gen.seed(seeds[i]) on this RRT's obstacles in one
+// launch.  The RRT object owns the nodes it returns (the reference leaks them).
+namespace cpprobotics {
+class Node {
+ public:
+  float x;
+  float y;
+  std::vector<float> path_x;
+  std::vector<float> path_y;
+  Node* parent;
+  float cost;
+  Node(float x_, float y_) : x(x_), y(y_), parent(NULL), cost(0) {}
+};
+
+class RRT {
+ public:
+  RRT(Node* start_, Node* end_, std::vector<std::vector<float> > ob_list_, std::vector<float> rand_area_,
+      float expand_dis_ = 1.0, float path_resolution_ = 1.0, int goal_sample_rate_ = 5, int max_iter_ = 500)
+      : start(start_), end(end_), expand_dis(expand_dis_), path_resolution(path_resolution_),
+        goal_sample_rate(goal_sample_rate_), max_iter(max_iter_), ob_list(ob_list_), rand_area(rand_area_),
+        next_seed(std::random_device()()) {
+    if (rand_area.size() != 2) throw std::runtime_error("RRT: rand_area needs {min, max}");
+  }
+  // the next planning() is the reference's after goal_gen.seed(s)
+  void seed(uint32_t s) { next_seed = s; }
+
+  std::vector<Node*> planning() {
+    std::vector<std::vector<Node*> > r = planning({start}, {end}, {next_seed});
+    next_seed = std::random_device()();
+    return r[0];
+  }
+
+  std::vector<std::vector<Node*> > planning(const std::vector<Node*>& starts, const std::vector<Node*>& ends,
+                                            const std::vector<uint32_t>& seeds) {
+    const size_t n = starts.size();
+    if (ends.size() != n || seeds.size() != n) throw std::runtime_error("RRT: starts, ends, seeds differ in length");
+    std::vector<std::vector<Node*> > out(n);
+    if (n == 0) return out;
+    crb_ctx* ctx = crb::Session::get();
+    crb_rrt_params prm;
+    prm.rand_min = rand_area[0];
+    prm.rand_max = rand_area[1];
+    prm.expand_dis = expand_dis;
+    prm.goal_sample_rate = goal_sample_rate;
+    prm.max_iter = CRB_RRT_MAX_ITER;
+    const size_t no = ob_list.size();
+    std::vector<float> h(3 * no + 5 * n);  // ob [no][3] | se [4][n] | seed [n]
+    for (size_t j = 0; j < no; ++j) {
+      if (ob_list[j].size() < 3) throw std::runtime_error("RRT: an obstacle needs {x, y, r}");
+      for (int c = 0; c < 3; ++c) h[3 * j + c] = ob_list[j][c];
+    }
+    for (size_t i = 0; i < n; ++i) {
+      h[3 * no + i] = starts[i]->x;
+      h[3 * no + n + i] = starts[i]->y;
+      h[3 * no + 2 * n + i] = ends[i]->x;
+      h[3 * no + 3 * n + i] = ends[i]->y;
+      std::memcpy(&h[3 * no + 4 * n + i], &seeds[i], 4);
+    }
+    int max_pts = 256;
+    for (;;) {
+      // ob, se, seed | len, status [2n] | path [2 max_pts n]
+      float* d = crb::Session::scratch(h.size() + 2 * n + 2 * (size_t)max_pts * n);
+      float *dse = d + 3 * no, *dls = dse + 5 * n, *dpath = dls + 2 * n;
+      crb::check(crb_memcpy_h2d(ctx, d, h.data(), h.size() * sizeof(float)), "h2d");
+      crb::check(crb_rrt_plan_batched(ctx, &prm, d, (int32_t)no, (int64_t)n, dse, (const uint32_t*)(dse + 4 * n),
+                                      max_pts, dpath, (int32_t*)dls, 0, nullptr, nullptr, nullptr, nullptr,
+                                      (int32_t*)(dls + n)),
+                 "crb_rrt_plan_batched");
+      std::vector<int32_t> ls(2 * n);
+      crb::check(crb_memcpy_d2h(ctx, ls.data(), dls, ls.size() * sizeof(int32_t)), "d2h");
+      int longest = 0;
+      for (size_t i = 0; i < n; ++i) {
+        if (ls[n + i] != CRB_RRT_FOUND)
+          throw std::runtime_error("RRT::planning: no path (status " + std::to_string(ls[n + i]) + ")");
+        if (ls[i] > longest) longest = ls[i];
+      }
+      if (longest > max_pts) {  // again with room for every whole path
+        max_pts = longest;
+        continue;
+      }
+      std::vector<float> p(2 * (size_t)max_pts * n);
+      crb::check(crb_memcpy_d2h(ctx, p.data(), dpath, p.size() * sizeof(float)), "d2h");
+      for (size_t i = 0; i < n; ++i) {
+        std::vector<Node*>& path = out[i];
+        path.push_back(ends[i]);
+        for (int k = 1; k + 1 < ls[i]; ++k) {
+          owned.emplace_back(new Node(p[(2 * (size_t)k) * n + i], p[(2 * (size_t)k + 1) * n + i]));
+          path.push_back(owned.back().get());
+        }
+        path.push_back(starts[i]);
+        for (size_t k = 1; k + 1 < path.size(); ++k) path[k]->parent = path[k + 1];
+      }
+      return out;
+    }
+  }
+
+ protected:
+  Node* start;
+  Node* end;
+  const float expand_dis;
+  const float path_resolution;
+  const int goal_sample_rate;
+  const int max_iter;
+  const std::vector<std::vector<float> > ob_list;
+  std::vector<float> rand_area;
+  uint32_t next_seed;
+  std::vector<std::unique_ptr<Node> > owned;
+};
 }  // namespace cpprobotics
 
 #endif  // CRB_REFERENCE_API_HPP_
