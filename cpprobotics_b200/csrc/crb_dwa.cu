@@ -203,6 +203,25 @@ crb_dwa_motion_kernel(int64_t n, float* __restrict__ xg, const float* __restrict
 
 static bool finite_pos(float v) { return isfinite(v) && v > 0.0f; }
 
+// Spacing of binary32 values at magnitude x >= 0 (x in double; 2^-149 below the normal range).
+static double ulp_f32(double x) {
+  if (x < 0x1p-126) return 0x1p-149;
+  int e = 0;
+  frexp(x, &e);  // x = m 2^e, m in [0.5, 1)
+  return ldexp(1.0, e - 24);
+}
+
+// Largest number of samples the reference's float loop `for (s = lo; s <= hi; s += reso)` (:126-127) can take on
+// one axis, plus one, for any state.  Every sample lies in [-m, m] (the window is clipped to the limits), so each
+// step s + reso rounds to at least d = reso - ulp(m + reso) / 2 above s; d <= 0 means a step can stall, and the
+// result is infinite.  The window's width is at most `range` (the limits) and at most 2 fl(half) plus half an ulp
+// of m for each of its rounded ends.  The extra sample of margin absorbs this function's own double rounding.
+static double dwa_axis_samples(double m, float reso, float half, double range) {
+  const double d = reso - 0.5 * ulp_f32(m + reso);
+  if (!(d > 0.0)) return INFINITY;
+  return fmin(2.0 * half + ulp_f32(m), range) / d + 2.0;
+}
+
 // Parameter limits of crb.h; *n_steps = the reference's rollout step count (:67-72), itself bounded.
 static int dwa_check_params(const crb_dwa_params* p, int* n_steps) {
   CRB_REQUIRE(p != nullptr, "params is NULL");
@@ -210,11 +229,14 @@ static int dwa_check_params(const crb_dwa_params* p, int* n_steps) {
   for (int k = 0; k < 12; ++k) CRB_REQUIRE(isfinite(f[k]), "every parameter must be finite");
   CRB_REQUIRE(finite_pos(p->v_reso) && finite_pos(p->yawrate_reso) && finite_pos(p->dt),
               "v_reso, yawrate_reso and dt must be > 0");
-  const double wv = fmin(2.0 * p->max_accel * p->dt, (double)p->max_speed - p->min_speed);
-  CRB_REQUIRE(wv / p->v_reso + 2.0 <= CRB_DWA_MAX_SPEED_SAMPLES,
+  // the kernel's max_accel * dt and max_dyawrate * dt: a float product, formed exactly in double and rounded once
+  const float hv = (float)((double)p->max_accel * p->dt), hw = (float)((double)p->max_dyawrate * p->dt);
+  const double mv = fmax(fabs((double)p->min_speed), fabs((double)p->max_speed));
+  CRB_REQUIRE(dwa_axis_samples(mv, p->v_reso, hv, (double)p->max_speed - p->min_speed) <=
+                  CRB_DWA_MAX_SPEED_SAMPLES,
               "the speed window allows more than CRB_DWA_MAX_SPEED_SAMPLES samples");
-  const double ww = fmin(2.0 * p->max_dyawrate * p->dt, 2.0 * (double)p->max_yawrate);
-  CRB_REQUIRE(ww / p->yawrate_reso + 2.0 <= CRB_DWA_MAX_YAWRATE_SAMPLES,
+  CRB_REQUIRE(dwa_axis_samples(fabs((double)p->max_yawrate), p->yawrate_reso, hw, 2.0 * (double)p->max_yawrate) <=
+                  CRB_DWA_MAX_YAWRATE_SAMPLES,
               "the yaw-rate window allows more than CRB_DWA_MAX_YAWRATE_SAMPLES samples");
   float t = 0.0f;
   int k = 0;

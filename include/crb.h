@@ -337,11 +337,13 @@ typedef struct crb_dwa_params {
 void crb_dwa_default_params(crb_dwa_params* p);
 
 /* Limits.  Every parameter must be finite, v_reso, yawrate_reso and dt > 0, and
- *   min(2 max_accel dt, max_speed - min_speed) / v_reso + 2          <= CRB_DWA_MAX_SPEED_SAMPLES
- *   min(2 max_dyawrate dt, 2 max_yawrate) / yawrate_reso + 2         <= CRB_DWA_MAX_YAWRATE_SAMPLES
- *   rollout steps (the reference's `time += dt` loop, :67-72)        <= CRB_DWA_MAX_STEPS
- * otherwise CRB_ERR_INVALID_ARG.  A window is sampled by the reference's float accumulation (:126-127); for a
- * state so large that v + v_reso == v the reference never terminates, here the axis stops at its cap. */
+ *   min(2 fl(max_accel dt) + ulp(Mv), max_speed - min_speed) / dv + 2      <= CRB_DWA_MAX_SPEED_SAMPLES
+ *   min(2 fl(max_dyawrate dt) + ulp(Mw), 2 max_yawrate) / dw + 2           <= CRB_DWA_MAX_YAWRATE_SAMPLES
+ *   rollout steps (the reference's `time += dt` loop, :67-72)              <= CRB_DWA_MAX_STEPS
+ * otherwise CRB_ERR_INVALID_ARG.  Here Mv = max(|min_speed|, |max_speed|), Mw = |max_yawrate|, ulp is the float
+ * spacing at a magnitude, and dv = v_reso - ulp(Mv + v_reso) / 2, dw = yawrate_reso - ulp(Mw + yawrate_reso) / 2
+ * must be > 0.  A window is sampled by the reference's float accumulation (:126-127), whose every sum rounds to
+ * at least dv (dw) above the last sample, so for any state it takes fewer samples than the cap and ends. */
 #define CRB_DWA_MAX_OBSTACLES 256
 #define CRB_DWA_MAX_SPEED_SAMPLES 64
 #define CRB_DWA_MAX_YAWRATE_SAMPLES 512

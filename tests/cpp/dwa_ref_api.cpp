@@ -1,7 +1,9 @@
 // A dynamic_window_approach.cpp-style program on include/crb/reference_api.hpp: its own Config class and the
 // reference's type aliases, dwa_control() and motion() called with the reference's signatures.
-// Usage: dwa_ref_api in.bin out.bin
+// Usage: dwa_ref_api in.bin out.bin [config.bin]
 //   in:  float32 m, n_ob, then m robots of (x[5], u[2], goal[2]), then n_ob rows (ox, oy)
+//   config (optional, else Config's defaults): float32 max_speed, min_speed, max_yawrate, max_accel, robot_radius,
+//        max_dyawrate, v_reso, yawrate_reso, dt, predict_time, to_goal_cost_gain, speed_cost_gain
 //   out: float32 per robot: u[2], n_pts, the returned trajectory (n_pts x 5), motion(x, u, config.dt)[5]
 #include <array>
 #include <cstdio>
@@ -34,7 +36,7 @@ class Config {
 };
 
 int main(int argc, char** argv) {
-  if (argc != 3) return 2;
+  if (argc != 3 && argc != 4) return 2;
   FILE* in = std::fopen(argv[1], "rb");
   if (!in) return 2;
   std::vector<float> buf;
@@ -46,6 +48,26 @@ int main(int argc, char** argv) {
   Obstacle ob;
   for (int k = 0; k < n_ob; ++k) ob.push_back(Point{{r[9 * m + 2 * k], r[9 * m + 2 * k + 1]}});
   Config config;
+  if (argc == 4) {  // set member by member, the way a program configures its own robot
+    float c[12];
+    FILE* cf = std::fopen(argv[3], "rb");
+    if (!cf) return 2;
+    const size_t got = std::fread(c, sizeof(float), 12, cf);
+    std::fclose(cf);
+    if (got != 12) return 2;
+    config.max_speed = c[0];
+    config.min_speed = c[1];
+    config.max_yawrate = c[2];
+    config.max_accel = c[3];
+    config.robot_radius = c[4];
+    config.max_dyawrate = c[5];
+    config.v_reso = c[6];
+    config.yawrate_reso = c[7];
+    config.dt = c[8];
+    config.predict_time = c[9];
+    config.to_goal_cost_gain = c[10];
+    config.speed_cost_gain = c[11];
+  }
   std::vector<float> out;
   try {
     for (int i = 0; i < m; ++i, r += 9) {
