@@ -570,7 +570,9 @@ int crb_grid_obstacle_map(crb_ctx* ctx, int64_t n_obs, const float* ox, const fl
  * One thread per query (a search is serial: its pop order is the result); persistent lanes take queries from an
  * atomic counter.  The slots' workspace is a grow-only buffer of the context: the first call at a larger
  * W * H * slots allocates (and synchronises the stream), so it cannot be captured in a CUDA graph; later calls only
- * enqueue (a memset and one kernel) and can.  DEVICE pointers, NULL allowed when n = 0. */
+ * enqueue (a memset and one kernel) and can.  Growing frees the old buffer, so a graph captured before a call that
+ * grew the workspace must not be replayed after it: its kernel would use freed device memory.  Capture again (or
+ * make the largest call before capturing).  DEVICE pointers, NULL allowed when n = 0. */
 int crb_grid_plan_batched(crb_ctx* ctx, int algo, const crb_grid_box* box, const uint8_t* map, float reso, int64_t n,
                           const float* sg, int max_pts, float* path, int32_t* path_len, float* cost,
                           int32_t* n_visited, int32_t* status);

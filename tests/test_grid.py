@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 
 import grid_cases as GC
+from grid_cases import same
 from cpprobotics_b200 import _lib, grid_box_of_obstacles, synth
 from oracle import grid as OG
 
@@ -21,17 +22,6 @@ GOLDEN = os.path.join(ROOT, "tests", "golden", "grid_golden.npz")
 CPP_API = os.path.join(ROOT, "tests", "cpp", "grid_ref_api.cpp")
 CPP_HEAP = os.path.join(ROOT, "tests", "cpp", "grid_heap_pin.cpp")
 ALGO_IDS = [a for a, _ in GC.ALGOS]
-
-
-def same(a, b):
-    """Bitwise equal, except that any NaN equals any NaN."""
-    a, b = np.asarray(a), np.asarray(b)
-    if a.shape != b.shape or a.dtype != b.dtype:
-        return False
-    if a.dtype.kind != "f":
-        return np.array_equal(a, b)
-    na, nb = np.isnan(a), np.isnan(b)
-    return np.array_equal(na, nb) and np.array_equal(a[~na].view(np.uint32), b[~nb].view(np.uint32))
 
 
 def _ref(algo):
