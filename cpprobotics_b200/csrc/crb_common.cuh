@@ -35,7 +35,6 @@ struct crb_ctx {
   // per-device function attributes already set for this context's device (a second context on another
   // device in the same process must set them again, so these are not process-global latches)
   int mpc_tasks_attr_set;
-  int ekf_tma_attr_set;
   int pf_step_attr_set;   // shared-memory carve-out preference of the crb_pf_step kernels (per device)
   int mpc_v0_attr_set;
   // NCCL communicator (crb_comm.cu); NULL = single GPU

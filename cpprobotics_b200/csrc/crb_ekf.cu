@@ -21,7 +21,6 @@
 // an infinite input the dense 0 * inf makes NaN of every entry, also of those this kernel computes without
 // that input (tests/test_ekf_edges.py).
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "crb_common.cuh"
 
@@ -178,168 +177,6 @@ crb_ekf_step_kernel(int64_t count, int64_t ld, float* __restrict__ x, float* __r
   for (int f = 0; f < 16; ++f) st_agents<V>(P + f * lds + is, Ps[f]);
 }
 
-// ---------------------------------------------------------------------------------------------------
-// TMA-staged variant (CRB_EKF_VARIANT=4): persistent CTAs, each tile of EKF_TILE agents is brought into
-// shared memory by 24 bulk async copies (cp.async.bulk, one 512-byte row segment per field; SASS: UBLKCP)
-// that complete on an mbarrier, EKF_STAGES tiles deep, and leaves through 20 bulk stores.  Loads of
-// tile k+S are in flight while tile k is computed without holding registers.  A/B against the
-// direct-load kernel in DESIGN.md 3.
-// ---------------------------------------------------------------------------------------------------
-#define EKF_NIN 24
-#define EKF_NOUT 20
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)),
-               "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok = 0;
-  while (!ok) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  }
-}
-__device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src, uint32_t bytes,
-                                         uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-          smem_u32(dst_smem)),
-      "l"(src), "r"(bytes), "r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void bulk_s2g(void* dst, const void* src_smem, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst),
-               "r"(smem_u32(src_smem)), "r"(bytes)
-               : "memory");
-}
-
-template <int EKF_TILE, int EKF_STAGES>
-__global__ void __launch_bounds__(EKF_TILE)
-crb_ekf_step_tma_kernel(int64_t count, int64_t ld, float* __restrict__ x, float* __restrict__ P,
-                        const float* __restrict__ z, const float* __restrict__ u, int64_t ld_zu,
-                        EkfArgs a) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  float* sin_ = (float*)smem_raw;                                        // [STAGES][NIN][TILE]
-  float* sout = sin_ + EKF_STAGES * EKF_NIN * EKF_TILE;                  // [2][NOUT][TILE]
-  uint64_t* full = (uint64_t*)(sout + 2 * EKF_NOUT * EKF_TILE);          // [STAGES]
-  const int tid = threadIdx.x;
-  const int64_t ntiles = (count + EKF_TILE - 1) / EKF_TILE;
-  if (tid == 0) {
-    for (int s = 0; s < EKF_STAGES; ++s) mbar_init(&full[s], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-
-  auto issue_loads = [&](int64_t tile, int stage) {  // thread 0 only
-    const int64_t i0 = tile * EKF_TILE;
-    const uint32_t cnt = (uint32_t)((count - i0) < EKF_TILE ? (count - i0) : EKF_TILE);
-    const uint32_t bytes = cnt * 4u;
-    float* dst = sin_ + (size_t)stage * EKF_NIN * EKF_TILE;
-    mbar_expect_tx(&full[stage], bytes * EKF_NIN);
-#pragma unroll
-    for (int f = 0; f < 4; ++f) bulk_g2s(dst + f * EKF_TILE, x + f * ld + i0, bytes, &full[stage]);
-#pragma unroll
-    for (int f = 0; f < 16; ++f)
-      bulk_g2s(dst + (4 + f) * EKF_TILE, P + f * ld + i0, bytes, &full[stage]);
-#pragma unroll
-    for (int f = 0; f < 2; ++f) {
-      bulk_g2s(dst + (20 + f) * EKF_TILE, z + f * ld_zu + i0, bytes, &full[stage]);
-      bulk_g2s(dst + (22 + f) * EKF_TILE, u + f * ld_zu + i0, bytes, &full[stage]);
-    }
-  };
-
-  // prologue: fill the pipeline
-  if (tid == 0) {
-    for (int s = 0; s < EKF_STAGES; ++s) {
-      const int64_t t = (int64_t)blockIdx.x + (int64_t)s * gridDim.x;
-      if (t < ntiles) issue_loads(t, s);
-    }
-  }
-  int k = 0;
-  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++k) {
-    const int stage = k % EKF_STAGES;
-    const uint32_t parity = (uint32_t)((k / EKF_STAGES) & 1);
-    const int ob = k & 1;
-    const int64_t i0 = tile * EKF_TILE;
-    const bool active = i0 + tid < count;
-    mbar_wait(&full[stage], parity);
-    const float* si = sin_ + (size_t)stage * EKF_NIN * EKF_TILE + tid;
-    float xs[4], Ps[16];
-#pragma unroll
-    for (int f = 0; f < 4; ++f) xs[f] = si[f * EKF_TILE];
-#pragma unroll
-    for (int f = 0; f < 16; ++f) Ps[f] = si[(4 + f) * EKF_TILE];
-    const float z0 = si[20 * EKF_TILE], z1 = si[21 * EKF_TILE];
-    const float u0 = si[22 * EKF_TILE], u1 = si[23 * EKF_TILE];
-    // the bulk store issued two tiles ago must have finished READING sout[ob] before it is rewritten
-    if (tid == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-    __syncthreads();  // every thread has its inputs in registers: the stage can be refilled
-    if (tid == 0) {
-      const int64_t nt = tile + (int64_t)EKF_STAGES * gridDim.x;
-      if (nt < ntiles) issue_loads(nt, stage);
-    }
-    if (active) ekf_step(xs, Ps, z0, z1, u0, u1, a);
-    float* so = sout + (size_t)ob * EKF_NOUT * EKF_TILE + tid;
-#pragma unroll
-    for (int f = 0; f < 4; ++f) so[f * EKF_TILE] = xs[f];
-#pragma unroll
-    for (int f = 0; f < 16; ++f) so[(4 + f) * EKF_TILE] = Ps[f];
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic writes -> async proxy
-    __syncthreads();
-    if (tid == 0) {
-      const uint32_t cnt = (uint32_t)((count - i0) < EKF_TILE ? (count - i0) : EKF_TILE);
-      const uint32_t bytes = cnt * 4u;
-      const float* src = sout + (size_t)ob * EKF_NOUT * EKF_TILE;
-#pragma unroll
-      for (int f = 0; f < 4; ++f) bulk_s2g(x + f * ld + i0, src + f * EKF_TILE, bytes);
-#pragma unroll
-      for (int f = 0; f < 16; ++f) bulk_s2g(P + f * ld + i0, src + (4 + f) * EKF_TILE, bytes);
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    }
-  }
-  if (tid == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-}
-
-static size_t ekf_tma_smem_bytes(int tile, int stages) {
-  return (size_t)(stages * EKF_NIN + 2 * EKF_NOUT) * tile * sizeof(float) + stages * sizeof(uint64_t);
-}
-
-template <int TILE, int STAGES>
-static int ekf_tma_launch(crb_ctx* ctx, cudaStream_t st, int64_t count, int64_t ld, float* x,
-                          float* P, const float* z, const float* u, int64_t ld_zu,
-                          const EkfArgs& a) {
-  // per-context latch (bit per instantiation): the attribute is per device, and a process may hold contexts
-  // on several devices
-  const size_t smem = ekf_tma_smem_bytes(TILE, STAGES);
-  const int bit = 1 << ((TILE == 256 ? 2 : 0) + (STAGES == 3 ? 1 : 0));
-  if (!(ctx->ekf_tma_attr_set & bit)) {
-    CRB_CUDA(cudaFuncSetAttribute(crb_ekf_step_tma_kernel<TILE, STAGES>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    ctx->ekf_tma_attr_set |= bit;
-  }
-  const int64_t ntiles = (count + TILE - 1) / TILE;
-  int per_sm = (int)((size_t)227 * 1024 / (smem + 1024));
-  if (per_sm * TILE > 2048) per_sm = 2048 / TILE;
-  int grid = ctx->sm_count * (per_sm > 0 ? per_sm : 1);
-  if ((int64_t)grid > ntiles) grid = (int)ntiles;
-  crb_ekf_step_tma_kernel<TILE, STAGES><<<grid, TILE, smem, st>>>(count, ld, x, P, z, u, ld_zu, a);
-  CRB_CUDA(cudaGetLastError());
-  ctx->launches++;
-  return CRB_OK;
-}
-
 static int ekf_launch(crb_ctx* ctx, cudaStream_t st, int64_t count, int64_t ld, float* x, float* P,
                       const float* z, const float* u, int64_t ld_zu, int n_steps,
                       const crb_ekf_params* prm) {
@@ -352,44 +189,15 @@ static int ekf_launch(crb_ctx* ctx, cudaStream_t st, int64_t count, int64_t ld, 
   // independent reads in flight per 256 agents, which covers H100's HBM latency.  Measured at 2^20 agents, 30
   // graph-captured launches over 3 buffer sets, on two H100 80GB HBM3 boxes (700 W limit): the two-agent form runs
   // 4.6 % and 6.4 % faster than the one-agent form, and 4, 2 or 6 CTAs per SM make no difference (DESIGN.md 3).
-  // CRB_EKF_VARIANT selects alternatives for A/B measurements.
-  static int variant = -1;
-  if (variant < 0) {
-    const char* e = getenv("CRB_EKF_VARIANT");
-    variant = e ? atoi(e) : 0;
-  }
-  // bulk copies need 16-byte aligned, 16-byte multiple row segments
-  const bool tma_ok = n_steps == 1 && (ld % 4) == 0 && (ld_zu % 4) == 0 && (count % 4) == 0 &&
-                      (((uintptr_t)x | (uintptr_t)P | (uintptr_t)z | (uintptr_t)u) & 15) == 0;
   // two agents per thread: every row segment a thread touches is 8-byte aligned
   const bool pair_ok = (count % 2) == 0 && (ld % 2) == 0 && (ld_zu % 2) == 0 &&
                        (((uintptr_t)x | (uintptr_t)P | (uintptr_t)z | (uintptr_t)u) & 7) == 0;
-  if (tma_ok && variant == 4) return ekf_tma_launch<128, 3>(ctx, st, count, ld, x, P, z, u, ld_zu, a);
-  if (tma_ok && variant == 5) return ekf_tma_launch<128, 2>(ctx, st, count, ld, x, P, z, u, ld_zu, a);
-  if (tma_ok && variant == 6) return ekf_tma_launch<256, 2>(ctx, st, count, ld, x, P, z, u, ld_zu, a);
-  if (tma_ok && variant == 7) return ekf_tma_launch<256, 3>(ctx, st, count, ld, x, P, z, u, ld_zu, a);
-  switch (variant) {
-    case 1:
-      crb_ekf_step_kernel<256, 4, 1><<<crb_grid_for(count, 256), 256, 0, st>>>(count, ld, x, P, z, u,
-                                                                            ld_zu, n_steps, a);
-      break;
-    case 2:
-      crb_ekf_step_kernel<128, 8, 1><<<crb_grid_for(count, 128), 128, 0, st>>>(count, ld, x, P, z, u,
-                                                                            ld_zu, n_steps, a);
-      break;
-    case 3:
-      crb_ekf_step_kernel<512, 2, 1><<<crb_grid_for(count, 512), 512, 0, st>>>(count, ld, x, P, z, u,
-                                                                            ld_zu, n_steps, a);
-      break;
-    default:
-      if (pair_ok)
-        CRB_CUDA(crb_launch_pdl(crb_ekf_step_kernel<128, 4, 2>, (unsigned)crb_grid_for(count / 2, 128), 128u, st,
-                                count, ld, x, P, z, u, ld_zu, n_steps, a));
-      else
-        CRB_CUDA(crb_launch_pdl(crb_ekf_step_kernel<256, 3, 1>, (unsigned)crb_grid_for(count, 256), 256u, st,
-                                count, ld, x, P, z, u, ld_zu, n_steps, a));
-  }
-  CRB_CUDA(cudaGetLastError());
+  if (pair_ok)
+    CRB_CUDA(crb_launch_pdl(crb_ekf_step_kernel<128, 4, 2>, (unsigned)crb_grid_for(count / 2, 128), 128u, st,
+                            count, ld, x, P, z, u, ld_zu, n_steps, a));
+  else
+    CRB_CUDA(crb_launch_pdl(crb_ekf_step_kernel<256, 3, 1>, (unsigned)crb_grid_for(count, 256), 256u, st,
+                            count, ld, x, P, z, u, ld_zu, n_steps, a));
   ctx->launches++;
   return CRB_OK;
 }
@@ -407,6 +215,7 @@ extern "C" int crb_ekf_step_batched(crb_ctx* ctx, int64_t n, float* x, float* P,
 
 // Host-pointer variant: chunks of agents stream through CRB_N_PIPE staging arenas, each on its own
 // stream (H2D chunk k+1 and D2H chunk k-1 overlap the kernel of chunk k: both copy engines busy).
+constexpr int64_t EKF_HOST_CHUNK = 131072;  // agents per chunk
 extern "C" int crb_ekf_step_batched_host(crb_ctx* ctx, int64_t n, float* x, float* P,
                                          const float* z, const float* u,
                                          const crb_ekf_params* prm, int n_steps) {
@@ -429,13 +238,7 @@ extern "C" int crb_ekf_step_batched_host(crb_ctx* ctx, int64_t n, float* x, floa
       return CRB_OK;
     }
   }
-  static int64_t chunk_pref = 0;  // CRB_EKF_CHUNK overrides the staging chunk (agents) for A/B
-  if (chunk_pref == 0) {
-    const char* e = getenv("CRB_EKF_CHUNK");
-    chunk_pref = e ? atoll(e) : 131072;
-    if (chunk_pref < 1024) chunk_pref = 131072;
-  }
-  const int64_t chunk_cap = n < chunk_pref ? n : chunk_pref;
+  const int64_t chunk_cap = n < EKF_HOST_CHUNK ? n : EKF_HOST_CHUNK;
   const size_t nf = 20 + (size_t)4 * n_steps;  // x4 P16 z2s u2s
   const size_t pitch = (size_t)chunk_cap * sizeof(float);
   for (int s = 0; s < CRB_N_PIPE; ++s) {

@@ -22,7 +22,7 @@ for line in txt.splitlines():
     m = re.match(r"\s+/\*([0-9a-f]{4})\*/\s+(.*?);", line)
     if m and cur is not None:
         funcs[cur].append((m.group(1), m.group(2).strip()))
-HOT = ["crb_ekf_step_kernel<256, 4>", "crb_ekf_step_tma_kernel<256, 2>", "crb_pf_predict_weight_lean_kernel<128, 12>",
+HOT = ["crb_ekf_step_kernel<128, 4, 2>", "crb_ekf_step_kernel<256, 3, 1>", "crb_pf_predict_weight_lean_kernel<128, 12>",
        "crb_mpc_tasks_kernel", "crb_mpc_solve_kernel<0>", "crb_lqr_dlqr_kernel<4, 1>", "crb_probe_ffma_kernel"]
 WATCH = ["FFMA2", "FADD2", "FMUL2", "FFMA", "FMUL", "FADD", "DFMA", "DMUL", "DADD", "MUFU", "UBLKCP", "UTMALDG", "LDGSTS",
          "SYNCS", "LDG", "STG", "LDS", "STS", "ATOMS", "ATOMG", "NANOSLEEP", "SHFL", "VOTE", "HMMA", "UTCHMMA", "UTCQMMA", "BRA"]

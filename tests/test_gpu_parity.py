@@ -392,31 +392,6 @@ def test_stats_reduce(engine):
     assert abs(out[6] - chk) < 1e-7 * n
 
 
-def test_ekf_tma_staged_variant_is_bitwise_the_direct_kernel(engine, tmp_path):
-    """CRB_EKF_VARIANT=4 selects the cp.async.bulk + mbarrier pipelined kernel (same ekf_step code): the
-    results must be bit-identical to the default kernel.  The variant is latched per process, so the
-    staged kernel runs in a child process."""
-    import subprocess
-    import sys
-    import torch
-    n = 300_004          # many tiles per CTA, ragged last tile (multiple of 4)
-    x, P, z, u = synth.ekf_inputs(n)
-    xd, Pd, zd, ud = _dev(x, P, z, u)
-    engine.ekf_estimation(xd, Pd, zd, ud)
-    torch.cuda.synchronize()
-    code = ("import sys, numpy as np, torch; sys.path.insert(0, %r)\n"
-            "from cpprobotics_b200 import Engine, synth\n"
-            "x, P, z, u = synth.ekf_inputs(%d)\n"
-            "e = Engine(0); t = [torch.from_numpy(a).cuda() for a in (x, P, z, u)]\n"
-            "e.ekf_estimation(*t); torch.cuda.synchronize()\n"
-            "np.savez(%r, x=t[0].cpu().numpy(), P=t[1].cpu().numpy())\n") % (
-                os.path.dirname(os.path.dirname(os.path.abspath(__file__))), n, str(tmp_path / "o.npz"))
-    env = dict(os.environ, CRB_EKF_VARIANT="4")
-    subprocess.check_call([sys.executable, "-c", code], env=env)
-    o = np.load(tmp_path / "o.npz")
-    assert np.array_equal(o["x"], xd.cpu().numpy()) and np.array_equal(o["P"], Pd.cpu().numpy())
-
-
 def test_closed_loop_on_device_matches_oracle_step_by_step(engine):
     """mpc_simulation's loop body (:372-376) entirely on the device: calc_ref_trajectory -> mpc_solve ->
     update, several steps without a host round trip.  Each step is checked against the oracle fed with
