@@ -48,6 +48,7 @@ CRB_GRID_FOUND = 0
 CRB_GRID_NO_PATH = 1
 CRB_GRID_START_OUTSIDE = 2
 CRB_GRID_BAD_POINT = 3
+CRB_LQR_TRACK_OK, CRB_LQR_TRACK_DARE_MAXITER, CRB_LQR_TRACK_BAD_INDEX = 0, 1, 2
 CRB_RRT_MAX_ITER = 16384
 CRB_RRT_FOUND = 0
 CRB_RRT_MAX_ITER_REACHED = 1
@@ -98,6 +99,11 @@ class GridBox(C.Structure):
 class RrtParams(C.Structure):
     _fields_ = [("rand_min", C.c_float), ("rand_max", C.c_float), ("expand_dis", C.c_float),
                 ("goal_sample_rate", C.c_int32), ("max_iter", C.c_int32)]
+
+
+class LqrTrackParams(C.Structure):
+    _fields_ = [("dt", C.c_double), ("wheelbase", C.c_double), ("max_steer", C.c_double), ("Q", C.c_float * 25),
+                ("R", C.c_float * 4), ("maxiter", C.c_int32), ("eps", C.c_float)]
 
 
 # name -> (restype, argtypes); every symbol include/crb.h declares
@@ -192,6 +198,13 @@ PROTOTYPES = {
     "crb_rrt_plan_batched": (C.c_int, [C.c_void_p, C.POINTER(RrtParams), C.c_void_p, C.c_int32, C.c_int64, C.c_void_p,
                                        C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "crb_lqr_track_default_params": (None, [C.POINTER(LqrTrackParams), C.c_int]),
+    "crb_lqr_steering_control_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                                   C.POINTER(LqrTrackParams), C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "crb_lqr_update_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.POINTER(LqrTrackParams)]),
     "crb_stats_reduce": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p]),
     "crb_probe_fp32_peak": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),

@@ -426,3 +426,103 @@ __device__ __forceinline__ float crb_atan2f_libm(float y, float x) {
     default: return __fsub_rn(__fsub_rn(z, pi_lo), pi);
   }
 }
+
+// ---- YAW_P2P with the reference's bits --------------------------------------------------------------------
+constexpr double kPi = 3.14159265358979323846;  // M_PI
+constexpr double kTwoPi = 2.0 * kPi;             // 2*M_PI (an exact doubling)
+
+// fmod(a, 2*M_PI), exactly.  fmod is exact in IEEE arithmetic; for |a| < 4 pi (every wrapped yaw) its result is
+// a itself or a -+ 2 pi, and that subtraction is exact (Sterbenz), so the general routine is only needed beyond.
+__device__ __forceinline__ double mptg_fmod_2pi(double a) {
+  const double aa = fabs(a);
+  if (aa < kTwoPi) return a;
+  if (aa < 2.0 * kTwoPi) return copysign(__dsub_rn(aa, kTwoPi), a);  // fmod's result has a's sign
+  return fmod(a, kTwoPi);
+}
+
+// YAW_P2P(angle) :18 on a float, in double, narrowed back to float by the assignment
+__device__ __forceinline__ float mptg_yaw_p2p(float yaw) {
+  double a = mptg_fmod_2pi(__dadd_rn((double)yaw, kPi));
+  a = mptg_fmod_2pi(__dsub_rn(a, kTwoPi));
+  return __double2float_rn(__dadd_rn(a, kPi));
+}
+
+// ---- (float)atan2(y, 1.0) with the HOST libm's bits (DESIGN.md §3.4) ----------------------------------------
+// The LQR programs' feed-forward is float ff = std::atan2(L*k, (double)1.0) (src/lqr_steer_control.cpp:125,
+// src/lqr_speed_steer_control.cpp:142): glibc's binary64 atan2 narrowed to float.  The narrowing is what has to be
+// reproduced, and it only depends on the binary64 result where that result lies within a few binary64 ulps of a
+// float rounding midpoint.  Fast path: CUDA's atan (<= 2 ulp) and glibc's (<= 1 ulp) are both within 3 ulps of the
+// true value's neighbourhood, so when the binary64 values 4 ulps either side of CUDA's result narrow to the same
+// float, that float is glibc's too.  Otherwise atan(y) is evaluated in double-double (relative error ~2^-100) and
+// its correctly rounded binary64 head is narrowed: glibc is correctly rounded wherever that matters, which the census
+// over every non-negative float k with y = 0.5 * k checks (tests/test_lqr_track.py).  Odd in y, as glibc is.
+struct crb_dd { double hi, lo; };
+__device__ __forceinline__ crb_dd crb_dd_fast(double a, double b) {  // |a| >= |b|
+  const double s = __dadd_rn(a, b);
+  return {s, __dsub_rn(b, __dsub_rn(s, a))};
+}
+__device__ __forceinline__ crb_dd crb_dd_add(crb_dd a, crb_dd b) {
+  const double s = __dadd_rn(a.hi, b.hi);
+  const double bb = __dsub_rn(s, a.hi);
+  const double e = __dadd_rn(__dsub_rn(a.hi, __dsub_rn(s, bb)), __dsub_rn(b.hi, bb));
+  return crb_dd_fast(s, __dadd_rn(e, __dadd_rn(a.lo, b.lo)));
+}
+__device__ __forceinline__ crb_dd crb_dd_mul(crb_dd a, crb_dd b) {
+  const double p = __dmul_rn(a.hi, b.hi);
+  const double e = __dadd_rn(__fma_rn(a.hi, b.hi, -p), __dadd_rn(__dmul_rn(a.hi, b.lo), __dmul_rn(a.lo, b.hi)));
+  return crb_dd_fast(p, e);
+}
+__device__ __forceinline__ crb_dd crb_dd_neg(crb_dd a) { return {-a.hi, -a.lo}; }
+__device__ __forceinline__ crb_dd crb_dd_div(crb_dd a, crb_dd b) {  // three quotient digits
+  const double q1 = __ddiv_rn(a.hi, b.hi);
+  const crb_dd r1 = crb_dd_add(a, crb_dd_neg(crb_dd_mul({q1, 0.0}, b)));
+  const double q2 = __ddiv_rn(r1.hi, b.hi);
+  const crb_dd r2 = crb_dd_add(r1, crb_dd_neg(crb_dd_mul({q2, 0.0}, b)));
+  const double q3 = __ddiv_rn(r2.hi, b.hi);
+  return crb_dd_add(crb_dd_fast(q1, q2), {q3, 0.0});
+}
+// atan(y) for finite y >= 0: atan(x) = atan(j/8) + atan(t), t = (x - j/8) / (1 + x j/8), |t| <= 1/16, with x = y or
+// 1/y (then pi/2 minus the result); the series in t^2 to t^25 (truncation < 2^-100 relative).  Out of line: it is
+// the rare path.
+static __device__ __noinline__ crb_dd crb_atan_dd(double y) {
+  const bool inv = y > 1.0;
+  crb_dd x = {y, 0.0};
+  if (inv) {
+    const double h = __drcp_rn(y);
+    x = crb_dd_fast(h, __ddiv_rn(__fma_rn(-h, y, 1.0), y));
+  }
+  const int j = (int)__dadd_rn(__dmul_rn(x.hi, 8.0), 0.5);
+  const double c = __dmul_rn((double)j, 0.125);
+  // atan(j/8), j = 0..8, as double-double (selects, not an indexed array: no local memory)
+  const double ah = j == 0 ? 0.0 : j == 1 ? 0x1.fd5ba9aac2f6ep-4 : j == 2 ? 0x1.f5b75f92c80ddp-3
+                  : j == 3 ? 0x1.6f61941e4def1p-2 : j == 4 ? 0x1.dac670561bb4fp-2 : j == 5 ? 0x1.1e00babdefeb4p-1
+                  : j == 6 ? 0x1.4978fa3269ee1p-1 : j == 7 ? 0x1.700a7c5784634p-1 : 0x1.921fb54442d18p-1;
+  const double al = j == 0 ? 0.0 : j == 1 ? -0x1.cd37686760c17p-59 : j == 2 ? 0x1.8ab6e3cf7afbdp-57
+                  : j == 3 ? -0x1.c63aae6f6e918p-56 : j == 4 ? 0x1.a2b7f222f65e2p-56 : j == 5 ? -0x1.928df287a668fp-58
+                  : j == 6 ? 0x1.2419a87f2a458p-56 : j == 7 ? -0x1.8c34d25aadef6p-56 : 0x1.1a62633145c07p-55;
+  const crb_dd num = crb_dd_add(x, {-c, 0.0});
+  const crb_dd den = crb_dd_add(crb_dd_mul(x, {c, 0.0}), {1.0, 0.0});
+  const crb_dd t = crb_dd_div(num, den);
+  const crb_dd s = crb_dd_mul(t, t);
+  crb_dd q = {__ddiv_rn(1.0, 25.0), 0.0};
+  for (int i = 11; i >= 0; --i) {  // q = sum_i (-1)^i t^(2i) / (2i + 1), Horner in s = t^2
+    const double dn = (double)(2 * i + 1);
+    const double h = __ddiv_rn(1.0, dn);
+    crb_dd ci = crb_dd_fast(h, __ddiv_rn(__fma_rn(-h, dn, 1.0), dn));
+    if (i & 1) ci = crb_dd_neg(ci);
+    q = crb_dd_add(ci, crb_dd_mul(s, q));
+  }
+  crb_dd r = crb_dd_add({ah, al}, crb_dd_mul(t, q));
+  if (inv) r = crb_dd_add({0x1.921fb54442d18p+0, 0x1.1a62633145c07p-54}, crb_dd_neg(r));
+  return r;
+}
+__device__ __forceinline__ float crb_atan2_1_to_float(double y) {
+  const double d = atan(y);  // NaN for NaN, +-pi/2 for +-inf
+  if (!isfinite(y)) return __double2float_rn(d);
+  const double ad = fabs(d);
+  const long long b = __double_as_longlong(ad);
+  if (__double2float_rn(__longlong_as_double(b > 4 ? b - 4 : 0)) == __double2float_rn(__longlong_as_double(b + 4)))
+    return __double2float_rn(d);
+  const float f = __double2float_rn(crb_atan_dd(fabs(y)).hi);
+  return y < 0.0 ? -f : f;
+}

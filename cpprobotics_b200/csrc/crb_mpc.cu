@@ -28,6 +28,7 @@
 #include "crb_common.cuh"
 
 #include "crb_mpc_core.cuh"
+#include "crb_plant.cuh"
 #include "crb_mpc_tasks.cuh"
 
 // Thread-per-problem kernel (first generation; CRB_MPC_VARIANT=0): solver workspace in global memory,
@@ -842,18 +843,14 @@ extern "C" int crb_mpc_solve_batched_host(crb_ctx* ctx, int64_t n, int T, const 
 }
 
 // ---- update(): src/model_predictive_control.cpp:69-81 ------------------------------------------------
-// MAX_STEER, DT, WB, MAX_SPEED, MIN_SPEED are double macros in the reference, so the float operands
-// promote to double and the result narrows on assignment; cos/sin/tan are the float overloads.
+// The step itself is crb_plant_step (crb_plant.cuh).
 // The constants come from crb_mpc_params (floats).  A parameter that equals the reference's macro rounded to
 // float is taken as the macro's own double value (so the defaults reproduce the reference bit for bit);
 // any other value is promoted from float.  The solver, the plant step and the xref lookup therefore always
 // use the same model.
-struct MpcPlantC {
-  double max_steer, dt, wb, max_speed, min_speed;
-};
 static double mpc_promote(float v, double ref) { return v == (float)ref ? ref : (double)v; }
-static MpcPlantC mpc_plant_constants(const crb_mpc_params* prm) {
-  MpcPlantC c;
+static PlantC mpc_plant_constants(const crb_mpc_params* prm) {
+  PlantC c;
   c.max_steer = mpc_promote(prm->max_steer, 45.0 / 180 * 3.14159265358979323846);
   c.dt = mpc_promote(prm->dt, 0.2);
   c.wb = mpc_promote(prm->wb, 2.5);
@@ -864,27 +861,12 @@ static MpcPlantC mpc_plant_constants(const crb_mpc_params* prm) {
 
 __global__ void __launch_bounds__(256)
 crb_mpc_plant_update_kernel(int64_t n, float* __restrict__ state, const float* __restrict__ u0,
-                            const MpcPlantC k) {
+                            const PlantC k) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const double MAX_STEER = k.max_steer, DT = k.dt, WB = k.wb;
-  const double MAX_SPEED = k.max_speed, MIN_SPEED = k.min_speed;
-  const float a = u0[i];
-  float delta = u0[n + i];
-  if ((double)delta >= MAX_STEER) delta = (float)MAX_STEER;
-  if ((double)delta <= -MAX_STEER) delta = (float)(-MAX_STEER);
-  const float x = state[i], y = state[n + i], yaw = state[2 * n + i], v = state[3 * n + i];
-  float sy, cy;
-  crb_sincosf_libm(yaw, sy, cy);   // std::cos / std::sin of a float: the host libm's bits (crb_common.cuh)
-  const float nx = (float)((double)x + (double)(v * cy) * DT);
-  const float ny = (float)((double)y + (double)(v * sy) * DT);
-  // std::tan of a float: glibc's bits.  |delta| <= max_steer < pi/2 (crb.h limits), inside crb_tanf_libm's
-  // proven range; a NaN delta stays NaN
-  const float nyaw = (float)((double)yaw + (double)v / WB * (double)crb_tanf_libm(delta) * DT);
-  float nv = (float)((double)v + (double)a * DT);
-  if ((double)nv > MAX_SPEED) nv = (float)MAX_SPEED;
-  if ((double)nv < MIN_SPEED) nv = (float)MIN_SPEED;
-  state[i] = nx; state[n + i] = ny; state[2 * n + i] = nyaw; state[3 * n + i] = nv;
+  float x = state[i], y = state[n + i], yaw = state[2 * n + i], v = state[3 * n + i];
+  crb_plant_step(x, y, yaw, v, u0[i], u0[n + i], k);
+  state[i] = x; state[n + i] = y; state[2 * n + i] = yaw; state[3 * n + i] = v;
 }
 
 extern "C" int crb_mpc_plant_update_batched(crb_ctx* ctx, int64_t n, float* state, const float* u0,

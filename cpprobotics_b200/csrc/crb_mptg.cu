@@ -22,25 +22,6 @@
 
 namespace {
 
-constexpr double kPi = 3.14159265358979323846;  // M_PI
-constexpr double kTwoPi = 2.0 * kPi;             // 2*M_PI (an exact doubling)
-
-// fmod(a, 2*M_PI), exactly.  fmod is exact in IEEE arithmetic; for |a| < 4 pi (every wrapped yaw) its result is
-// a itself or a -+ 2 pi, and that subtraction is exact (Sterbenz), so the general routine is only needed beyond.
-__device__ __forceinline__ double mptg_fmod_2pi(double a) {
-  const double aa = fabs(a);
-  if (aa < kTwoPi) return a;
-  if (aa < 2.0 * kTwoPi) return copysign(__dsub_rn(aa, kTwoPi), a);  // fmod's result has a's sign
-  return fmod(a, kTwoPi);
-}
-
-// YAW_P2P(angle) :18 on a float, in double, narrowed back to float by the assignment
-__device__ __forceinline__ float mptg_yaw_p2p(float yaw) {
-  double a = mptg_fmod_2pi(__dadd_rn((double)yaw, kPi));
-  a = mptg_fmod_2pi(__dsub_rn(a, kTwoPi));
-  return __double2float_rn(__dadd_rn(a, kPi));
-}
-
 // Eigen 3.3 compute_inverse<Matrix3f, Matrix3f, 3>: cofactor_3x3<i,j> = m(i1,j1) m(i2,j2) - m(i1,j2) m(i2,j1)
 // with i1 = (i+1)%3, i2 = (i+2)%3 (likewise j); det = (c00 m00 + c10 m10) + c20 m20; out(i,j) =
 // cofactor_3x3<j,i> * (1 / det).  m[r][c].

@@ -19,8 +19,6 @@
 
 namespace {
 
-constexpr double kPi = 3.14159265358979323846;  // M_PI
-
 __device__ __forceinline__ float slp_nan() { return __int_as_float(0x7fc00000); }
 
 // a finite argument outside crb_sincosf_libm's proven range (inf and NaN give NaN, as glibc does)

@@ -20,6 +20,9 @@ Method names follow the reference functions they replace:
   Engine.grid_obstacle_map   <- calc_obstacle_map()                              src/a_star.cpp:48-78
   Engine.grid_plan           <- a_star_planning() / dijkstra_star_planning()     src/a_star.cpp:110-244, src/dijkstra.cpp
   Engine.rrt_plan            <- RRT::planning()                                  include/rrt.h:75-159
+  Engine.lqr_steering_control <- lqr_steering_control() (+ calc_nearest_index)   src/lqr_steer_control.cpp:98-133,
+                                                                                 src/lqr_speed_steer_control.cpp:108-151
+  Engine.lqr_update          <- update()                 src/lqr_steer_control.cpp:136-146 (same text in both programs)
 
 All arrays are SoA field-major float32 (`[fields, n]`, C-contiguous); see include/crb.h.  Methods
 without a suffix take CUDA tensors (torch is only the device allocator / stream owner); `*_host`
@@ -35,7 +38,8 @@ from typing import Optional
 import numpy as np
 
 from . import _lib
-from ._lib import DwaParams, EkfParams, GridBox, MpcParams, MptgParams, PfParams, RrtParams, check, load_library
+from ._lib import (DwaParams, EkfParams, GridBox, LqrTrackParams, MpcParams, MptgParams, PfParams, RrtParams, check,
+                   load_library)
 
 try:  # torch is the device-memory / stream / distributed plumbing, never the compute path
     import torch
@@ -85,6 +89,14 @@ def rrt_default_params() -> RrtParams:
     """RRT's constructor defaults (expand_dis 1.0, goal_sample_rate 5, max_iter 500) and the demo's rand_area {-2, 15}."""
     p = RrtParams()
     load_library().crb_rrt_default_params(C.byref(p))
+    return p
+
+
+def lqr_track_default_params(nx: int) -> LqrTrackParams:
+    """The LQR programs' constants for nx = 4 (lqr_steer_control) or 5 (lqr_speed_steer_control): dt 0.1, wheelbase
+    0.5, max_steer 45/180*pi (doubles), Q = I, R = I or 1, maxiter 150, eps 0.01f."""
+    p = LqrTrackParams()
+    load_library().crb_lqr_track_default_params(C.byref(p), int(nx))
     return p
 
 
@@ -704,6 +716,52 @@ class Engine:
             "crb_rrt_plan_batched")
         return dict(path=path, path_len=path_len, tree=tree, parent=parent, n_nodes=n_nodes, n_iter=n_iter,
                     status=status)
+
+    # ---- LQR path tracking ------------------------------------------------------------------------------------------
+    def lqr_steering_control(self, nx: int, state, course, ind, pe, pth_e, params: Optional[LqrTrackParams] = None,
+                             u=None, K=None, iters=None, status=None):
+        """lqr_steering_control() for n vehicles on one course.  nx 4 (lqr_steer_control) or 5
+        (lqr_speed_steer_control); state [4, n] (x, y, yaw, v); course (cx, cy, cyaw, ck) for nx 4 or (cx, cy, cyaw,
+        ck, sp) for nx 5, 1-D float32 each; ind [n] int32 (in/out for nx 4, out for nx 5), pe, pth_e [n] in/out.
+        Returns dict(u [nu, n] (delta | ai, delta), K [nu*nx, n] or None, iters, status (CRB_LQR_TRACK_*)); u, iters
+        and status are allocated when not given, K only when passed.  CUDA tensors; only enqueues."""
+        n = int(state.shape[-1])
+        nu = 1 if nx == 4 else 2
+        _shape(state, 4, n, "state")
+        if len(course) != (4 if nx == 4 else 5):
+            raise ValueError(f"course: expected {4 if nx == 4 else 5} arrays for nx = {nx}, got {len(course)}")
+        nc = int(course[0].shape[0])
+        for a, name in zip(course, ("cx", "cy", "cyaw", "ck", "sp")):
+            _shape(a, 1, nc, name)
+        for a, name in ((ind, "ind"), (pe, "pe"), (pth_e, "pth_e")):
+            _shape(a, 1, n, name)
+        dev = state.device
+        if u is None:
+            u = torch.empty((nu, n), dtype=torch.float32, device=dev)
+        iters = iters if iters is not None else torch.empty(n, dtype=torch.int32, device=dev)
+        status = status if status is not None else torch.empty(n, dtype=torch.int32, device=dev)
+        _shape(u, nu, n, "u")
+        if K is not None:
+            _shape(K, nu * nx, n, "K")
+        prm = params if params is not None else lqr_track_default_params(nx)
+        f = lambda a, name: _ptr(a, np.float32, device=True, name=name)  # noqa: E731
+        check(self.lib.crb_lqr_steering_control_batched(
+            self.ctx, n, int(nx), f(state, "state"), f(course[0], "cx"), f(course[1], "cy"), f(course[2], "cyaw"),
+            f(course[3], "ck"), f(course[4], "sp") if nx == 5 else None, nc, C.byref(prm),
+            _ptr(ind, np.int32, device=True, name="ind"), f(pe, "pe"), f(pth_e, "pth_e"), f(u, "u"), f(K, "K"),
+            _ptr(iters, np.int32, device=True, name="iters"), _ptr(status, np.int32, device=True, name="status")),
+            "crb_lqr_steering_control_batched")
+        return dict(u=u, K=K, iters=iters, status=status)
+
+    def lqr_update(self, state, a, delta, params: Optional[LqrTrackParams] = None):
+        """update() of the LQR programs for n vehicles, in place: state [4, n], a [n], delta [n].  CUDA tensors."""
+        n = int(state.shape[-1])
+        _shape(state, 4, n, "state"); _shape(a, 1, n, "a"); _shape(delta, 1, n, "delta")
+        prm = params if params is not None else lqr_track_default_params(4)
+        check(self.lib.crb_lqr_update_batched(
+            self.ctx, n, _ptr(state, np.float32, device=True, name="state"), _ptr(a, np.float32, device=True, name="a"),
+            _ptr(delta, np.float32, device=True, name="delta"), C.byref(prm)), "crb_lqr_update_batched")
+        return state
 
     # ---- multi-GPU: the communicator lives in libcrb (crb_comm.cu), not in torch --------------------
     @staticmethod

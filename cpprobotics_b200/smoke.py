@@ -196,5 +196,24 @@ def run() -> None:
     assert ok, "RRT GPU result is not bit-identical to the checker"
     print(f"smoke RRT   65 queries on the demo map: bit-identical to the checker; "
           f"{int((rr['status'] == 0).sum().item())} found")
+    # LQR path tracking: 4- and 5-state control, then update, for 257 vehicles on the demo-shaped course, every output as
+    # the checker
+    from oracle import lqrt as OL  # checker only
+    lcourse = synth.lqr_course("demo")
+    lst, lind, lpe, lpth = synth.lqr_track_inputs(257, lcourse, seed=0x5A0)
+    dcourse = [torch.from_numpy(a).to(dev) for a in lcourse]
+    for nx in (4, 5):
+        dst = torch.from_numpy(lst).to(dev)
+        dind, dpe, dpth = (torch.from_numpy(a.copy()).to(dev) for a in (lind, lpe, lpth))
+        lr = eng.lqr_steering_control(nx, dst, dcourse[: 4 if nx == 4 else 5], dind, dpe, dpth)
+        nu = 1 if nx == 4 else 2
+        eng.lqr_update(dst, lr["u"][0].contiguous() if nx == 5 else torch.zeros_like(dpe), lr["u"][nu - 1].contiguous())
+        torch.cuda.synchronize()
+        lo = OL.control(nx, lst, lcourse, lind, lpe, lpth)
+        lnew = OL.update(lst, lo["u"][0] if nx == 5 else np.zeros(257, np.float32), lo["u"][nu - 1])
+        ok = all(same_nan(g, w) for g, w in ((lr["u"], lo["u"]), (dind, lo["ind"]), (dpe, lo["pe"]), (dpth, lo["pth_e"]),
+                                             (lr["iters"], lo["iters"]), (lr["status"], lo["status"]), (dst, lnew)))
+        assert ok, f"LQR tracking (nx {nx}) GPU result is not bit-identical to the checker"
+    print("smoke LQRT  257 vehicles, 4- and 5-state control and update on the demo course: bit-identical to the checker")
     print(f"smoke ok: {eng.launches} kernel launches through libcrb.so")
     eng.close()

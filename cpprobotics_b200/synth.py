@@ -463,3 +463,135 @@ def rrt_inputs(n: int, ob, lo: float, hi: float, seed: int = 0xC0FFEE, i0: int =
     se = np.ascontiguousarray(np.stack([sx, sy, gx, gy]).astype(np.float32))
     seeds = (splitmix64(idx ^ np.uint64(seed)) >> np.uint64(32)).astype(np.uint32)
     return se, seeds
+
+
+# ---- LQR path tracking (src/lqr_steer_control.cpp, src/lqr_speed_steer_control.cpp) ------------------------------
+# The demos' waypoints (main() of each program); the course is input data, so a float64 natural cubic spline here
+# stands in for the reference's Spline2D (its bits are not reproduced, only its shape).
+LQR_DEMO_WAYPOINTS = {
+    "demo": ([0.0, 6.0, 12.5, 10.0, 7.5, 3.0, -1.0], [0.0, -3.0, -5.0, 6.5, 3.0, 5.0, -2.0]),          # lqr_steer
+    "demo_speed": ([0.0, 6.0, 12.5, 10.0, 17.5, 20.0, 25.0], [0.0, -3.0, -5.0, 6.5, 3.0, 0.0, 0.0]),  # speed+steer
+}
+LQR_KINDS = ("straight", "circle", "sine", "scurve", "demo", "demo_speed")
+LQR_TARGET_SPEED = 10.0 / 3.6
+
+
+def _natural_spline(t, v):
+    """Coefficients of the natural cubic spline through (t, v): value, first and second derivative callables."""
+    t, v = np.asarray(t, np.float64), np.asarray(v, np.float64)
+    h = np.diff(t)
+    m = len(t)
+    A = np.zeros((m, m))
+    r = np.zeros(m)
+    A[0, 0] = A[-1, -1] = 1.0
+    for i in range(1, m - 1):
+        A[i, i - 1], A[i, i], A[i, i + 1] = h[i - 1], 2.0 * (h[i - 1] + h[i]), h[i]
+        r[i] = 3.0 * ((v[i + 1] - v[i]) / h[i] - (v[i] - v[i - 1]) / h[i - 1])
+    c = np.linalg.solve(A, r)
+    b = (v[1:] - v[:-1]) / h - h * (2.0 * c[:-1] + c[1:]) / 3.0
+    d = (c[1:] - c[:-1]) / (3.0 * h)
+
+    def seg(s):
+        i = np.clip(np.searchsorted(t, s, side="right") - 1, 0, m - 2)
+        return i, s - t[i]
+
+    def f(s, der=0):
+        i, x = seg(s)
+        if der == 0:
+            return v[i] + b[i] * x + c[i] * x ** 2 + d[i] * x ** 3
+        if der == 1:
+            return b[i] + 2.0 * c[i] * x + 3.0 * d[i] * x ** 2
+        return 2.0 * c[i] + 6.0 * d[i] * x
+    return f
+
+
+def lqr_speed_profile(cyaw, target_speed: float = LQR_TARGET_SPEED) -> np.ndarray:
+    """calc_speed_profile of src/lqr_steer_control.cpp:35-53 (the speed+steer program's version writes past the end
+    of its vector): target_speed, its sign flipped after each 45-90 degree yaw step, 0 at those steps and at the end."""
+    sp = np.full(len(cyaw), np.float32(target_speed), np.float32)
+    direction = 1.0
+    for i in range(len(cyaw) - 1):
+        dyaw = abs(float(np.float32(cyaw[i + 1]) - np.float32(cyaw[i])))
+        switch = (np.pi / 4.0 < dyaw) and (dyaw < np.pi / 2.0)
+        if switch:
+            direction = -direction
+        sp[i] = target_speed * (-1 if direction != 1.0 else 1)
+        if switch:
+            sp[i] = 0.0
+    sp[-1] = 0.0
+    return sp
+
+
+def lqr_course(kind: str, ds: float = 0.1):
+    """A float32 course (cx, cy, cyaw, ck, sp) sampled every ds metres: "straight" (40 m along a slanted line),
+    "circle" (radius 8, one lap), "sine" (amplitude 3, wavelength 20, 60 m), "scurve" (two opposite 10 m arcs), or the
+    demos' waypoints through a float64 natural cubic spline over chord length ("demo" of lqr_steer_control, "demo_speed"
+    of lqr_speed_steer_control).  sp is lqr_speed_profile of the yaw at the demos' 10 km/h."""
+    if kind == "straight":
+        s = np.arange(0.0, 40.0, ds)
+        th = 0.3
+        x, y = s * np.cos(th), s * np.sin(th)
+        yaw, k = np.full_like(s, th), np.zeros_like(s)
+    elif kind == "circle":
+        r = 8.0
+        s = np.arange(0.0, 2 * np.pi * r, ds)
+        a = s / r
+        x, y = r * np.sin(a), r - r * np.cos(a)
+        yaw, k = a, np.full_like(s, 1.0 / r)
+    elif kind == "sine":
+        xs = np.arange(0.0, 60.0, ds)
+        w = 2 * np.pi / 20.0
+        x, y = xs, 3.0 * np.sin(w * xs)
+        dy, ddy = 3.0 * w * np.cos(w * xs), -3.0 * w * w * np.sin(w * xs)
+        yaw, k = np.arctan2(dy, 1.0), ddy / (1.0 + dy * dy) ** 1.5
+    elif kind == "scurve":
+        r = 10.0
+        s = np.arange(0.0, np.pi * r, ds)
+        a = s / r
+        half = a < np.pi / 2
+        a2 = a - np.pi / 2
+        x = np.where(half, r * np.sin(a), r + r * np.sin(np.pi / 2 - a2))
+        y = np.where(half, r - r * np.cos(a), r + r - r * np.cos(np.pi / 2 - a2))
+        yaw = np.where(half, a, np.pi / 2 - a2)
+        k = np.where(half, 1.0 / r, -1.0 / r)
+    elif kind in LQR_DEMO_WAYPOINTS:
+        wx, wy = (np.asarray(w, np.float64) for w in LQR_DEMO_WAYPOINTS[kind])
+        t = np.concatenate([[0.0], np.cumsum(np.hypot(np.diff(wx), np.diff(wy)))])
+        fx, fy = _natural_spline(t, wx), _natural_spline(t, wy)
+        s = np.arange(0.0, t[-1], ds)
+        x, y = fx(s), fy(s)
+        dx, dy, ddx, ddy = fx(s, 1), fy(s, 1), fx(s, 2), fy(s, 2)
+        yaw = np.arctan2(dy, dx)
+        k = (ddy * dx - ddx * dy) / (dx * dx + dy * dy) ** 1.5
+    else:
+        raise ValueError(f"unknown course kind {kind!r}; one of {LQR_KINDS}")
+    cx, cy, cyaw, ck = (np.ascontiguousarray(a, np.float32) for a in (x, y, yaw, k))
+    return cx, cy, cyaw, ck, lqr_speed_profile(cyaw)
+
+
+def lqr_track_inputs(n: int, course, seed: int = 0xC0FFEE):
+    """n vehicles around a course: a random course point, up to 2 m off it (a tenth of them up to 30 m), yaw the
+    course heading plus up to +-1 rad (a twentieth anywhere in +-200 rad), speed from {0, the demo's 10 km/h, 1, 0.3,
+    -1.5} or uniform in [-3, 6]; pe, pth_e small and ind a random course index.  Returns (state [4, n] float32,
+    ind [n] int32, pe [n] float32, pth_e [n] float32)."""
+    cx, cy, cyaw = course[0], course[1], course[2]
+    rng = np.random.default_rng(seed)
+    nc = len(cx)
+    j = rng.integers(0, nc, n)
+    off = rng.uniform(-2.0, 2.0, (2, n))
+    far = rng.random(n) < 0.1
+    off[:, far] *= 15.0
+    x = cx[j] + off[0]
+    y = cy[j] + off[1]
+    yaw = cyaw[j] + rng.uniform(-1.0, 1.0, n)
+    wild = rng.random(n) < 0.05
+    yaw[wild] = rng.uniform(-200.0, 200.0, int(wild.sum()))
+    v = rng.uniform(-3.0, 6.0, n)
+    pick = rng.integers(0, 6, n)
+    table = np.array([0.0, LQR_TARGET_SPEED, 1.0, 0.3, -1.5])
+    v = np.where(pick < 5, table[np.minimum(pick, 4)], v)
+    state = np.ascontiguousarray(np.stack([x, y, yaw, v]).astype(np.float32))
+    ind = rng.integers(0, nc, n).astype(np.int32)
+    pe = rng.uniform(-1.0, 1.0, n).astype(np.float32)
+    pth_e = rng.uniform(-0.5, 0.5, n).astype(np.float32)
+    return state, ind, pe, pth_e

@@ -35,6 +35,11 @@
  *                                          :31-45), dijkstra_star_planning()  src/dijkstra.cpp
  *   crb_rrt_plan_batched                <- RRT::planning()       include/rrt.h:75-159 (GetNearestNode :161-174,
  *                                          CollisionCheck :176-181)
+ *   crb_lqr_steering_control_batched    <- lqr_steering_control() src/lqr_steer_control.cpp:98-133 (4 states),
+ *                                          src/lqr_speed_steer_control.cpp:108-151 (5 states), with
+ *                                          calc_nearest_index() :55-73 / :65-83 and solve_DARE() + dlqr() inside
+ *   crb_lqr_update_batched              <- update()              src/lqr_steer_control.cpp:136-146,
+ *                                          src/lqr_speed_steer_control.cpp:154-164
  *   crb_stats_*                         <- (no reference counterpart) per-GPU summary statistics, the
  *                                          only thing that ever crosses NVLink (one all-gather).
  *
@@ -636,6 +641,61 @@ int crb_rrt_plan_batched(crb_ctx* ctx, const crb_rrt_params* prm, const float* o
                          const float* se, const uint32_t* seed, int32_t max_pts, float* path, int32_t* path_len,
                          int32_t max_nodes, float* tree, int32_t* parent, int32_t* n_nodes, int32_t* n_iter,
                          int32_t* status);
+
+/* ---- LQR path tracking (src/lqr_steer_control.cpp, src/lqr_speed_steer_control.cpp) ------------------------------- */
+/* The per-tick functions of the two LQR programs for a fleet on one course; the caller keeps the loop
+ * (closed_loop_prediction is not a function with defined behaviour in the reference: its time never advances).
+ * Bit-exact with the reference built for x86-64 with GCC 13 and glibc 2.39: float arithmetic without contraction,
+ * the double macros DT, L and MAX_STEER promoting what they touch, YAW_P2P in double, glibc's atan2f in
+ * calc_nearest_index, glibc's double atan2 narrowed to float for the feed-forward, glibc's sinf / cosf / tanf in
+ * update (DESIGN.md §3.1-3.4). */
+typedef struct crb_lqr_track_params {
+  double dt;        /* DT: the error-rate divisor, A(0,1) = A(2,3) = (float)dt, B(4,1) (5 states); update's step */
+  double wheelbase; /* L: B(3) = v / L, the feed-forward atan2(L * k, 1), update's yaw rate */
+  double max_steer; /* MAX_STEER: update clamps delta to [-max_steer, max_steer] */
+  float Q[25];      /* state cost, column-major 5x5; the top-left nx x nx block is used: Q(r,c) = Q[r + 5c] */
+  float R[4];       /* input cost, column-major 2x2; the top-left nu x nu block is used (R[0] for 4 states) */
+  int32_t maxiter;  /* solve_DARE's iteration cap (the reference's 150) */
+  float eps;        /* solve_DARE's tolerance on max|Xn - X| (the reference's 0.01f) */
+} crb_lqr_track_params;
+/* The reference's constants: dt 0.1, wheelbase 0.5, max_steer 45.0/180*M_PI, Q = I, R = I (nx 5) or 1 (nx 4),
+ * maxiter 150, eps 0.01f.  nx is 4 or 5 (any other value is treated as 5). */
+void crb_lqr_track_default_params(crb_lqr_track_params* p, int nx);
+
+/* Per-vehicle status of crb_lqr_steering_control_batched. */
+#define CRB_LQR_TRACK_OK 0
+#define CRB_LQR_TRACK_DARE_MAXITER 1 /* solve_DARE stopped at maxiter without max|Xn - X| < eps (always at v = 0);
+                                        a flag only: the outputs are the reference's, computed from the last X */
+#define CRB_LQR_TRACK_BAD_INDEX 2    /* no course point won the scan (every squared distance NaN or >= FLT_MAX) and
+                                        the incoming ind is outside [0, ncourse), where the reference reads out of
+                                        bounds: u and K are NaN, iters 0, ind / pe / pth_e are left as they are */
+
+/* lqr_steering_control for n vehicles against one course shared by the batch.
+ *   nx 4: lqr_steer_control.cpp (nu = 1); nx 5: lqr_speed_steer_control.cpp (nu = 2)
+ *   state [4][n] (x, y, yaw, v)
+ *   cx, cy, cyaw, ck [ncourse]; sp [ncourse] for nx 5 (the target speed), NULL for nx 4
+ *   ind [n] int32: nx 4 in/out, the nearest index kept across calls (the reference's int& ind: it is only assigned
+ *        when a course point wins the scan); nx 5 out, the nearest index of this call (the reference's local, from 0)
+ *   pe, pth_e [n] in/out: the previous lateral and heading errors, replaced by this call's
+ *   u [nu][n]: nx 4 delta; nx 5 (ai, delta), the reference's {ai, delta}
+ *   optional outputs, NULL = not written: K [nu*nx][n] the gain (column-major nu x nx), iters [n] int32 DARE
+ *   iterations, status [n] int32 CRB_LQR_TRACK_*
+ * calc_nearest_index scans the WHOLE course with a strict '<' against FLT_MAX, so the first minimum wins, and returns
+ * the signed squared distance (negated when YAW_P2P(cyaw[ind] - atan2f(dyl, dxl)) < 0), as the reference does.
+ * Non-finite states follow the reference's arithmetic (NaN payloads aside).  One thread per vehicle; each block
+ * streams the course through shared memory in tiles.  Returns CRB_ERR_INVALID_ARG before any device work unless
+ * nx is 4 or 5, ncourse >= 1, sp is given exactly when nx is 5, and prm is valid (crb_lqr_update_batched's limits,
+ * finite Q and R, finite eps, maxiter >= 0).  DEVICE pointers; only enqueues (graph-capturable). */
+int crb_lqr_steering_control_batched(crb_ctx* ctx, int64_t n, int nx, const float* state, const float* cx,
+                                     const float* cy, const float* cyaw, const float* ck, const float* sp,
+                                     int32_t ncourse, const crb_lqr_track_params* prm, int32_t* ind, float* pe,
+                                     float* pth_e, float* u, float* K, int32_t* iters, int32_t* status);
+/* update(State&, a, delta) of the LQR programs for n vehicles: state [4][n] in/out, a [n], delta [n].  The kinematic
+ * bicycle of crb_mpc_plant_update_batched with prm's dt, wheelbase and max_steer used as the doubles they are, and
+ * no speed clamp.  Requires finite dt, wheelbase and max_steer with |max_steer| < 120 (the range in which tanf is
+ * restated); otherwise CRB_ERR_INVALID_ARG.  DEVICE pointers. */
+int crb_lqr_update_batched(crb_ctx* ctx, int64_t n, float* state, const float* a, const float* delta,
+                           const crb_lqr_track_params* prm);
 
 /* ---- multi-GPU: communicator owned by the context (NCCL, opened at run time) ---------------------- */
 /* The batch shards over GPUs by contiguous agent ranges (one crb_ctx per device, one host thread or process

@@ -16,6 +16,9 @@
 //   a_star_planning(sx, sy, gx, gy, ox, oy, reso, rr), dijkstra_star_planning(...)
 //                                                            src/a_star.cpp:110-244, src/dijkstra.cpp
 //   Node, RRT(start, end, ob_list, rand_area, expand_dis, ...).planning()   include/rrt.h:21-159
+//   lqr_steer_control::{lqr_steering_control, update}        src/lqr_steer_control.cpp:98-146
+//   lqr_speed_steer_control::{lqr_steering_control, update}  src/lqr_speed_steer_control.cpp:108-164
+//                                                            (namespaces: ::update above is the MPC program's)
 //
 // Eigen is not a dependency: crb::Mat<R,C> is a POD with the memory layout of
 // Eigen::Matrix<float,R,C> (column-major, contiguous, no padding), enough of its interface for the
@@ -870,6 +873,149 @@ class RRT {
   uint32_t next_seed;
   std::vector<std::unique_ptr<Node> > owned;
 };
+}  // namespace cpprobotics
+
+// ---------------------------------------------------------------------------------------------------
+// LQR path tracking: src/lqr_steer_control.cpp and src/lqr_speed_steer_control.cpp.  Each program's functions live
+// in a namespace named after it, because both programs and the MPC program (above) define update() with one
+// signature; a main() written against one program says `using namespace cpprobotics::lqr_steer_control;` and calls
+// lqr_steering_control(...) and lqr_steer_control::update(...).  calc_nearest_index runs inside lqr_steering_control.
+// The single-vehicle calls copy the course to the device on every call, as the reference copies its vectors by value;
+// the batched overloads take a fleet at once.
+// ---------------------------------------------------------------------------------------------------
+namespace cpprobotics {
+namespace detail {
+// one control call for n vehicles on host arrays (AoS State), through the session's device arena
+inline void lqr_control(int nx, const std::vector<State>& st, const Vec_f& cx, const Vec_f& cy, const Vec_f& cyaw,
+                        const Vec_f& ck, const Vec_f* sp, int32_t* ind, float* pe, float* pth_e, float* u) {
+  const int64_t n = (int64_t)st.size();
+  const size_t nc = cx.size();
+  if (nc == 0 || cy.size() != nc || cyaw.size() != nc || ck.size() != nc || (sp && sp->size() != nc))
+    throw std::runtime_error("lqr_steering_control: the course vectors must be non-empty and of one length");
+  if (n == 0) return;
+  const int nu = nx == 4 ? 1 : 2;
+  const size_t nn = (size_t)n;
+  // layout: course (4 or 5 x nc) | state 4n | ind n | pe n | pth_e n | u nu*n
+  const size_t need = (sp ? 5 : 4) * nc + (4 + 3 + nu) * nn;
+  crb_ctx* ctx = crb::Session::get();
+  float* base = crb::Session::scratch(need);
+  float* dcx = base;
+  float* dcy = dcx + nc;
+  float* dcyaw = dcy + nc;
+  float* dck = dcyaw + nc;
+  float* dsp = sp ? dck + nc : nullptr;
+  float* dst = dck + nc + (sp ? nc : 0);
+  int32_t* dind = (int32_t*)(dst + 4 * nn);
+  float* dpe = (float*)(dind + nn);
+  float* dpth = dpe + nn;
+  float* du = dpth + nn;
+  std::vector<float> soa(4 * nn);
+  for (size_t i = 0; i < nn; ++i) {
+    soa[i] = st[i].x; soa[nn + i] = st[i].y; soa[2 * nn + i] = st[i].yaw; soa[3 * nn + i] = st[i].v;
+  }
+  crb::check(crb_memcpy_h2d(ctx, dcx, cx.data(), nc * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dcy, cy.data(), nc * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dcyaw, cyaw.data(), nc * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dck, ck.data(), nc * 4), "crb_memcpy_h2d");
+  if (sp) crb::check(crb_memcpy_h2d(ctx, dsp, sp->data(), nc * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dst, soa.data(), soa.size() * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dind, ind, nn * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dpe, pe, nn * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dpth, pth_e, nn * 4), "crb_memcpy_h2d");
+  crb_lqr_track_params prm;
+  crb_lqr_track_default_params(&prm, nx);
+  crb::check(crb_lqr_steering_control_batched(ctx, n, nx, dst, dcx, dcy, dcyaw, dck, dsp, (int32_t)nc, &prm, dind, dpe,
+                                              dpth, du, nullptr, nullptr, nullptr),
+             "crb_lqr_steering_control_batched");
+  crb::check(crb_memcpy_d2h(ctx, ind, dind, nn * 4), "crb_memcpy_d2h");
+  crb::check(crb_memcpy_d2h(ctx, pe, dpe, nn * 4), "crb_memcpy_d2h");
+  crb::check(crb_memcpy_d2h(ctx, pth_e, dpth, nn * 4), "crb_memcpy_d2h");
+  crb::check(crb_memcpy_d2h(ctx, u, du, nu * nn * 4), "crb_memcpy_d2h");
+}
+// update() of the LQR programs for n vehicles, in place
+inline void lqr_update(std::vector<State>& st, const Vec_f& a, const Vec_f& delta) {
+  const size_t nn = st.size();
+  if (a.size() != nn || delta.size() != nn) throw std::runtime_error("update: a and delta need one value per state");
+  if (nn == 0) return;
+  crb_ctx* ctx = crb::Session::get();
+  float* dst = crb::Session::scratch(6 * nn);
+  float* da = dst + 4 * nn;
+  float* dd = da + nn;
+  std::vector<float> soa(4 * nn);
+  for (size_t i = 0; i < nn; ++i) {
+    soa[i] = st[i].x; soa[nn + i] = st[i].y; soa[2 * nn + i] = st[i].yaw; soa[3 * nn + i] = st[i].v;
+  }
+  crb::check(crb_memcpy_h2d(ctx, dst, soa.data(), soa.size() * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, da, a.data(), nn * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dd, delta.data(), nn * 4), "crb_memcpy_h2d");
+  crb_lqr_track_params prm;
+  crb_lqr_track_default_params(&prm, 4);  // update is the same text in both programs
+  crb::check(crb_lqr_update_batched(ctx, (int64_t)nn, dst, da, dd, &prm), "crb_lqr_update_batched");
+  crb::check(crb_memcpy_d2h(ctx, soa.data(), dst, soa.size() * 4), "crb_memcpy_d2h");
+  for (size_t i = 0; i < nn; ++i) {
+    st[i].x = soa[i]; st[i].y = soa[nn + i]; st[i].yaw = soa[2 * nn + i]; st[i].v = soa[3 * nn + i];
+  }
+}
+}  // namespace detail
+
+namespace lqr_steer_control {
+// src/lqr_steer_control.cpp:98-133: ind, pe, pth_e carry over between calls; returns delta
+inline float lqr_steering_control(State state, Vec_f cx, Vec_f cy, Vec_f cyaw, Vec_f ck, int& ind, float& pe,
+                                  float& pth_e) {
+  int32_t i = ind;
+  float delta = 0.0f;
+  detail::lqr_control(4, std::vector<State>(1, state), cx, cy, cyaw, ck, nullptr, &i, &pe, &pth_e, &delta);
+  ind = i;
+  return delta;
+}
+// a fleet on one course: ind, pe, pth_e one per state (in/out); returns delta per state
+inline Vec_f lqr_steering_control(const std::vector<State>& states, const Vec_f& cx, const Vec_f& cy,
+                                  const Vec_f& cyaw, const Vec_f& ck, std::vector<int>& ind, Vec_f& pe, Vec_f& pth_e) {
+  const size_t n = states.size();
+  if (ind.size() != n || pe.size() != n || pth_e.size() != n)
+    throw std::runtime_error("lqr_steering_control: ind, pe and pth_e need one value per state");
+  std::vector<int32_t> i32(ind.begin(), ind.end());
+  Vec_f delta(n);
+  detail::lqr_control(4, states, cx, cy, cyaw, ck, nullptr, i32.data(), pe.data(), pth_e.data(), delta.data());
+  for (size_t i = 0; i < n; ++i) ind[i] = i32[i];
+  return delta;
+}
+// :136-146
+inline void update(State& state, float a, float delta) {
+  std::vector<State> s(1, state);
+  detail::lqr_update(s, Vec_f(1, a), Vec_f(1, delta));
+  state = s[0];
+}
+inline void update(std::vector<State>& states, const Vec_f& a, const Vec_f& delta) { detail::lqr_update(states, a, delta); }
+}  // namespace lqr_steer_control
+
+namespace lqr_speed_steer_control {
+// src/lqr_speed_steer_control.cpp:108-151: returns {ai, delta}; pe, pth_e carry over between calls
+inline Vec_f lqr_steering_control(State state, Vec_f cx, Vec_f cy, Vec_f cyaw, Vec_f ck, Vec_f sp, float& pe,
+                                  float& pth_e) {
+  int32_t ind = 0;
+  float u[2];
+  detail::lqr_control(5, std::vector<State>(1, state), cx, cy, cyaw, ck, &sp, &ind, &pe, &pth_e, u);
+  return Vec_f{u[0], u[1]};
+}
+// a fleet on one course: pe, pth_e one per state (in/out); returns {ai, delta} per state
+inline std::vector<Vec_f> lqr_steering_control(const std::vector<State>& states, const Vec_f& cx, const Vec_f& cy,
+                                               const Vec_f& cyaw, const Vec_f& ck, const Vec_f& sp, Vec_f& pe,
+                                               Vec_f& pth_e) {
+  const size_t n = states.size();
+  if (pe.size() != n || pth_e.size() != n)
+    throw std::runtime_error("lqr_steering_control: pe and pth_e need one value per state");
+  std::vector<int32_t> ind(n, 0);
+  Vec_f u(2 * n);
+  detail::lqr_control(5, states, cx, cy, cyaw, ck, &sp, ind.data(), pe.data(), pth_e.data(), u.data());
+  std::vector<Vec_f> out(n);
+  for (size_t i = 0; i < n; ++i) out[i] = Vec_f{u[i], u[n + i]};
+  return out;
+}
+// :154-164
+inline void update(State& state, float a, float delta) { lqr_steer_control::update(state, a, delta); }
+inline void update(std::vector<State>& states, const Vec_f& a, const Vec_f& delta) { detail::lqr_update(states, a, delta); }
+}  // namespace lqr_speed_steer_control
 }  // namespace cpprobotics
 
 #endif  // CRB_REFERENCE_API_HPP_
