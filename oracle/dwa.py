@@ -1,5 +1,5 @@
 """ctypes wrapper of oracle/lib/liboracle_dwa.so — the CPU restatement of src/dynamic_window_approach.cpp
-(dwa_control, motion, glibc's acosf).  Built by `make -C oracle -f dwa.mk` (python __graft_entry__.py).
+(dwa_control, motion, glibc's acosf).  Built by `make -C oracle` (python __graft_entry__.py).
 
 TEST INFRASTRUCTURE ONLY, like oracle.py: tests/, __graft_entry__.smoke() and scripts may import it, the product
 package (cpprobotics_b200/) never does.
@@ -11,30 +11,26 @@ import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "liboracle_dwa.so")
+from ._load import LIB_DIR, checker
+
+LIB_PATH = os.path.join(LIB_DIR, "liboracle_dwa.so")
 
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 i32p = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
-_lib = None
+
+
+PROTOTYPES = {
+    "crb_oracle_num_threads": (C.c_int, []),
+    "crb_oracle_libm_acosf": (C.c_float, [C.c_float]),
+    "crb_oracle_libm_acosf_census": (C.c_int64, [C.c_uint32, C.c_uint32]),
+    "crb_oracle_dwa_motion": (None, [C.c_int64, f32p, f32p, C.c_float, C.c_int]),
+    "crb_oracle_dwa_control": (None, [C.c_int64, f32p, f32p, f32p, C.c_void_p, C.c_int, C.c_void_p, f32p, i32p,
+                                      C.c_void_p, C.c_int]),
+}
 
 
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            raise RuntimeError(f"{LIB_PATH} missing: run `make -C oracle -f dwa.mk` (or python __graft_entry__.py)")
-        L = C.CDLL(LIB_PATH)
-        L.crb_oracle_num_threads.restype = C.c_int
-        L.crb_oracle_libm_acosf.restype = C.c_float
-        L.crb_oracle_libm_acosf.argtypes = [C.c_float]
-        L.crb_oracle_libm_acosf_census.restype = C.c_int64
-        L.crb_oracle_libm_acosf_census.argtypes = [C.c_uint32, C.c_uint32]
-        L.crb_oracle_dwa_motion.argtypes = [C.c_int64, f32p, f32p, C.c_float, C.c_int]
-        L.crb_oracle_dwa_control.argtypes = [C.c_int64, f32p, f32p, f32p, C.c_void_p, C.c_int, C.c_void_p,
-                                             f32p, i32p, C.c_void_p, C.c_int]
-        _lib = L
-    return _lib
+    return checker(LIB_PATH, PROTOTYPES)
 
 
 def num_threads() -> int:

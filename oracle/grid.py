@@ -1,6 +1,6 @@
 """ctypes wrapper of oracle/lib/liboracle_grid.so — the CPU restatement of src/a_star.cpp and src/dijkstra.cpp: the
 obstacle cells and box, calc_obstacle_map, the two searches with calc_final_path, the expansion trace, and the
-restated libstdc++ heap on its own.  Built by `make -C oracle -f grid.mk` (python __graft_entry__.py).
+restated libstdc++ heap on its own.  Built by `make -C oracle` (python __graft_entry__.py).
 
 TEST INFRASTRUCTURE ONLY, like oracle.py: tests/, __graft_entry__.smoke() and scripts may import it, the product
 package (cpprobotics_b200/) never does.
@@ -12,13 +12,13 @@ import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "liboracle_grid.so")
+from ._load import LIB_DIR, checker
+
+LIB_PATH = os.path.join(LIB_DIR, "liboracle_grid.so")
 
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 i32p = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
 u8p = np.ctypeslib.ndpointer(np.uint8, flags="C_CONTIGUOUS")
-_lib = None
 
 # include/crb.h
 ASTAR, DIJKSTRA = 0, 1
@@ -26,26 +26,19 @@ FOUND, NO_PATH, START_OUTSIDE, BAD_POINT = 0, 1, 2, 3
 MAX_SIDE, MAX_CELLS = 32768, 1 << 24
 
 
+PROTOTYPES = {
+    "crb_oracle_grid_box": (C.c_int, [C.c_int64, f32p, f32p, C.c_float, i32p]),
+    "crb_oracle_grid_map": (None, [C.c_int64, f32p, f32p, C.c_float, C.c_float, i32p, u8p]),
+    "crb_oracle_grid_plan": (None, [C.c_int, i32p, u8p, C.c_float, C.c_int64, f32p, C.c_int, C.c_void_p, i32p, f32p,
+                                    i32p, i32p, C.c_int]),
+    "crb_oracle_grid_trace": (C.c_int64, [C.c_int, i32p, u8p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
+                                          i32p, C.c_int64]),
+    "crb_oracle_grid_heap_run": (C.c_int64, [C.c_int64, u8p, f32p, i32p]),
+}
+
+
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            raise RuntimeError(f"{LIB_PATH} missing: run `make -C oracle -f grid.mk` (or python __graft_entry__.py)")
-        L = C.CDLL(LIB_PATH)
-        L.crb_oracle_grid_box.restype = C.c_int
-        L.crb_oracle_grid_box.argtypes = [C.c_int64, f32p, f32p, C.c_float, i32p]
-        L.crb_oracle_grid_map.restype = None
-        L.crb_oracle_grid_map.argtypes = [C.c_int64, f32p, f32p, C.c_float, C.c_float, i32p, u8p]
-        L.crb_oracle_grid_plan.restype = None
-        L.crb_oracle_grid_plan.argtypes = [C.c_int, i32p, u8p, C.c_float, C.c_int64, f32p, C.c_int, C.c_void_p,
-                                           i32p, f32p, i32p, i32p, C.c_int]
-        L.crb_oracle_grid_trace.restype = C.c_int64
-        L.crb_oracle_grid_trace.argtypes = [C.c_int, i32p, u8p, C.c_float, C.c_float, C.c_float, C.c_float,
-                                            C.c_float, i32p, C.c_int64]
-        L.crb_oracle_grid_heap_run.restype = C.c_int64
-        L.crb_oracle_grid_heap_run.argtypes = [C.c_int64, u8p, f32p, i32p]
-        _lib = L
-    return _lib
+    return checker(LIB_PATH, PROTOTYPES)
 
 
 def num_threads() -> int:

@@ -1,6 +1,6 @@
 """ctypes wrapper of oracle/lib/liboracle_lqrt.so — the CPU restatement of calc_nearest_index, lqr_steering_control and
 update of src/lqr_steer_control.cpp (nx 4) and src/lqr_speed_steer_control.cpp (nx 5).  Built by
-`make -C oracle -f lqrt.mk` (python __graft_entry__.py).
+`make -C oracle` (python __graft_entry__.py).
 
 TEST INFRASTRUCTURE ONLY, like oracle.py: tests/, __graft_entry__.smoke() and scripts may import it, the product
 package (cpprobotics_b200/) never does.
@@ -12,12 +12,12 @@ import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "liboracle_lqrt.so")
+from ._load import LIB_DIR, checker
+
+LIB_PATH = os.path.join(LIB_DIR, "liboracle_lqrt.so")
 
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 i32p = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
-_lib = None
 
 # include/crb.h
 OK, DARE_MAXITER, BAD_INDEX = 0, 1, 2
@@ -47,24 +47,18 @@ def params_from(prm) -> Params:
     return p
 
 
+PROTOTYPES = {
+    "crb_oracle_lqrt_nearest": (C.c_float, [f32p, f32p, f32p, f32p, C.c_int32, C.POINTER(C.c_int32)]),
+    "crb_oracle_lqrt_control_batched": (None, [C.c_int64, C.c_int, f32p, f32p, f32p, f32p, f32p, C.c_void_p, C.c_int32,
+                                               C.POINTER(Params), i32p, f32p, f32p, f32p, C.c_void_p, i32p, i32p,
+                                               C.c_int]),
+    "crb_oracle_lqrt_update_batched": (None, [C.c_int64, f32p, f32p, f32p, C.POINTER(Params), C.c_int]),
+    "crb_oracle_lqrt_ff_check": (C.c_int64, [C.c_double, C.c_uint32, C.c_uint32, f32p]),
+}
+
+
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            raise RuntimeError(f"{LIB_PATH} missing: run `make -C oracle -f lqrt.mk` (or python __graft_entry__.py)")
-        L = C.CDLL(LIB_PATH)
-        L.crb_oracle_lqrt_nearest.restype = C.c_float
-        L.crb_oracle_lqrt_nearest.argtypes = [f32p, f32p, f32p, f32p, C.c_int32, C.POINTER(C.c_int32)]
-        L.crb_oracle_lqrt_control_batched.restype = None
-        L.crb_oracle_lqrt_control_batched.argtypes = [C.c_int64, C.c_int, f32p, f32p, f32p, f32p, f32p, C.c_void_p,
-                                                      C.c_int32, C.POINTER(Params), i32p, f32p, f32p, f32p, C.c_void_p,
-                                                      i32p, i32p, C.c_int]
-        L.crb_oracle_lqrt_update_batched.restype = None
-        L.crb_oracle_lqrt_update_batched.argtypes = [C.c_int64, f32p, f32p, f32p, C.POINTER(Params), C.c_int]
-        L.crb_oracle_lqrt_ff_check.restype = C.c_int64
-        L.crb_oracle_lqrt_ff_check.argtypes = [C.c_double, C.c_uint32, C.c_uint32, f32p]
-        _lib = L
-    return _lib
+    return checker(LIB_PATH, PROTOTYPES)
 
 
 def num_threads() -> int:

@@ -1,5 +1,5 @@
 """ctypes wrapper of oracle/lib/liboracle_mptg.so — the CPU restatement of include/trajectory_optimizer.h
-(optimizer_traj) and include/motion_model.h (MotionModel, glibc's tanf).  Built by `make -C oracle -f mptg.mk`
+(optimizer_traj) and include/motion_model.h (MotionModel, glibc's tanf).  Built by `make -C oracle`
 (python __graft_entry__.py).
 
 TEST INFRASTRUCTURE ONLY, like oracle.py: tests/, __graft_entry__.smoke() and scripts may import it, the product
@@ -12,11 +12,11 @@ import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "liboracle_mptg.so")
+from ._load import LIB_DIR, checker
+
+LIB_PATH = os.path.join(LIB_DIR, "liboracle_mptg.so")
 
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
-_lib = None
 
 # include/crb.h
 CONVERGED, MAX_ITER_REACHED, EMPTY_TRAJ, STEP_CAP, OUT_OF_RANGE = 0, 1, 2, 3, 4
@@ -43,23 +43,19 @@ def mptg_params(**over) -> MptgParams:
     return p
 
 
+PROTOTYPES = {
+    "crb_oracle_num_threads": (C.c_int, []),
+    "crb_oracle_libm_tanf": (C.c_float, [C.c_float]),
+    "crb_oracle_libm_tanf_census": (C.c_int64, [C.c_uint32, C.c_uint32]),
+    "crb_oracle_mptg_optimize": (None, [C.c_int64, f32p, f32p, f32p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "crb_oracle_mptg_generate": (None, [C.c_int64, f32p, f32p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_int]),
+}
+
+
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            raise RuntimeError(f"{LIB_PATH} missing: run `make -C oracle -f mptg.mk` (or python __graft_entry__.py)")
-        L = C.CDLL(LIB_PATH)
-        L.crb_oracle_num_threads.restype = C.c_int
-        L.crb_oracle_libm_tanf.restype = C.c_float
-        L.crb_oracle_libm_tanf.argtypes = [C.c_float]
-        L.crb_oracle_libm_tanf_census.restype = C.c_int64
-        L.crb_oracle_libm_tanf_census.argtypes = [C.c_uint32, C.c_uint32]
-        L.crb_oracle_mptg_optimize.argtypes = [C.c_int64, f32p, f32p, f32p, C.c_void_p, C.c_int, C.c_void_p,
-                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-        L.crb_oracle_mptg_generate.argtypes = [C.c_int64, f32p, f32p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
-                                               C.c_void_p, C.c_void_p, C.c_int]
-        _lib = L
-    return _lib
+    return checker(LIB_PATH, PROTOTYPES)
 
 
 def num_threads() -> int:

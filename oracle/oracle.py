@@ -10,29 +10,68 @@ import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "liboracle.so")
+from ._load import LIB_DIR, checker
+
+LIB_PATH = os.path.join(LIB_DIR, "liboracle.so")
 
 ORDER_SEQ = 0
 ORDER_PAIRWISE = 1
 
-_lib = None
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 f64p = np.ctypeslib.ndpointer(np.float64, flags="C_CONTIGUOUS")
 i32p = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
 
 
-FAST_LIB_PATH = os.path.join(_HERE, "lib", "liboracle_fast.so")
-_libs = {}
+class MpcParams(C.Structure):
+    """Field-for-field the same as crb_mpc_params (include/crb.h)."""
+    _fields_ = [("dt", C.c_float), ("wb", C.c_float), ("max_steer", C.c_float),
+                ("max_accel", C.c_float), ("max_speed", C.c_float), ("min_speed", C.c_float),
+                ("w_a", C.c_float), ("w_delta", C.c_float), ("w_da", C.c_float),
+                ("w_ddelta", C.c_float), ("w_x", C.c_float), ("w_y", C.c_float),
+                ("w_yaw", C.c_float), ("w_v", C.c_float), ("max_iter", C.c_int),
+                ("du_th", C.c_float), ("max_ls", C.c_int), ("j_tol", C.c_float)]
+
+
+PROTOTYPES = {
+    "crb_oracle_num_threads": (C.c_int, []),
+    "crb_oracle_motion_model": (None, [f32p, f32p, C.c_double, f32p]),
+    "crb_oracle_jacobF": (None, [f32p, f32p, C.c_double, f32p]),
+    "crb_oracle_ekf_estimation": (None, [f32p, f32p, f32p, f32p, f32p, f32p, C.c_double, C.c_int]),
+    "crb_oracle_ekf_estimation_f64": (None, [f64p, f64p, f64p, f64p, f64p, f64p, C.c_double]),
+    "crb_oracle_ekf_step_batched": (None, [C.c_int64, f32p, f32p, f32p, f32p, f32p, f32p, C.c_double, C.c_int,
+                                           C.c_int, C.c_int]),
+    "crb_oracle_gauss_likelihood": (C.c_float, [C.c_float, C.c_float, C.c_double]),
+    "crb_oracle_pf_particle": (None, [f32p, f32p, f64p, f32p, f32p, f32p, C.c_int, C.c_float, C.c_double,
+                                      C.c_double]),
+    "crb_oracle_philox_normal2": (None, [C.c_uint64, C.c_uint64, f32p]),
+    "crb_oracle_philox_uniform12": (C.c_double, [C.c_uint64, C.c_uint64]),
+    "crb_oracle_pf_predict_weight_batched": (None, [C.c_int64, f32p, f32p, C.c_void_p, C.c_uint64, f32p, C.c_int,
+                                                    f32p, f32p, C.c_float, C.c_double, C.c_double, C.c_int]),
+    "crb_oracle_pf_estimate": (None, [C.c_int64, f32p, f32p, f32p, f32p, C.POINTER(C.c_double)]),
+    "crb_oracle_pf_resample": (C.c_int, [C.c_int64, f32p, f32p, f64p, C.c_float, C.c_int, C.POINTER(C.c_float)]),
+    "crb_oracle_dlqr_batched": (None, [C.c_int64, C.c_int, C.c_int, f32p, f32p, f32p, f32p, C.c_int, C.c_float,
+                                       f32p, f32p, i32p, C.c_int]),
+    "crb_oracle_sincosf": (None, [C.c_float, C.POINTER(C.c_float), C.POINTER(C.c_float)]),
+    "crb_oracle_mpc_solve_batched": (None, [C.c_int64, C.c_int, f32p, f32p, C.c_void_p, C.POINTER(MpcParams),
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "crb_oracle_plant_update": (None, [f32p, C.c_float, C.c_float]),
+    "crb_oracle_plant_update_k": (None, [f32p, C.c_float, C.c_float, f64p]),
+    "crb_oracle_calc_nearest_index": (C.c_int, [f32p, f32p, f32p, C.c_int, C.c_int]),
+    "crb_oracle_calc_ref_trajectory": (None, [f32p, f32p, f32p, f32p, f32p, C.c_int, C.c_float, C.c_int,
+                                              C.POINTER(C.c_int), f32p]),
+    "crb_oracle_calc_ref_trajectory_dt": (None, [f32p, f32p, f32p, f32p, f32p, C.c_int, C.c_float, C.c_int,
+                                                 C.POINTER(C.c_int), f32p, C.c_double]),
+}
 
 
 def use_library(which: str = "faithful") -> bool:
     """Selects the build the wrappers below call: "faithful" = liboracle.so (-O2 -ffp-contract=off, the
     parity oracle), "fast" = liboracle_fast.so (same sources, -O3 -march=x86-64-v3 -ffp-contract=fast:
-    BASELINE.md's B2 "what the host can do" timing arm; NOT a parity reference).  Returns False (and
-    keeps the faithful build) when the fast build is missing or the CPU lacks AVX2/FMA."""
-    global _lib, LIB_PATH
-    want = os.path.join(_HERE, "lib", "liboracle.so")
+    BASELINE.md's B2 "what the host can do" timing arm; NOT a parity reference), "O0" = liboracle_O0.so
+    (BASELINE.md B0 "as shipped", the reference's CMakeLists.txt:5: a timing arm only).  Returns False (and
+    selects the faithful build) when the build asked for is missing or, for "fast", the CPU lacks AVX2/FMA."""
+    global LIB_PATH
+    want = os.path.join(LIB_DIR, "liboracle.so")
     ok = True
     if which == "fast":
         flags = ""
@@ -40,46 +79,23 @@ def use_library(which: str = "faithful") -> bool:
             flags = open("/proc/cpuinfo").read()
         except OSError:
             pass
-        if os.path.exists(FAST_LIB_PATH) and " avx2" in flags and " fma" in flags:
-            want = FAST_LIB_PATH
+        fast = os.path.join(LIB_DIR, "liboracle_fast.so")
+        if os.path.exists(fast) and " avx2" in flags and " fma" in flags:
+            want = fast
         else:
             ok = False
-    if which == "O0":   # BASELINE.md B0 "as shipped" (-O0, the reference's CMakeLists.txt:5): a timing arm only
-        p0 = os.path.join(_HERE, "lib", "liboracle_O0.so")
+    if which == "O0":
+        p0 = os.path.join(LIB_DIR, "liboracle_O0.so")
         if os.path.exists(p0):
             want = p0
         else:
             ok = False
-    _libs[LIB_PATH] = _lib
     LIB_PATH = want
-    _lib = _libs.get(want)
     return ok
 
 
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            raise RuntimeError(f"{LIB_PATH} missing: run `make -C oracle` (or python __graft_entry__.py)")
-        L = C.CDLL(LIB_PATH)
-        L.crb_oracle_num_threads.restype = C.c_int
-        L.crb_oracle_motion_model.argtypes = [f32p, f32p, C.c_double, f32p]
-        L.crb_oracle_jacobF.argtypes = [f32p, f32p, C.c_double, f32p]
-        L.crb_oracle_ekf_estimation.argtypes = [f32p, f32p, f32p, f32p, f32p, f32p, C.c_double, C.c_int]
-        L.crb_oracle_ekf_estimation_f64.argtypes = [f64p, f64p, f64p, f64p, f64p, f64p, C.c_double]
-        L.crb_oracle_ekf_step_batched.argtypes = [C.c_int64, f32p, f32p, f32p, f32p, f32p, f32p,
-                                                  C.c_double, C.c_int, C.c_int, C.c_int]
-        L.crb_oracle_gauss_likelihood.restype = C.c_float
-        L.crb_oracle_gauss_likelihood.argtypes = [C.c_float, C.c_float, C.c_double]
-        L.crb_oracle_pf_particle.argtypes = [f32p, f32p, f64p, f32p, f32p, f32p, C.c_int, C.c_float,
-                                             C.c_double, C.c_double]
-        L.crb_oracle_philox_normal2.argtypes = [C.c_uint64, C.c_uint64, f32p]
-        L.crb_oracle_pf_predict_weight_batched.argtypes = [
-            C.c_int64, f32p, f32p, C.c_void_p, C.c_uint64, f32p, C.c_int, f32p, f32p, C.c_float,
-            C.c_double, C.c_double, C.c_int]
-        L.crb_oracle_pf_estimate.argtypes = [C.c_int64, f32p, f32p, f32p, f32p, C.POINTER(C.c_double)]
-        _lib = L
-    return _lib
+    return checker(LIB_PATH, PROTOTYPES)
 
 
 def num_threads() -> int:
@@ -178,8 +194,6 @@ def pf_predict_weight_batched(px, pw, noise, landmarks, seed=0, consts=None, nth
 def pf_resample(px, pw, uniforms, nth=None, reference_mode=False):
     """resampling() :120-148.  uniforms [n] in [1,2).  Returns (px, pw, did_resample, neff)."""
     L = lib()
-    L.crb_oracle_pf_resample.restype = C.c_int
-    L.crb_oracle_pf_resample.argtypes = [C.c_int64, f32p, f32p, f64p, C.c_float, C.c_int, C.POINTER(C.c_float)]
     px = np.ascontiguousarray(px, np.float32).copy()
     pw = np.ascontiguousarray(pw, np.float32).copy()
     n = px.shape[1]
@@ -190,18 +204,13 @@ def pf_resample(px, pw, uniforms, nth=None, reference_mode=False):
 
 
 def philox_uniform12(seed, index):
-    L = lib()
-    L.crb_oracle_philox_uniform12.restype = C.c_double
-    L.crb_oracle_philox_uniform12.argtypes = [C.c_uint64, C.c_uint64]
-    return L.crb_oracle_philox_uniform12(int(seed), int(index))
+    return lib().crb_oracle_philox_uniform12(int(seed), int(index))
 
 
 def dlqr_batched(A, B, Q, R, nx, nu, maxiter=150, eps=0.01, nthreads=0):
     """A [nx*nx, n], B [nx*nu, n] column-major per agent; Q [nx*nx], R [nu*nu] shared.
     Returns dict(K [nu*nx, n], X [nx*nx, n], iters [n])."""
     L = lib()
-    L.crb_oracle_dlqr_batched.argtypes = [C.c_int64, C.c_int, C.c_int, f32p, f32p, f32p, f32p, C.c_int, C.c_float,
-                                          f32p, f32p, i32p, C.c_int]
     A = np.ascontiguousarray(A, np.float32); B = np.ascontiguousarray(B, np.float32)
     n = A.shape[1]
     K = np.zeros((nu * nx, n), np.float32); X = np.zeros((nx * nx, n), np.float32); it = np.zeros(n, np.int32)
@@ -221,16 +230,6 @@ def pf_estimate(px, pw):
 
 
 # ---- MPC -------------------------------------------------------------------------------------------------
-class MpcParams(C.Structure):
-    """Field-for-field the same as crb_mpc_params (include/crb.h)."""
-    _fields_ = [("dt", C.c_float), ("wb", C.c_float), ("max_steer", C.c_float),
-                ("max_accel", C.c_float), ("max_speed", C.c_float), ("min_speed", C.c_float),
-                ("w_a", C.c_float), ("w_delta", C.c_float), ("w_da", C.c_float),
-                ("w_ddelta", C.c_float), ("w_x", C.c_float), ("w_y", C.c_float),
-                ("w_yaw", C.c_float), ("w_v", C.c_float), ("max_iter", C.c_int),
-                ("du_th", C.c_float), ("max_ls", C.c_int), ("j_tol", C.c_float)]
-
-
 def mpc_params(**over) -> MpcParams:
     """Reference constants (src/model_predictive_control.cpp:26-39, :202-210, :247-250, :326)."""
     d = dict(dt=0.2, wb=2.5, max_steer=np.float32(45.0 / 180 * np.pi), max_accel=1.0,
@@ -245,22 +244,7 @@ def mpc_params(**over) -> MpcParams:
 
 
 def _mpc_lib():
-    L = lib()
-    if not getattr(L, "_mpc_ready", False):
-        L.crb_oracle_sincosf.argtypes = [C.c_float, C.POINTER(C.c_float), C.POINTER(C.c_float)]
-        L.crb_oracle_mpc_solve_batched.argtypes = [
-            C.c_int64, C.c_int, f32p, f32p, C.c_void_p, C.POINTER(MpcParams), C.c_void_p, C.c_void_p,
-            C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
-        L.crb_oracle_plant_update.argtypes = [f32p, C.c_float, C.c_float]
-        L.crb_oracle_plant_update_k.argtypes = [f32p, C.c_float, C.c_float, f64p]
-        L.crb_oracle_calc_nearest_index.restype = C.c_int
-        L.crb_oracle_calc_nearest_index.argtypes = [f32p, f32p, f32p, C.c_int, C.c_int]
-        L.crb_oracle_calc_ref_trajectory.argtypes = [f32p, f32p, f32p, f32p, f32p, C.c_int, C.c_float,
-                                                     C.c_int, C.POINTER(C.c_int), f32p]
-        L.crb_oracle_calc_ref_trajectory_dt.argtypes = [f32p, f32p, f32p, f32p, f32p, C.c_int, C.c_float,
-                                                        C.c_int, C.POINTER(C.c_int), f32p, C.c_double]
-        L._mpc_ready = True
-    return L
+    return lib()
 
 
 def sincosf(x):

@@ -1,5 +1,5 @@
 """ctypes wrapper of oracle/lib/liboracle_rrt.so — the CPU restatement of RRT::planning (include/rrt.h) with
-std::mt19937, its two distributions and glibc's atan2f written out.  Built by `make -C oracle -f rrt.mk`
+std::mt19937, its two distributions and glibc's atan2f written out.  Built by `make -C oracle`
 (python __graft_entry__.py).
 
 TEST INFRASTRUCTURE ONLY, like oracle.py: tests/, __graft_entry__.smoke() and scripts may import it, the product
@@ -12,44 +12,35 @@ import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "liboracle_rrt.so")
+from ._load import LIB_DIR, checker
+
+LIB_PATH = os.path.join(LIB_DIR, "liboracle_rrt.so")
 
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 i32p = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
 u32p = np.ctypeslib.ndpointer(np.uint32, flags="C_CONTIGUOUS")
 i64p = np.ctypeslib.ndpointer(np.int64, flags="C_CONTIGUOUS")
-_lib = None
 
 # include/crb.h
 FOUND, MAX_ITER, BAD_INPUT = 0, 1, 2
 MAX_ITER_LIMIT = 16384
 
 
+PROTOTYPES = {
+    "crb_oracle_rrt_mt_run": (None, [C.c_uint32, C.c_int64, u32p]),
+    "crb_oracle_rrt_dist_run": (C.c_int64, [C.c_int, C.c_float, C.c_float, C.c_int64, u32p, u32p, i32p]),
+    "crb_oracle_rrt_atanf": (C.c_float, [C.c_float]),
+    "crb_oracle_rrt_atan2f": (C.c_float, [C.c_float, C.c_float]),
+    "crb_oracle_rrt_atanf_census": (C.c_int64, [C.c_uint32, C.c_uint32]),
+    "crb_oracle_rrt_atan2f_pairs": (C.c_int64, [C.c_int64, f32p, f32p]),
+    "crb_oracle_rrt_plan": (None, [C.c_float, C.c_float, C.c_float, C.c_int32, C.c_int32, f32p, C.c_int32, C.c_int64,
+                                   f32p, u32p, C.c_int32, C.c_void_p, i32p, C.c_int32, C.c_void_p, C.c_void_p, i32p,
+                                   i32p, i32p, i64p, i32p, C.c_int]),
+}
+
+
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            raise RuntimeError(f"{LIB_PATH} missing: run `make -C oracle -f rrt.mk` (or python __graft_entry__.py)")
-        L = C.CDLL(LIB_PATH)
-        L.crb_oracle_rrt_mt_run.restype = None
-        L.crb_oracle_rrt_mt_run.argtypes = [C.c_uint32, C.c_int64, u32p]
-        L.crb_oracle_rrt_dist_run.restype = C.c_int64
-        L.crb_oracle_rrt_dist_run.argtypes = [C.c_int, C.c_float, C.c_float, C.c_int64, u32p, u32p, i32p]
-        L.crb_oracle_rrt_atanf.restype = C.c_float
-        L.crb_oracle_rrt_atanf.argtypes = [C.c_float]
-        L.crb_oracle_rrt_atan2f.restype = C.c_float
-        L.crb_oracle_rrt_atan2f.argtypes = [C.c_float, C.c_float]
-        L.crb_oracle_rrt_atanf_census.restype = C.c_int64
-        L.crb_oracle_rrt_atanf_census.argtypes = [C.c_uint32, C.c_uint32]
-        L.crb_oracle_rrt_atan2f_pairs.restype = C.c_int64
-        L.crb_oracle_rrt_atan2f_pairs.argtypes = [C.c_int64, f32p, f32p]
-        L.crb_oracle_rrt_plan.restype = None
-        L.crb_oracle_rrt_plan.argtypes = [C.c_float, C.c_float, C.c_float, C.c_int32, C.c_int32, f32p, C.c_int32,
-                                          C.c_int64, f32p, u32p, C.c_int32, C.c_void_p, i32p, C.c_int32, C.c_void_p,
-                                          C.c_void_p, i32p, i32p, i32p, i64p, i32p, C.c_int]
-        _lib = L
-    return _lib
+    return checker(LIB_PATH, PROTOTYPES)
 
 
 def num_threads() -> int:

@@ -1,5 +1,5 @@
 // oracle/shim/ref_wrap.cpp — C entry points around the reference's own functions.  The reference source
-// file is #included from where it lies (REF_SRC, set by build_ref.sh) with main() renamed; nothing of it
+// file is #included from where it lies (REF_SRC, set by oracle/Makefile) with main() renamed; nothing of it
 // is copied into this repository.  WHICH selects the program: 1 EKF, 2 PF, 3 MPC.
 #define main crb_reference_main
 #include REF_SRC

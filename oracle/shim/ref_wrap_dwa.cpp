@@ -1,5 +1,5 @@
 // oracle/shim/ref_wrap_dwa.cpp — C entry points around the reference's own src/dynamic_window_approach.cpp.  The
-// file is #included from where it lies (REF_SRC, set by oracle/dwa.mk) with main() renamed; nothing of it is copied
+// file is #included from where it lies (REF_SRC, set by oracle/Makefile) with main() renamed; nothing of it is copied
 // into this repository.  <algorithm> and <limits> come first: the file uses std::max / std::min and
 // std::numeric_limits and relies on real OpenCV's headers to include them.
 #include <algorithm>

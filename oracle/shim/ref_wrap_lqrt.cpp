@@ -1,6 +1,6 @@
 // oracle/shim/ref_wrap_lqrt.cpp — C entry points around the LQR programs' own calc_nearest_index,
 // lqr_steering_control and update.  The reference source file is #included from where it lies (REF_SRC, set by
-// oracle/lqrt.mk) with main() renamed; nothing of it is copied into this repository.  WHICH selects the program:
+// oracle/Makefile) with main() renamed; nothing of it is copied into this repository.  WHICH selects the program:
 // 4 src/lqr_steer_control.cpp, 5 src/lqr_speed_steer_control.cpp.  st is (x, y, yaw, v).
 #define main crb_reference_main
 #include REF_SRC

@@ -1,5 +1,5 @@
 // oracle/shim/ref_wrap_mptg.cpp — C entry points around the reference's own include/trajectory_optimizer.h (and the
-// include/motion_model.h it includes).  The header is #included from where it lies (REF_HDR, set by oracle/mptg.mk);
+// include/motion_model.h it includes).  The header is #included from where it lies (REF_HDR, set by oracle/Makefile);
 // nothing of it is copied into this repository.  <limits> comes first: the header uses std::numeric_limits and
 // relies on real OpenCV's headers to include it.
 #include <limits>

@@ -1,5 +1,5 @@
 // oracle/shim/ref_wrap_slp.cpp — C entry points around the reference's own src/state_lattice_planner.cpp.  The file
-// is #included from where it lies (REF_SRC, set by oracle/slp.mk) with main() renamed; nothing of it is copied into
+// is #included from where it lies (REF_SRC, set by oracle/Makefile) with main() renamed; nothing of it is copied into
 // this repository.  <limits> comes first: the file and the headers it includes use std::numeric_limits and rely on
 // real OpenCV's headers to include it.
 #include <limits>

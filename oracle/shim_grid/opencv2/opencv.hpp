@@ -1,5 +1,5 @@
 // oracle/shim_grid/opencv2/opencv.hpp — NOT OpenCV: the stand-ins of oracle/shim/opencv2 plus what src/a_star.cpp and
-// src/dijkstra.cpp also use, cv::Point and cv::rectangle.  oracle/grid.mk puts this directory ahead of oracle/shim, so
+// src/dijkstra.cpp also use, cv::Point and cv::rectangle.  oracle/Makefile puts this directory ahead of oracle/shim, so
 // the planners' <opencv2/opencv.hpp> resolves here while <opencv2/core/core.hpp> and <opencv2/highgui/highgui.hpp>
 // resolve to oracle/shim (whose copy of opencv.hpp is then already included).
 //

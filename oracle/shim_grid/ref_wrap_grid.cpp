@@ -1,6 +1,6 @@
 // oracle/shim_grid/ref_wrap_grid.cpp — C entry point around the reference's own src/a_star.cpp or src/dijkstra.cpp (one
 // library each: both files define Node and calc_final_path).  The file is #included from where it lies (REF_SRC, set
-// by oracle/grid.mk) with main() renamed; nothing of it is copied into this repository.  REF_PLAN names the planner
+// by oracle/Makefile) with main() renamed; nothing of it is copied into this repository.  REF_PLAN names the planner
 // (a_star_planning or dijkstra_star_planning).
 //
 // The planners return nothing; everything they compute is drawn with cv::rectangle, which oracle/shim_grid's OpenCV

@@ -1,5 +1,5 @@
 // oracle/shim_rrt/opencv2/opencv.hpp — NOT OpenCV: the stand-ins of oracle/shim/opencv2 plus what include/rrt.h also
-// uses, cv::Point.  oracle/rrt.mk puts this directory ahead of oracle/shim, so the header's <opencv2/opencv.hpp>
+// uses, cv::Point.  oracle/Makefile puts this directory ahead of oracle/shim, so the header's <opencv2/opencv.hpp>
 // resolves here while <opencv2/core/core.hpp> and <opencv2/highgui/highgui.hpp> resolve to oracle/shim.
 //
 // RRT::planning loops until it reaches the goal and draws one cv::line per accepted node.  cv::Point is a type of its

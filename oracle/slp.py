@@ -1,7 +1,7 @@
 """ctypes wrapper of oracle/lib/liboracle_slp.so — the CPU restatement of src/state_lattice_planner.cpp's samplers
 (sample_states, calc_uniform_polar_states, calc_biased_polar_states, calc_lane_states) and its lookup-table search.
 generate_path is that search followed by the optimizer of liboracle_mptg.so (oracle/mptg.py).  Built by
-`make -C oracle -f slp.mk` (python __graft_entry__.py).
+`make -C oracle` (python __graft_entry__.py).
 
 TEST INFRASTRUCTURE ONLY, like oracle.py: tests/, __graft_entry__.smoke() and scripts may import it, the product
 package (cpprobotics_b200/) never does.
@@ -13,14 +13,14 @@ import os
 
 import numpy as np
 
+from ._load import LIB_DIR, checker
+
 from . import mptg as OM
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "liboracle_slp.so")
+LIB_PATH = os.path.join(LIB_DIR, "liboracle_slp.so")
 
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 i32p = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
-_lib = None
 
 # include/crb.h
 UNIFORM, BIASED, LANE = 0, 1, 2
@@ -52,17 +52,14 @@ def slp_params():
     return OM.mptg_params(base_l=1.0, ds=0.1, max_iter=100, cost_th=0.1, h_step=(0.5, 0.02, 0.02)), float(np.float32(3.0))
 
 
+PROTOTYPES = {
+    "crb_oracle_slp_sample": (None, [C.c_int64, C.POINTER(Sampler), C.c_int, f32p, f32p, i32p, C.c_void_p, C.c_int]),
+    "crb_oracle_slp_search": (None, [C.c_int64, f32p, f32p, C.c_int, C.c_void_p, f32p, C.c_void_p, C.c_int]),
+}
+
+
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            raise RuntimeError(f"{LIB_PATH} missing: run `make -C oracle -f slp.mk` (or python __graft_entry__.py)")
-        L = C.CDLL(LIB_PATH)
-        L.crb_oracle_slp_sample.argtypes = [C.c_int64, C.POINTER(Sampler), C.c_int, f32p, f32p, i32p, C.c_void_p,
-                                            C.c_int]
-        L.crb_oracle_slp_search.argtypes = [C.c_int64, f32p, f32p, C.c_int, C.c_void_p, f32p, C.c_void_p, C.c_int]
-        _lib = L
-    return _lib
+    return checker(LIB_PATH, PROTOTYPES)
 
 
 def sample(s: Sampler, qp, nthreads=0):

@@ -14,6 +14,7 @@ sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 
 import dwa_cases  # noqa: E402
 from cpprobotics_b200 import synth  # noqa: E402
+from oracle import _load  # noqa: E402
 from oracle import dwa as OD  # noqa: E402
 
 N = 128
@@ -52,7 +53,9 @@ def reference(lib, x, u, goal, ob, params):
 
 
 def main():
-    lib = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libref_dwa.so"))
+    lib = _load.reference("dwa")
+    if lib is None:
+        raise SystemExit("oracle/_ref not built: needs the reference tree (make -C oracle)")
     p = OD.dwa_params()
     out = {}
     for name, ob in OBSTACLE_SETS.items():

@@ -1,5 +1,5 @@
 """Writes tests/golden/grid_golden.npz from the reference's own text (oracle/_ref/libref_astar.so, libref_dijkstra.so,
-built by `make -C oracle -f grid.mk` where the reference tree is present): for each planner, the demo's obstacle map,
+built by `make -C oracle` where the reference tree is present): for each planner, the demo's obstacle map,
 expansion trace and path, and 24 seeded scenarios' inputs and paths (tests/grid_cases.py).  Cells are int16.
 
   python tests/golden/make_grid_golden.py"""
@@ -23,7 +23,7 @@ def main():
     for algo, name in GC.ALGOS:
         L = GC.ref_lib(algo)
         if L is None:
-            raise SystemExit("oracle/_ref not built: needs the reference tree (make -C oracle -f grid.mk)")
+            raise SystemExit("oracle/_ref not built: needs the reference tree (make -C oracle)")
         ox, oy, reso, rr, sg = GC.demo()
         r = GC.ref_run(L, *sg[:, 0], ox, oy, reso, rr)
         for k in ("map_cells", "trace", "path"):

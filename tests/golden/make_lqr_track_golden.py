@@ -1,5 +1,5 @@
 """Writes tests/golden/lqr_track_golden.npz from the reference's own text (oracle/_ref/libref_lqrt4.so and
-libref_lqrt5.so, built by `make -C oracle -f lqrt.mk` where the reference tree is present): lqr_steering_control's
+libref_lqrt5.so, built by `make -C oracle` where the reference tree is present): lqr_steering_control's
 outputs (u, ind, pe, pth_e) for 512 vehicles on each program's demo-shaped course, and update on 512 states.
 
   python tests/golden/make_lqr_track_golden.py"""
@@ -16,6 +16,7 @@ sys.path.insert(0, os.path.dirname(HERE))
 
 import lqr_track_cases as LC  # noqa: E402
 from cpprobotics_b200 import synth  # noqa: E402
+from oracle._load import reference  # noqa: E402
 
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 N = 512
@@ -25,10 +26,9 @@ def main():
     out = {}
     state = ind = pe = pth_e = None
     for nx in (4, 5):
-        path = os.path.join(ROOT, "oracle", "_ref", f"libref_lqrt{nx}.so")
-        if not os.path.exists(path):
-            raise SystemExit("oracle/_ref not built: needs the reference tree (oracle/shim/build_ref.sh)")
-        L = C.CDLL(path)
+        L = reference(f"lqrt{nx}")
+        if L is None:
+            raise SystemExit("oracle/_ref not built: needs the reference tree (make -C oracle)")
         course = synth.lqr_course("demo" if nx == 4 else "demo_speed")
         if state is None:
             state, ind, pe, pth_e = synth.lqr_track_inputs(N, course, seed=0x601D)
@@ -59,7 +59,7 @@ def main():
                     f"pth_e{nx}": o_pth})
     out.update(state=state, ind=ind, pe=pe, pth_e=pth_e)
     st, a, delta = LC.update_cases(N, seed=0x601E)
-    L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libref_lqrt4.so"))
+    L = reference("lqrt4")
     L.ref_lqr_update4.restype = None
     L.ref_lqr_update4.argtypes = [f32p, C.c_float, C.c_float]
     new = st.copy()

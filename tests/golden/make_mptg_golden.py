@@ -14,6 +14,7 @@ sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 
 import mptg_cases  # noqa: E402
 from cpprobotics_b200 import synth  # noqa: E402
+from oracle import _load  # noqa: E402
 from oracle import mptg as OM  # noqa: E402
 
 N = 96
@@ -53,7 +54,9 @@ def golden_sets():
 
 
 def main():
-    lib = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libref_mptg.so"))
+    lib = _load.reference("mptg")
+    if lib is None:
+        raise SystemExit("oracle/_ref not built: needs the reference tree (make -C oracle)")
     out = {}
     for name, st, tg, pa, prm in golden_sets():
         q, traj, tl, cost = reference(lib, st, tg, pa, prm, MAX_PTS)

@@ -4,7 +4,7 @@ of oracle/shim, see oracle/shim/README.md) on seeded inputs.  tests/test_oracle_
 CPU oracle against this file bit for bit, so the pin also holds where neither /root/reference nor
 oracle/_ref exists (a fresh clone, the GPU box).
 
-    make -C oracle ref && python tests/golden/make_ref_golden.py        (needs /root/reference)
+    make -C oracle && python tests/golden/make_ref_golden.py        (needs /root/reference)
 """
 import ctypes as C
 import os
@@ -17,16 +17,18 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 from cpprobotics_b200 import synth  # noqa: E402
 from oracle import oracle as O  # noqa: E402
+from oracle._load import reference  # noqa: E402
 
-REF = os.path.join(ROOT, "oracle", "_ref")
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 f64p = np.ctypeslib.ndpointer(np.float64, flags="C_CONTIGUOUS")
 
 
 def main():
+    L = reference("ekf")
+    if L is None:
+        raise SystemExit("oracle/_ref not built: needs the reference tree (make -C oracle)")
     out = {}
     # ---- EKF: ekf_estimation (src/extended_kalman_filter.cpp:64-78), 512 agents x 1 step ------------------
-    L = C.CDLL(os.path.join(REF, "libref_ekf.so"))
     L.ref_ekf_estimation.argtypes = [f32p] * 6
     n = 512
     x, P, z, u = synth.ekf_inputs(n, seed=0xBEEF)
@@ -39,7 +41,7 @@ def main():
     out.update(ekf_x=x, ekf_P=P, ekf_z=z, ekf_u=u, ekf_x_out=xo, ekf_P_out=Po)
 
     # ---- PF: pf_localization (:73-109) and resampling (:111-148), NP = 100 ---------------------------------
-    L = C.CDLL(os.path.join(REF, "libref_pf.so"))
+    L = reference("pf")
     L.ref_pf_np.restype = C.c_int
     L.ref_pf_localization.argtypes = [f32p, f32p, f32p, f32p, f32p, C.c_int, f32p, f32p, C.c_float, C.c_uint, f64p]
     L.ref_resampling.restype = C.c_int
@@ -63,7 +65,7 @@ def main():
                     f"rs{case}_px_out": rx.reshape(NP, 4).T.copy(), f"rs{case}_pw_out": rw})
 
     # ---- MPC helpers: update (:69-81), calc_nearest_index / calc_ref_trajectory (:107-170), FG_EVAL (:199-252)
-    L = C.CDLL(os.path.join(REF, "libref_mpc.so"))
+    L = reference("mpc")
     L.ref_mpc_T.restype = C.c_int
     L.ref_update.argtypes = [f32p, C.c_float, C.c_float]
     L.ref_calc_ref_trajectory.argtypes = [f32p, f32p, f32p, f32p, f32p, C.c_int, C.c_float, C.POINTER(C.c_int), f32p]
@@ -97,8 +99,8 @@ def main():
     out.update(fg_vars=v, fg_out=fg)
 
     # ---- LQR: solve_DARE + dlqr of both demos (lqr_steer_control.cpp:75-96, lqr_speed_steer_control.cpp:85-106)
-    for nx, nu, name in ((4, 1, "libref_lqr4.so"), (5, 2, "libref_lqr5.so")):
-        L = C.CDLL(os.path.join(REF, name))
+    for nx, nu in ((4, 1), (5, 2)):
+        L = reference(f"lqr{nx}")
         A, B, Qm, Rm = synth.lqr_inputs(64, nx, seed=77)
         K, X = np.zeros((nu * nx, 64), np.float32), np.zeros((nx * nx, 64), np.float32)
         for i in range(64):

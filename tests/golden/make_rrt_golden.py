@@ -1,5 +1,5 @@
 """Writes tests/golden/rrt_golden.npz from the reference's own text (oracle/_ref/libref_rrt.so, built by
-`make -C oracle -f rrt.mk` where the reference tree is present): the demo's node_list (tree, parents) and path for
+`make -C oracle` where the reference tree is present): the demo's node_list (tree, parents) and path for
 goal_gen seeds 1..32, and 16 scattered maps' inputs and paths (tests/rrt_cases.py).
 
   python tests/golden/make_rrt_golden.py"""
@@ -22,7 +22,7 @@ SCATTERED = 16
 def main():
     L = RC.ref_lib()
     if L is None:
-        raise SystemExit("oracle/_ref not built: needs the reference tree (make -C oracle -f rrt.mk)")
+        raise SystemExit("oracle/_ref not built: needs the reference tree (make -C oracle)")
     d = synth.RRT_DEMO
     prm, ob = RC.demo_prm(), synth.rrt_demo_obstacles()
     out = {}

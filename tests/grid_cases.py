@@ -4,16 +4,13 @@ the demo, seeded scenarios inside the reference's defined domain, corner cases, 
 the boxes away from the demo (rectangular, offset, at the ends of the int range, degenerate, a maze, maximum size),
 each with a one-line reason."""
 import ctypes as C
-import os
 
 import numpy as np
 
 from cpprobotics_b200 import synth
 from oracle import grid as OG
+from oracle._load import reference
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = {OG.ASTAR: os.path.join(ROOT, "oracle", "_ref", "libref_astar.so"),
-       OG.DIJKSTRA: os.path.join(ROOT, "oracle", "_ref", "libref_dijkstra.so")}
 ALGOS = ((OG.ASTAR, "astar"), (OG.DIJKSTRA, "dijkstra"))
 IMG_RESO = 5   # the planners' img_reso: a cell x is drawn from x * 5 + 1
 
@@ -30,8 +27,7 @@ def same(a, b):
 
 
 def ref_lib(algo):
-    p = REF[algo]
-    return C.CDLL(p) if os.path.exists(p) else None
+    return reference(dict(ALGOS)[algo])
 
 
 def ref_run(L, sx, sy, gx, gy, ox, oy, reso, rr):

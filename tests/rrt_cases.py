@@ -1,19 +1,16 @@
 """Inputs and reference calls for tests/test_rrt.py and tests/golden/make_rrt_golden.py: the demo, scattered maps,
 corner cases, and the reference's own RRT::planning (oracle/_ref/libref_rrt.so) with a seeded goal_gen."""
 import ctypes as C
-import os
 
 import numpy as np
 
 from cpprobotics_b200 import synth
 from oracle import rrt as OR
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "oracle", "_ref", "libref_rrt.so")
+from oracle._load import reference
 
 
 def ref_lib():
-    return C.CDLL(REF) if os.path.exists(REF) else None
+    return reference("rrt")
 
 
 def demo_prm(max_iter=4096):

@@ -8,10 +8,10 @@ import numpy as np
 
 from cpprobotics_b200 import synth
 from oracle import slp as OS
+from oracle._load import reference
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TABLE_CSV = os.path.join(ROOT, "tests", "golden", "lookuptable.csv")
-REF = os.path.join(ROOT, "oracle", "_ref", "libref_slp.so")
 
 
 def table():
@@ -25,7 +25,7 @@ def sampler_of(fields, **over):
 
 
 def ref_lib():
-    return C.CDLL(REF) if os.path.exists(REF) else None
+    return reference("slp")
 
 
 def _vp(a):

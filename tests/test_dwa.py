@@ -12,9 +12,9 @@ import pytest
 import dwa_cases as D
 from cpprobotics_b200 import _lib, synth
 from oracle import dwa as OD
+from oracle._load import reference
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "oracle", "_ref", "libref_dwa.so")
 GOLDEN = os.path.join(ROOT, "tests", "golden", "dwa_golden.npz")
 CPP = os.path.join(ROOT, "tests", "cpp", "dwa_ref_api.cpp")
 
@@ -46,10 +46,11 @@ def test_acosf_restatement_is_the_host_acosf_on_every_float_in_unit_interval():
 
 
 def _ref_lib():
-    if not os.path.exists(REF):
-        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle -f dwa.mk)")
+    L = reference("dwa")
+    if L is None:
+        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle)")
     import golden.make_dwa_golden as G
-    return C.CDLL(REF), G
+    return L, G
 
 
 @pytest.mark.parametrize("k", [0, 10, 64])
@@ -108,9 +109,10 @@ def test_defaults_are_the_reference_config_and_layout_matches(tmp_path):
     for k, _ in _lib.DwaParams._fields_:
         assert np.float32(getattr(lp, k)) == np.float32(getattr(op, k)), k
     assert np.float32(lp.max_yawrate) == np.float32(40.0 * 3.141592653 / 180.0) == np.float32(0.6981317)
-    if os.path.exists(REF):
+    L = reference("dwa")
+    if L is not None:
         cfg = np.zeros(12, np.float32)
-        C.CDLL(REF).ref_dwa_default_config(cfg.ctypes.data_as(C.c_void_p))
+        L.ref_dwa_default_config(cfg.ctypes.data_as(C.c_void_p))
         assert bits_equal(cfg, np.array([getattr(lp, k) for k, _ in _lib.DwaParams._fields_], np.float32))
     n = C.c_int(0)
     assert _lib.load_library().crb_dwa_rollout_points(C.byref(lp), C.byref(n)) == 0 and n.value == 32

@@ -14,9 +14,9 @@ import pytest
 import dwa_cases as D
 from cpprobotics_b200 import _lib, synth
 from oracle import dwa as OD
+from oracle._load import reference
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "oracle", "_ref", "libref_dwa.so")
 CPP = os.path.join(ROOT, "tests", "cpp", "dwa_ref_api.cpp")
 VCAP, WCAP = _lib.CRB_DWA_MAX_SPEED_SAMPLES, _lib.CRB_DWA_MAX_YAWRATE_SAMPLES
 f32 = np.float32
@@ -90,10 +90,11 @@ def robots(name, n, ob, seed):
 
 
 def _ref_lib():
-    if not os.path.exists(REF):
-        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle -f dwa.mk)")
+    L = reference("dwa")
+    if L is None:
+        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle)")
     import golden.make_dwa_golden as G
-    return C.CDLL(REF), G
+    return L, G
 
 
 def check_outcome(name, x, u, o, p):
@@ -308,10 +309,11 @@ def test_gpu_is_bitwise_the_checker_and_the_reference(engine, name, n):
     assert bits_equal(_gpu(engine, x, u, g, ob, p, outputs=False)["u"], o["u"])   # NULL outputs: the same u
     if n > 1:
         check_outcome(name, x, u, r, p)
-    if os.path.exists(REF):
+    L = reference("dwa")
+    if L is not None:
         import golden.make_dwa_golden as G
         cols = np.unique(np.r_[np.arange(0, n, max(1, n // 48)), np.arange(max(0, n - 8), n)])
-        ru, rc, rt, _ = G.reference(C.CDLL(REF), *(np.ascontiguousarray(a[:, cols]) for a in (x, u, g)), ob, p)
+        ru, rc, rt, _ = G.reference(L, *(np.ascontiguousarray(a[:, cols]) for a in (x, u, g)), ob, p)
         assert bits_equal(r["u"][:, cols], ru) and bits_equal(r["cost"][cols], rc)
         assert bits_equal(r["traj"][:, cols], rt)
 

@@ -27,7 +27,7 @@ ALGO_IDS = [a for a, _ in GC.ALGOS]
 def _ref(algo):
     L = GC.ref_lib(algo)
     if L is None:
-        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle -f grid.mk)")
+        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle)")
     return L
 
 

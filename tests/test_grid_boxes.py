@@ -505,7 +505,7 @@ def test_map_rr_cases_straddle_the_diagonal():
 def test_square_cases_are_bitwise_the_reference_text(algo, case):
     L = GC.ref_lib(algo)
     if L is None:
-        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle -f grid.mk)")
+        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle)")
     _, ox, oy, reso, rr, sx, sy, gx, gy = next(c for c in GC.square_cases() if c[0] == case)
     box = OG.box_of_obstacles(ox, oy, reso)
     m = OG.obstacle_map(ox, oy, reso, rr, box)

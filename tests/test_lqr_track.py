@@ -19,9 +19,9 @@ import lqr_track_cases as LC
 from cpprobotics_b200 import _lib, lqr_track_default_params, synth
 from oracle import lqrt as OL
 from oracle import oracle as O
+from oracle._load import reference
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "oracle", "_ref")
 GOLDEN = os.path.join(ROOT, "tests", "golden", "lqr_track_golden.npz")
 CPP_API = os.path.join(ROOT, "tests", "cpp", "lqr_ref_api.cpp")
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
@@ -44,10 +44,9 @@ def _bits_equal(a, b):
 def ref():
     libs = {}
     for nx in (4, 5):
-        path = os.path.join(REF, f"libref_lqrt{nx}.so")
-        if not os.path.exists(path):
-            pytest.skip("oracle/_ref not built")
-        L = C.CDLL(path)
+        L = reference(f"lqrt{nx}")
+        if L is None:
+            pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle)")
         i32r = C.POINTER(C.c_int)
         fr = C.POINTER(C.c_float)
         getattr(L, f"ref_lqr_nearest{nx}").restype = C.c_float

@@ -14,9 +14,9 @@ import pytest
 import mptg_cases as MC
 from cpprobotics_b200 import _lib, synth
 from oracle import mptg as OM
+from oracle._load import reference
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "oracle", "_ref", "libref_mptg.so")
 GOLDEN = os.path.join(ROOT, "tests", "golden", "mptg_golden.npz")
 CPP = os.path.join(ROOT, "tests", "cpp", "mptg_ref_api.cpp")
 MAX_PTS = 128  # the golden fixture's
@@ -57,10 +57,11 @@ def test_tanf_restatement_is_the_host_tanf_on_every_float_below_120():
 
 
 def _ref_lib():
-    if not os.path.exists(REF):
-        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle -f mptg.mk)")
+    L = reference("mptg")
+    if L is None:
+        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle)")
     import golden.make_mptg_golden as G
-    return C.CDLL(REF), G
+    return L, G
 
 
 def _compare_with_reference(L, G, st, tg, pa, prm, max_pts=MAX_PTS):

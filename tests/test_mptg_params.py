@@ -18,9 +18,9 @@ import pytest
 import mptg_cases as MC
 from cpprobotics_b200 import _lib, synth
 from oracle import mptg as OM
+from oracle._load import reference
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "oracle", "_ref", "libref_mptg.so")
 f32, f64 = np.float32, np.float64
 EPS = 2.0 ** -24                 # float32 unit roundoff
 PI, TWO_PI = np.pi, 2.0 * np.pi  # M_PI and 2 * M_PI as doubles
@@ -199,10 +199,11 @@ def check_result(o, o_prev, st, tg, prm, max_pts):
 
 # ---- CPU ------------------------------------------------------------------------------------------------------
 def _ref_lib():
-    if not os.path.exists(REF):
-        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle -f mptg.mk)")
+    L = reference("mptg")
+    if L is None:
+        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle)")
     import golden.make_mptg_golden as G
-    return C.CDLL(REF), G
+    return L, G
 
 
 def test_sets_reach_what_they_are_for():

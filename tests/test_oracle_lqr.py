@@ -1,7 +1,6 @@
 """CPU: solve_DARE()/dlqr() restatement (row f-4) against SciPy's DARE solution, the reference's own text
 (oracle/_ref) and its iteration semantics."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
@@ -9,8 +8,8 @@ import scipy.linalg as sl
 
 from cpprobotics_b200 import synth
 from oracle import oracle as O
+from oracle._load import reference
 
-REF = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref")
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 
 
@@ -39,12 +38,12 @@ def test_iteration_cap_and_tolerance_semantics():
     assert (tight["iters"] >= loose["iters"]).all()
 
 
+# lib is the library's file name: the test ids have carried it since the test was written
 @pytest.mark.parametrize("nx,nu,lib", [(4, 1, "libref_lqr4.so"), (5, 2, "libref_lqr5.so")])
 def test_restatement_is_bitwise_the_reference_text(nx, nu, lib):
-    path = os.path.join(REF, lib)
-    if not os.path.exists(path):
-        pytest.skip("oracle/_ref not built")
-    L = C.CDLL(path)
+    L = reference(lib.removeprefix("libref_").removesuffix(".so"))
+    if L is None:
+        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle)")
     A, B, Q, R = synth.lqr_inputs(200, nx, seed=12)
     r = O.dlqr_batched(A, B, Q, R, nx, nu)
     for i in range(200):

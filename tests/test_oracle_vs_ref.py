@@ -1,8 +1,7 @@
 """CPU: pins the oracle against the reference's OWN source files, compiled unmodified against header shims
 (oracle/shim -> oracle/_ref/libref_*.so; see oracle/shim/README.md for what this does and does not pin).
-Skipped when oracle/_ref was not built (it is built whenever /root/reference is present)."""
+Skipped when oracle/_ref was not built (make -C oracle builds it where the reference tree is present)."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
@@ -10,21 +9,21 @@ import pytest
 import ref_mpc as M
 from cpprobotics_b200 import synth
 from oracle import oracle as O
+from oracle._load import reference
 
-REF = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref")
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 f64p = np.ctypeslib.ndpointer(np.float64, flags="C_CONTIGUOUS")
 
 
 def _load(name):
-    path = os.path.join(REF, name)
-    if not os.path.exists(path):
-        pytest.skip("oracle/_ref not built (needs /root/reference: make -C oracle ref)")
-    return C.CDLL(path)
+    L = reference(name)
+    if L is None:
+        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle)")
+    return L
 
 
 def test_ekf_restatement_is_bitwise_the_reference_text():
-    L = _load("libref_ekf.so")
+    L = _load("ekf")
     L.ref_motion_model.argtypes = [f32p, f32p, f32p]
     L.ref_jacobF.argtypes = [f32p, f32p, f32p]
     L.ref_ekf_estimation.argtypes = [f32p] * 6
@@ -47,7 +46,7 @@ def test_ekf_restatement_is_bitwise_the_reference_text():
 
 
 def test_ekf_known_answer_through_the_reference_text():
-    L = _load("libref_ekf.so")
+    L = _load("ekf")
     L.ref_ekf_estimation.argtypes = [f32p] * 6
     dt, Q, R = O.ekf_constants()
     x, P = np.zeros(4, np.float32), np.eye(4, dtype=np.float32).reshape(-1).copy()
@@ -57,7 +56,7 @@ def test_ekf_known_answer_through_the_reference_text():
 
 
 def test_pf_restatement_is_bitwise_the_reference_text():
-    L = _load("libref_pf.so")
+    L = _load("pf")
     L.ref_gauss_likelihood.restype = C.c_float
     L.ref_gauss_likelihood.argtypes = [C.c_float, C.c_float]
     L.ref_pf_np.restype = C.c_int
@@ -93,7 +92,7 @@ def test_pf_restatement_is_bitwise_the_reference_text():
 
 
 def test_mpc_helpers_are_bitwise_the_reference_text():
-    L = _load("libref_mpc.so")
+    L = _load("mpc")
     L.ref_mpc_T.restype = C.c_int
     L.ref_update.argtypes = [f32p, C.c_float, C.c_float]
     L.ref_calc_nearest_index.restype = C.c_int
@@ -123,7 +122,7 @@ def test_nlp_statement_equals_fg_eval_and_solution_satisfies_it():
     """FG_EVAL::operator() (:199-252) evaluated by the reference's own code: (a) our statement of the cost
     (tests/ref_mpc.nlp_cost) is the same function, (b) the solver's answer is feasible for the reference's
     constraints and its reported cost is the reference's fg[0]."""
-    L = _load("libref_mpc.so")
+    L = _load("mpc")
     L.ref_fg_eval.argtypes = [f32p, f64p, f64p]
     T = 6
     course = synth.mpc_course()
@@ -152,7 +151,7 @@ def test_nlp_statement_equals_fg_eval_and_solution_satisfies_it():
 def test_resampling_restatement_is_bitwise_the_reference_text():
     """resampling() + cumsum() (:111-148) of the reference's own source against oracle.pf_resample in
     reference_mode, on peaked weights (Neff < NP/2 -> resample) and on flat ones (no resample)."""
-    L = _load("libref_pf.so")
+    L = _load("pf")
     L.ref_resampling.restype = C.c_int
     L.ref_resampling.argtypes = [f32p, f32p, C.c_uint, f64p]
     NP = 100

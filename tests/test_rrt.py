@@ -39,7 +39,7 @@ def same(a, b):
 def _ref():
     L = RC.ref_lib()
     if L is None:
-        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle -f rrt.mk)")
+        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle)")
     return L
 
 

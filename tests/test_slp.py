@@ -37,7 +37,7 @@ def same(a, b):
 def _ref():
     L = SC.ref_lib()
     if L is None:
-        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle -f slp.mk)")
+        pytest.skip("oracle/_ref not built (needs the reference tree: make -C oracle)")
     return L
 
 
