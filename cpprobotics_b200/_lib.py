@@ -48,7 +48,8 @@ CRB_GRID_FOUND = 0
 CRB_GRID_NO_PATH = 1
 CRB_GRID_START_OUTSIDE = 2
 CRB_GRID_BAD_POINT = 3
-CRB_LQR_TRACK_OK, CRB_LQR_TRACK_DARE_MAXITER, CRB_LQR_TRACK_BAD_INDEX = 0, 1, 2
+CRB_LQR_TRACK_OK, CRB_LQR_TRACK_DARE_MAXITER, CRB_LQR_TRACK_BAD_INDEX, CRB_LQR_TRACK_BAD_COURSE = 0, 1, 2, 3
+CRB_MPC_REF_OK, CRB_MPC_REF_BAD_COURSE = 0, 1
 CRB_RRT_MAX_ITER = 16384
 CRB_RRT_FOUND = 0
 CRB_RRT_MAX_ITER_REACHED = 1
@@ -166,6 +167,10 @@ PROTOTYPES = {
                                                       C.c_void_p, C.c_void_p, C.c_void_p,
                                                       C.c_void_p, C.c_int32, C.c_float, C.c_void_p,
                                                       C.c_void_p, C.POINTER(MpcParams)]),
+    "crb_mpc_calc_ref_trajectory_many_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                                           C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p,
+                                                           C.c_void_p, C.POINTER(MpcParams)]),
     "crb_lqr_dlqr_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
                                        C.c_void_p]),
@@ -203,6 +208,11 @@ PROTOTYPES = {
                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                                    C.POINTER(LqrTrackParams), C.c_void_p, C.c_void_p, C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "crb_lqr_steering_control_many_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                        C.c_int32, C.c_int64, C.c_void_p, C.POINTER(LqrTrackParams),
+                                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                        C.c_void_p, C.c_void_p]),
     "crb_lqr_update_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.POINTER(LqrTrackParams)]),
     "crb_stats_reduce": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,

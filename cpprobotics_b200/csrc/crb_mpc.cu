@@ -886,21 +886,20 @@ extern "C" int crb_mpc_plant_update_batched(crb_ctx* ctx, int64_t n, float* stat
 }
 
 // ---- calc_ref_trajectory :130-170 with calc_nearest_index :107-127 -------------------------------------
-__global__ void __launch_bounds__(256)
-crb_mpc_ref_traj_kernel(int64_t n, int T, const float* __restrict__ state,
-                        const float* __restrict__ cx, const float* __restrict__ cy,
-                        const float* __restrict__ cyaw, const float* __restrict__ sp, int ncourse,
-                        float dl, int32_t* __restrict__ target_ind, float* __restrict__ xref,
-                        const double DT) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float sx = state[i], sy = state[n + i], sv = state[3 * n + i];
+// Agent i against the course cx .. sp of ncourse points; both lookup kernels run it.  The search window and the end
+// clamp never leave [0, ncourse): an index at or past 2^31 (a target_ind below -9) ends the window, as one at or past
+// ncourse does, and ind + dind is compared in 64 bits, so a sum past INT_MAX clamps to the last point.
+__device__ __forceinline__ void mpc_ref_traj_agent(int64_t i, int64_t n, int T, float sx, float sy, float sv,
+                                                   const float* __restrict__ cx, const float* __restrict__ cy,
+                                                   const float* __restrict__ cyaw, const float* __restrict__ sp,
+                                                   int ncourse, float dl, int32_t* __restrict__ target_ind,
+                                                   float* __restrict__ xref, const double DT) {
   const int pind = target_ind[i];
   // calc_nearest_index: float-typed index (:109), strict '<' keeps the first minimum (:115)
   float mind = 3.402823466e+38f;
   float find = 0;
   for (unsigned int j = (unsigned int)pind; j < (unsigned int)pind + 10u; ++j) {
-    if ((int)j >= ncourse) break;
+    if (j >= (unsigned int)ncourse) break;
     const float idx = cx[j] - sx;
     const float idy = cy[j] - sy;
     const float d_e = idx * idx + idy * idy;
@@ -912,13 +911,60 @@ crb_mpc_ref_traj_kernel(int64_t n, int T, const float* __restrict__ state,
   for (int t = 0; t < T; ++t) {
     travel = (float)((double)travel + (double)fabsf(sv) * DT);  // :149
     const int dind = (int)roundf(travel / dl);                  // :150
-    const int j = (ind + dind) < ncourse ? ind + dind : ncourse - 1;
+    const int j = (int64_t)ind + dind < ncourse ? ind + dind : ncourse - 1;
     xref[((int64_t)t * 4 + 0) * n + i] = cx[j];
     xref[((int64_t)t * 4 + 1) * n + i] = cy[j];
     xref[((int64_t)t * 4 + 2) * n + i] = cyaw[j];
     xref[((int64_t)t * 4 + 3) * n + i] = sp[j];
   }
   target_ind[i] = ind;  // :169
+}
+
+__global__ void __launch_bounds__(256)
+crb_mpc_ref_traj_kernel(int64_t n, int T, const float* __restrict__ state,
+                        const float* __restrict__ cx, const float* __restrict__ cy,
+                        const float* __restrict__ cyaw, const float* __restrict__ sp, int ncourse,
+                        float dl, int32_t* __restrict__ target_ind, float* __restrict__ xref,
+                        const double DT) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  mpc_ref_traj_agent(i, n, T, state[i], state[n + i], state[3 * n + i], cx, cy, cyaw, sp, ncourse, dl, target_ind,
+                     xref, DT);
+}
+
+// The lookup with a course per agent: the agent's course reference is checked before any course data is read
+// (course_of[i] in [0, n_courses), 0 <= course_off[c] < course_off[c + 1] <= npts, a length that fits in int); a bad
+// one gives NaN xref, leaves target_ind and sets CRB_MPC_REF_BAD_COURSE.  One thread per agent: the window is 10
+// points and the horizon at most CRB_MPC_MAX_T.
+__global__ void __launch_bounds__(256)
+crb_mpc_lookup_many_kernel(int64_t n, int T, const float* __restrict__ state, const float* __restrict__ cx,
+                           const float* __restrict__ cy, const float* __restrict__ cyaw,
+                           const float* __restrict__ sp, const int64_t* __restrict__ course_off, int32_t n_courses,
+                           int64_t npts, const int32_t* __restrict__ course_of, float dl,
+                           int32_t* __restrict__ target_ind, float* __restrict__ xref, int32_t* __restrict__ status,
+                           const double DT) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int32_t c = course_of[i];
+  int64_t a = 0, b = 0;
+  if (c >= 0 && c < n_courses) { a = course_off[c]; b = course_off[c + 1]; }
+  if (c < 0 || c >= n_courses || a < 0 || a >= b || b > npts || b - a > 0x7fffffff) {
+    const float q = __int_as_float(0x7fffffff);
+    for (int f = 0; f < 4 * T; ++f) xref[(int64_t)f * n + i] = q;
+    if (status) status[i] = CRB_MPC_REF_BAD_COURSE;
+    return;
+  }
+  mpc_ref_traj_agent(i, n, T, state[i], state[n + i], state[3 * n + i], cx + a, cy + a, cyaw + a, sp + a, (int)(b - a),
+                     dl, target_ind, xref, DT);
+  if (status) status[i] = CRB_MPC_REF_OK;
+}
+
+static int mpc_check_lookup(int64_t n, int T, float dl, const crb_mpc_params* prm) {
+  CRB_REQUIRE(n >= 0 && T >= 1 && T <= CRB_MPC_MAX_T, "n < 0 or T out of range");
+  CRB_REQUIRE(dl > 0.0f, "dl <= 0");
+  // the lookup uses only dt
+  CRB_REQUIRE(prm != nullptr && isfinite(prm->dt) && prm->dt > 0.0f, "prm is NULL or dt not finite and > 0");
+  return CRB_OK;
 }
 
 extern "C" int crb_mpc_calc_ref_trajectory_batched(crb_ctx* ctx, int64_t n, int T,
@@ -928,15 +974,35 @@ extern "C" int crb_mpc_calc_ref_trajectory_batched(crb_ctx* ctx, int64_t n, int 
                                                    int32_t* target_ind, float* xref,
                                                    const crb_mpc_params* prm) {
   CRB_REQUIRE(ctx != nullptr, "ctx is NULL");
-  CRB_REQUIRE(n >= 0 && T >= 1 && T <= CRB_MPC_MAX_T, "n < 0 or T out of range");
-  CRB_REQUIRE(ncourse >= 1 && dl > 0.0f, "empty course or dl <= 0");
-  // the lookup uses only dt
-  CRB_REQUIRE(prm != nullptr && isfinite(prm->dt) && prm->dt > 0.0f, "prm is NULL or dt not finite and > 0");
+  CRB_REQUIRE(ncourse >= 1, "empty course");
+  const int rc = mpc_check_lookup(n, T, dl, prm);
+  if (rc) return rc;
   if (n == 0) return CRB_OK;
   CRB_REQUIRE(state && cx && cy && cyaw && sp && target_ind && xref, "NULL array");
   CRB_DEVICE_GUARD(ctx);   // ctx->device is current for this call, the caller's device is restored after it
   crb_mpc_ref_traj_kernel<<<crb_grid_for(n, 256), 256, 0, ctx->stream>>>(
       n, T, state, cx, cy, cyaw, sp, ncourse, dl, target_ind, xref, mpc_plant_constants(prm).dt);
+  CRB_CUDA(cudaGetLastError());
+  ctx->launches++;
+  return CRB_OK;
+}
+
+extern "C" int crb_mpc_calc_ref_trajectory_many_batched(crb_ctx* ctx, int64_t n, int T, const float* state,
+                                                        const float* cx, const float* cy, const float* cyaw,
+                                                        const float* sp, const int64_t* course_off,
+                                                        int32_t n_courses, int64_t npts, const int32_t* course_of,
+                                                        float dl, int32_t* target_ind, float* xref, int32_t* status,
+                                                        const crb_mpc_params* prm) {
+  CRB_REQUIRE(ctx != nullptr, "ctx is NULL");
+  CRB_REQUIRE(n_courses >= 1 && npts >= 1, "n_courses and npts must be >= 1");
+  const int rc = mpc_check_lookup(n, T, dl, prm);
+  if (rc) return rc;
+  if (n == 0) return CRB_OK;
+  CRB_REQUIRE(state && cx && cy && cyaw && sp && course_off && course_of && target_ind && xref, "NULL array");
+  CRB_DEVICE_GUARD(ctx);
+  crb_mpc_lookup_many_kernel<<<crb_grid_for(n, 256), 256, 0, ctx->stream>>>(
+      n, T, state, cx, cy, cyaw, sp, course_off, n_courses, npts, course_of, dl, target_ind, xref, status,
+      mpc_plant_constants(prm).dt);
   CRB_CUDA(cudaGetLastError());
   ctx->launches++;
   return CRB_OK;

@@ -8,6 +8,7 @@ Method names follow the reference functions they replace:
   Engine.mpc_solve           <- mpc_solve()             src/model_predictive_control.cpp:255-346
   Engine.mpc_plant_update    <- update()                src/model_predictive_control.cpp:69-81
   Engine.calc_ref_trajectory <- calc_ref_trajectory()   src/model_predictive_control.cpp:130-170
+  Engine.calc_ref_trajectory_many <- the same, each agent on its own course (synth.pack_courses)
   Engine.dwa_control         <- dwa_control()           src/dynamic_window_approach.cpp:148-155
   Engine.dwa_motion          <- motion()                src/dynamic_window_approach.cpp:43-50
   Engine.mptg_optimize       <- TrajectoryOptimizer::optimizer_traj()  include/trajectory_optimizer.h:53-128
@@ -22,6 +23,7 @@ Method names follow the reference functions they replace:
   Engine.rrt_plan            <- RRT::planning()                                  include/rrt.h:75-159
   Engine.lqr_steering_control <- lqr_steering_control() (+ calc_nearest_index)   src/lqr_steer_control.cpp:98-133,
                                                                                  src/lqr_speed_steer_control.cpp:108-151
+  Engine.lqr_steering_control_many <- the same, each vehicle on its own course (synth.pack_courses)
   Engine.lqr_update          <- update()                 src/lqr_steer_control.cpp:136-146 (same text in both programs)
 
 All arrays are SoA field-major float32 (`[fields, n]`, C-contiguous); see include/crb.h.  Methods
@@ -160,7 +162,7 @@ def _ptr(a, dtype, *, device: Optional[bool], name: str) -> int:
         return None
     if torch is not None and isinstance(a, torch.Tensor):
         want = {np.float32: torch.float32, np.int32: torch.int32, np.float64: torch.float64,
-                np.uint8: torch.uint8}[dtype]
+                np.uint8: torch.uint8, np.int64: torch.int64}[dtype]
         if a.dtype != want:
             raise TypeError(f"{name}: expected {want}, got {a.dtype}")
         if not a.is_contiguous():
@@ -407,6 +409,32 @@ class Engine:
             _ptr(target_ind, np.int32, device=True, name="target_ind"),
             _ptr(xref, np.float32, device=True, name="xref"), C.byref(prm)),
             "crb_mpc_calc_ref_trajectory_batched")
+
+    def calc_ref_trajectory_many(self, state, courses, course_of, dl: float, target_ind, xref, T: int,
+                                 params: Optional[MpcParams] = None, status=None):
+        """calc_ref_trajectory with a course per agent.  courses (cx, cy, cyaw, sp, course_off): the concatenated
+        courses [npts] float32 and course_off [n_courses + 1] int64 (synth.pack_courses); course_of [n] int32, the
+        course of each agent; target_ind [n] in/out, course-local; xref [4*T, n] out; status [n] int32
+        (CRB_MPC_REF_*) is allocated when not given.  Returns status.  CUDA tensors; only enqueues."""
+        n = int(state.shape[-1])
+        _shape(state, 4, n, "state"); _shape(xref, 4 * T, n, "xref")
+        cx, cy, cyaw, sp, off = courses
+        npts = int(cx.shape[0])
+        for a, name in ((cx, "cx"), (cy, "cy"), (cyaw, "cyaw"), (sp, "sp")):
+            _shape(a, 1, npts, name)
+        _shape(course_of, 1, n, "course_of"); _shape(target_ind, 1, n, "target_ind")
+        status = status if status is not None else torch.empty(n, dtype=torch.int32, device=state.device)
+        _shape(status, 1, n, "status")
+        prm = params if params is not None else mpc_default_params()
+        f = lambda a, name: _ptr(a, np.float32, device=True, name=name)  # noqa: E731
+        check(self.lib.crb_mpc_calc_ref_trajectory_many_batched(
+            self.ctx, n, int(T), f(state, "state"), f(cx, "cx"), f(cy, "cy"), f(cyaw, "cyaw"), f(sp, "sp"),
+            _ptr(off, np.int64, device=True, name="course_off"), int(off.shape[0]) - 1, npts,
+            _ptr(course_of, np.int32, device=True, name="course_of"), C.c_float(dl),
+            _ptr(target_ind, np.int32, device=True, name="target_ind"), f(xref, "xref"),
+            _ptr(status, np.int32, device=True, name="status"), C.byref(prm)),
+            "crb_mpc_calc_ref_trajectory_many_batched")
+        return status
 
     # ---- LQR --------------------------------------------------------------------------------------
     def dlqr(self, A, B, Q, R, nx: int, nu: int, maxiter: int = 150, eps: float = 0.01, K=None, X=None,
@@ -751,6 +779,42 @@ class Engine:
             _ptr(ind, np.int32, device=True, name="ind"), f(pe, "pe"), f(pth_e, "pth_e"), f(u, "u"), f(K, "K"),
             _ptr(iters, np.int32, device=True, name="iters"), _ptr(status, np.int32, device=True, name="status")),
             "crb_lqr_steering_control_batched")
+        return dict(u=u, K=K, iters=iters, status=status)
+
+    def lqr_steering_control_many(self, nx: int, state, courses, course_of, ind, pe, pth_e,
+                                  params: Optional[LqrTrackParams] = None, u=None, K=None, iters=None, status=None):
+        """lqr_steering_control() for n vehicles, each on its own course.  courses (cx, cy, cyaw, ck, course_off) for
+        nx 4 or (cx, cy, cyaw, ck, sp, course_off) for nx 5: the concatenated courses [npts] float32 and course_off
+        [n_courses + 1] int64 (synth.pack_courses); course_of [n] int32, the course of each vehicle.  ind is
+        course-local.  Everything else as lqr_steering_control; status may be CRB_LQR_TRACK_BAD_COURSE."""
+        n = int(state.shape[-1])
+        nu = 1 if nx == 4 else 2
+        _shape(state, 4, n, "state")
+        if len(courses) != (5 if nx == 4 else 6):
+            raise ValueError(f"courses: expected {5 if nx == 4 else 6} arrays for nx = {nx}, got {len(courses)}")
+        pts, off = courses[:-1], courses[-1]
+        npts = int(pts[0].shape[0])
+        for a, name in zip(pts, ("cx", "cy", "cyaw", "ck", "sp")):
+            _shape(a, 1, npts, name)
+        for a, name in ((course_of, "course_of"), (ind, "ind"), (pe, "pe"), (pth_e, "pth_e")):
+            _shape(a, 1, n, name)
+        dev = state.device
+        if u is None:
+            u = torch.empty((nu, n), dtype=torch.float32, device=dev)
+        iters = iters if iters is not None else torch.empty(n, dtype=torch.int32, device=dev)
+        status = status if status is not None else torch.empty(n, dtype=torch.int32, device=dev)
+        _shape(u, nu, n, "u")
+        if K is not None:
+            _shape(K, nu * nx, n, "K")
+        prm = params if params is not None else lqr_track_default_params(nx)
+        f = lambda a, name: _ptr(a, np.float32, device=True, name=name)  # noqa: E731
+        check(self.lib.crb_lqr_steering_control_many_batched(
+            self.ctx, n, int(nx), f(state, "state"), f(pts[0], "cx"), f(pts[1], "cy"), f(pts[2], "cyaw"),
+            f(pts[3], "ck"), f(pts[4], "sp") if nx == 5 else None, _ptr(off, np.int64, device=True, name="course_off"),
+            int(off.shape[0]) - 1, npts, _ptr(course_of, np.int32, device=True, name="course_of"), C.byref(prm),
+            _ptr(ind, np.int32, device=True, name="ind"), f(pe, "pe"), f(pth_e, "pth_e"), f(u, "u"), f(K, "K"),
+            _ptr(iters, np.int32, device=True, name="iters"), _ptr(status, np.int32, device=True, name="status")),
+            "crb_lqr_steering_control_many_batched")
         return dict(u=u, K=K, iters=iters, status=status)
 
     def lqr_update(self, state, a, delta, params: Optional[LqrTrackParams] = None):

@@ -215,5 +215,45 @@ def run() -> None:
                                              (lr["iters"], lo["iters"]), (lr["status"], lo["status"]), (dst, lnew)))
         assert ok, f"LQR tracking (nx {nx}) GPU result is not bit-identical to the checker"
     print("smoke LQRT  257 vehicles, 4- and 5-state control and update on the demo course: bit-identical to the checker")
+    # a course per vehicle: 257 vehicles in random order over 8 fleet courses, 4- and 5-state control and the MPC
+    # lookup, every output as the checker run course by course
+    mcourses = synth.fleet_courses(8, seed=0x5A1)
+    packed = synth.pack_courses(mcourses)
+    mof = np.random.default_rng(0x5A2).integers(0, 8, 257).astype(np.int32)
+    mst = np.zeros((4, 257), np.float32)
+    mind = np.zeros(257, np.int32)
+    for c in range(8):
+        sel = np.nonzero(mof == c)[0]
+        mst[:, sel], mind[sel] = synth.lqr_track_inputs(sel.size, mcourses[c], seed=c)[:2]
+    dpk = [torch.from_numpy(a).to(dev) for a in packed]
+    for nx in (4, 5):
+        dind = torch.from_numpy(mind.copy()).to(dev)
+        dz = torch.zeros(257, dtype=torch.float32, device=dev)
+        dz2 = torch.zeros(257, dtype=torch.float32, device=dev)
+        mr = eng.lqr_steering_control_many(nx, torch.from_numpy(mst).to(dev), dpk[:4] + dpk[5:] if nx == 4 else dpk,
+                                           torch.from_numpy(mof).to(dev), dind, dz, dz2)
+        torch.cuda.synchronize()
+        ok = True
+        for c in range(8):
+            sel = np.nonzero(mof == c)[0]
+            z = np.zeros(sel.size, np.float32)
+            mo = OL.control(nx, mst[:, sel], mcourses[c], mind[sel], z, z)
+            sel_t = torch.from_numpy(sel)
+            ok = ok and all(same_nan(g[..., sel_t], w) for g, w in ((mr["u"].cpu(), mo["u"]), (dind.cpu(), mo["ind"]),
+                                                                    (mr["status"].cpu(), mo["status"])))
+        assert ok, f"many-course LQR tracking (nx {nx}) GPU result is not bit-identical to the checker"
+    T = 8
+    dti = torch.from_numpy(mind.copy()).to(dev)
+    xr = torch.empty((4 * T, 257), dtype=torch.float32, device=dev)
+    eng.calc_ref_trajectory_many(torch.from_numpy(mst).to(dev), (dpk[0], dpk[1], dpk[2], dpk[4], dpk[5]),
+                                 torch.from_numpy(mof).to(dev), 1.0, dti, xr, T)
+    torch.cuda.synchronize()
+    xh, th = xr.cpu(), dti.cpu().numpy()
+    for i in range(257):
+        cx, cy, cyaw, _, sp = mcourses[mof[i]]
+        wx, wt = O.calc_ref_trajectory(mst[:, i], cx, cy, cyaw, sp, 1.0, T, int(mind[i]))
+        assert wt == th[i] and same_nan(xh[:, i], wx.reshape(-1)), "many-course MPC lookup is not the checker"
+    print("smoke MANY  257 vehicles on 8 courses, LQR control (4 and 5 states) and the MPC lookup: bit-identical to "
+          "the checker")
     print(f"smoke ok: {eng.launches} kernel launches through libcrb.so")
     eng.close()

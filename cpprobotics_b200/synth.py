@@ -595,3 +595,49 @@ def lqr_track_inputs(n: int, course, seed: int = 0xC0FFEE):
     pe = rng.uniform(-1.0, 1.0, n).astype(np.float32)
     pth_e = rng.uniform(-0.5, 0.5, n).astype(np.float32)
     return state, ind, pe, pth_e
+
+
+# ---- many courses: the *_many entry points (a course per vehicle) ---------------------------------------------------
+def pack_courses(courses):
+    """A list of courses (cx, cy, cyaw, ck, sp) -> (cx, cy, cyaw, ck, sp, course_off): each field of every course
+    concatenated in list order (float32 [npts]) and course_off (int64 [n_courses + 1]), course c being
+    [course_off[c], course_off[c + 1])."""
+    lens = [len(c[0]) for c in courses]
+    off = np.zeros(len(courses) + 1, np.int64)
+    off[1:] = np.cumsum(lens)
+    fields = tuple(np.ascontiguousarray(np.concatenate([np.asarray(c[f], np.float32).reshape(-1) for c in courses])
+                                        if courses else np.zeros(0, np.float32)) for f in range(5))
+    return fields + (off,)
+
+
+def _mpc_course_with_curvature():
+    cx, cy, cyaw, sp = mpc_course()
+    s = np.arange(0.0, 500.0, 1.0)
+    dy, ddy = np.cos(s / 20.0), -np.sin(s / 20.0) / 20.0
+    return cx, cy, cyaw, (ddy / (1.0 + dy * dy) ** 1.5).astype(np.float32), sp
+
+
+def fleet_courses(n_courses: int, seed: int = 0xF1EE7):
+    """n_courses varied courses (cx, cy, cyaw, ck, sp) for a fleet: each a random stretch of one of the LQR_KINDS
+    courses or the MPC course (mpc_course, with its curvature), rotated by a random angle (cyaw turns with it) and
+    moved by up to 500 m.  Lengths run from 2 points to the whole base course; every 16th course (the second, the
+    eighteenth, ...) and about one in twenty others have a single point.  Deterministic for a seed."""
+    rng = np.random.default_rng(seed)
+    bases = [lqr_course(k) for k in LQR_KINDS] + [_mpc_course_with_curvature()]
+    out = []
+    for c in range(n_courses):
+        b = bases[int(rng.integers(0, len(bases)))]
+        nb = len(b[0])
+        if c % 16 == 1 or rng.random() < 0.05:
+            ln = 1
+        else:
+            ln = int(rng.integers(2, nb + 1))
+        s0 = int(rng.integers(0, nb - ln + 1))
+        th = rng.uniform(-np.pi, np.pi)
+        tx, ty = rng.uniform(-500.0, 500.0, 2)
+        x, y = (np.asarray(a[s0:s0 + ln], np.float64) for a in b[:2])
+        ct, st = np.cos(th), np.sin(th)
+        out.append(tuple(np.ascontiguousarray(a, np.float32) for a in (
+            ct * x - st * y + tx, st * x + ct * y + ty, np.asarray(b[2][s0:s0 + ln], np.float64) + th,
+            b[3][s0:s0 + ln], b[4][s0:s0 + ln])))
+    return out

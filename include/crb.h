@@ -15,6 +15,8 @@
  *   crb_mpc_solve_batched[_host]        <- mpc_solve() + FG_EVAL            src/model_predictive_control.cpp:188-346
  *   crb_mpc_plant_update_batched        <- update()                          src/model_predictive_control.cpp:69-81
  *   crb_mpc_calc_ref_trajectory_batched <- calc_ref_trajectory() :130-170 + calc_nearest_index() :107-127
+ *   crb_mpc_calc_ref_trajectory_many_batched <- the same, each agent on its own course (the reference takes the
+ *                                          course per call)
  *   crb_lqr_dlqr_batched                <- solve_DARE() + dlqr()  src/lqr_steer_control.cpp:75-96,
  *                                          src/lqr_speed_steer_control.cpp:85-106
  *   crb_dwa_control_batched             <- dwa_control()         src/dynamic_window_approach.cpp:148-155
@@ -38,6 +40,8 @@
  *   crb_lqr_steering_control_batched    <- lqr_steering_control() src/lqr_steer_control.cpp:98-133 (4 states),
  *                                          src/lqr_speed_steer_control.cpp:108-151 (5 states), with
  *                                          calc_nearest_index() :55-73 / :65-83 and solve_DARE() + dlqr() inside
+ *   crb_lqr_steering_control_many_batched <- the same, each vehicle on its own course (the reference takes the
+ *                                          course per call)
  *   crb_lqr_update_batched              <- update()              src/lqr_steer_control.cpp:136-146,
  *                                          src/lqr_speed_steer_control.cpp:154-164
  *   crb_stats_*                         <- (no reference counterpart) per-GPU summary statistics, the
@@ -312,13 +316,39 @@ int crb_mpc_plant_update_batched(crb_ctx* ctx, int64_t n, float* state, const fl
  *   state [4][n]; target_ind [n] in/out (int32); xref [4*T][n] out
  * Integer index work is bit-exact with the reference, including its quirks (float-typed index,
  * :109; strict '<' first-minimum tie-break, :115; monotone target_ind, :139).  The reference reads
- * cx[pind+9] without a bounds check (:110); here the search window is clipped to the course.
+ * cx[pind+9] without a bounds check (:110); here the search window is clipped to the course, and a target_ind
+ * below -9 (a window index at or past 2^31 as the reference's unsigned loop counts) searches nothing.
  * Replaces: calc_ref_trajectory() :130-170 and calc_nearest_index() :107-127. */
 int crb_mpc_calc_ref_trajectory_batched(crb_ctx* ctx, int64_t n, int T, const float* state,
                                         const float* cx, const float* cy, const float* cyaw,
                                         const float* sp, int32_t ncourse, float dl,
                                         int32_t* target_ind, float* xref,
                                         const crb_mpc_params* prm);
+
+/* Per-agent status of crb_mpc_calc_ref_trajectory_many_batched. */
+#define CRB_MPC_REF_OK 0
+#define CRB_MPC_REF_BAD_COURSE 1 /* course_of[i] does not name a course of 1 to INT32_MAX points inside [0, npts):
+                                    xref is NaN and target_ind is left as it is */
+
+/* Course store of the *_many_batched entry points: every course's points concatenated.
+ *   cx, cy, cyaw, ck, sp [npts]  the courses back to back (npts is int64_t)
+ *   course_off [n_courses + 1] int64_t: course c is [course_off[c], course_off[c + 1])
+ *   course_of [n] int32_t: the course of each agent; agents may share a course and need not be sorted by it
+ * The offsets are device data: each agent's course is checked on the device before any course point is read
+ * (0 <= c < n_courses, 0 <= course_off[c] < course_off[c + 1] <= npts, a length that fits in int32); an agent that
+ * fails gets its entry point's BAD_COURSE status and nothing outside the arrays is read.  Indices (ind, target_ind)
+ * are course-local: they count from the start of the agent's own course, as the reference sees them. */
+
+/* crb_mpc_calc_ref_trajectory_batched with a course per agent (the course store above; no ck).  Each agent's
+ * outputs are bitwise those of crb_mpc_calc_ref_trajectory_batched run on its own course, at any target_ind.
+ * status [n] int32 CRB_MPC_REF_* is optional (NULL = not written).  CRB_ERR_INVALID_ARG before any device work as
+ * crb_mpc_calc_ref_trajectory_batched, and unless n_courses >= 1, npts >= 1 and, for n > 0, course_off and
+ * course_of are given.  DEVICE pointers; only enqueues (graph-capturable). */
+int crb_mpc_calc_ref_trajectory_many_batched(crb_ctx* ctx, int64_t n, int T, const float* state, const float* cx,
+                                             const float* cy, const float* cyaw, const float* sp,
+                                             const int64_t* course_off, int32_t n_courses, int64_t npts,
+                                             const int32_t* course_of, float dl, int32_t* target_ind, float* xref,
+                                             int32_t* status, const crb_mpc_params* prm);
 
 /* ---- LQR (SURVEY.md §8 row f-4) ------------------------------------------------------------------- */
 /* Discrete LQR gain by the reference's fixed-point DARE iteration, one problem per agent.
@@ -669,6 +699,9 @@ void crb_lqr_track_default_params(crb_lqr_track_params* p, int nx);
 #define CRB_LQR_TRACK_BAD_INDEX 2    /* no course point won the scan (every squared distance NaN or >= FLT_MAX) and
                                         the incoming ind is outside [0, ncourse), where the reference reads out of
                                         bounds: u and K are NaN, iters 0, ind / pe / pth_e are left as they are */
+#define CRB_LQR_TRACK_BAD_COURSE 3   /* crb_lqr_steering_control_many_batched: course_of[i] does not name a course
+                                        of 1 to INT32_MAX points inside [0, npts): u and K are NaN, iters 0, ind / pe /
+                                        pth_e are left as they are */
 
 /* lqr_steering_control for n vehicles against one course shared by the batch.
  *   nx 4: lqr_steer_control.cpp (nu = 1); nx 5: lqr_speed_steer_control.cpp (nu = 2)
@@ -690,6 +723,20 @@ int crb_lqr_steering_control_batched(crb_ctx* ctx, int64_t n, int nx, const floa
                                      const float* cy, const float* cyaw, const float* ck, const float* sp,
                                      int32_t ncourse, const crb_lqr_track_params* prm, int32_t* ind, float* pe,
                                      float* pth_e, float* u, float* K, int32_t* iters, int32_t* status);
+/* crb_lqr_steering_control_batched with a course per vehicle: cx, cy, cyaw, ck, sp [npts], course_off and course_of
+ * are the course store described above crb_mpc_calc_ref_trajectory_many_batched; every other argument is as there,
+ * including the 4-state program's persistent ind and CRB_LQR_TRACK_BAD_INDEX, both against the vehicle's own course.
+ * Each vehicle's outputs are bitwise those of crb_lqr_steering_control_batched run on its own course.  Each warp
+ * searches one vehicle's course at a time (coalesced loads, a warp argmin that keeps the first minimum), then one
+ * thread per vehicle runs the rest.  CRB_ERR_INVALID_ARG before any device work as crb_lqr_steering_control_batched,
+ * and unless n_courses >= 1, npts >= 1 and, for n > 0, course_off and course_of are given.  DEVICE pointers; only
+ * enqueues (graph-capturable). */
+int crb_lqr_steering_control_many_batched(crb_ctx* ctx, int64_t n, int nx, const float* state, const float* cx,
+                                          const float* cy, const float* cyaw, const float* ck, const float* sp,
+                                          const int64_t* course_off, int32_t n_courses, int64_t npts,
+                                          const int32_t* course_of, const crb_lqr_track_params* prm, int32_t* ind,
+                                          float* pe, float* pth_e, float* u, float* K, int32_t* iters,
+                                          int32_t* status);
 /* update(State&, a, delta) of the LQR programs for n vehicles: state [4][n] in/out, a [n], delta [n].  The kinematic
  * bicycle of crb_mpc_plant_update_batched with prm's dt, wheelbase and max_steer used as the doubles they are, and
  * no speed clamp.  Requires finite dt, wheelbase and max_steer with |max_steer| < 120 (the range in which tanf is

@@ -881,7 +881,7 @@ class RRT {
 // signature; a main() written against one program says `using namespace cpprobotics::lqr_steer_control;` and calls
 // lqr_steering_control(...) and lqr_steer_control::update(...).  calc_nearest_index runs inside lqr_steering_control.
 // The single-vehicle calls copy the course to the device on every call, as the reference copies its vectors by value;
-// the batched overloads take a fleet at once.
+// the batched overloads take a fleet at once, on one course or with a course per vehicle.
 // ---------------------------------------------------------------------------------------------------
 namespace cpprobotics {
 namespace detail {
@@ -927,6 +927,67 @@ inline void lqr_control(int nx, const std::vector<State>& st, const Vec_f& cx, c
   crb::check(crb_lqr_steering_control_batched(ctx, n, nx, dst, dcx, dcy, dcyaw, dck, dsp, (int32_t)nc, &prm, dind, dpe,
                                               dpth, du, nullptr, nullptr, nullptr),
              "crb_lqr_steering_control_batched");
+  crb::check(crb_memcpy_d2h(ctx, ind, dind, nn * 4), "crb_memcpy_d2h");
+  crb::check(crb_memcpy_d2h(ctx, pe, dpe, nn * 4), "crb_memcpy_d2h");
+  crb::check(crb_memcpy_d2h(ctx, pth_e, dpth, nn * 4), "crb_memcpy_d2h");
+  crb::check(crb_memcpy_d2h(ctx, u, du, nu * nn * 4), "crb_memcpy_d2h");
+}
+// one control call for n vehicles, vehicle i on its own course (cx[i], cy[i], ...), through the session's device arena:
+// the courses packed back to back with one int64 offset per course, course_of[i] = i
+inline void lqr_control_many(int nx, const std::vector<State>& st, const std::vector<Vec_f>& cx,
+                             const std::vector<Vec_f>& cy, const std::vector<Vec_f>& cyaw, const std::vector<Vec_f>& ck,
+                             const std::vector<Vec_f>* sp, int32_t* ind, float* pe, float* pth_e, float* u) {
+  const size_t nn = st.size();
+  if (cx.size() != nn || cy.size() != nn || cyaw.size() != nn || ck.size() != nn || (sp && sp->size() != nn))
+    throw std::runtime_error("lqr_steering_control: one course per state");
+  std::vector<int64_t> off(nn + 1, 0);
+  for (size_t i = 0; i < nn; ++i) {
+    const size_t nc = cx[i].size();
+    if (nc == 0 || cy[i].size() != nc || cyaw[i].size() != nc || ck[i].size() != nc || (sp && (*sp)[i].size() != nc))
+      throw std::runtime_error("lqr_steering_control: each course's vectors must be non-empty and of one length");
+    off[i + 1] = off[i] + (int64_t)nc;
+  }
+  if (nn == 0) return;
+  const int nu = nx == 4 ? 1 : 2;
+  const size_t np = (size_t)off[nn];
+  const int nf = sp ? 5 : 4;
+  // layout: course_off (n+1) int64 | course fields (nf x np) | state 4n | ind n | pe n | pth_e n | u nu*n | course_of n
+  const size_t need = 2 * (nn + 1) + nf * np + (4 + 3 + nu + 1) * nn;
+  crb_ctx* ctx = crb::Session::get();
+  float* arena = crb::Session::scratch(need);
+  int64_t* doff = (int64_t*)arena;
+  float* base = arena + 2 * (nn + 1);
+  const std::vector<Vec_f>* fields[5] = {&cx, &cy, &cyaw, &ck, sp};
+  std::vector<float> packed(np);
+  for (int f = 0; f < nf; ++f) {
+    for (size_t i = 0; i < nn; ++i) std::copy((*fields[f])[i].begin(), (*fields[f])[i].end(), packed.begin() + off[i]);
+    crb::check(crb_memcpy_h2d(ctx, base + f * np, packed.data(), np * 4), "crb_memcpy_h2d");
+  }
+  float* dst = base + nf * np;
+  int32_t* dind = (int32_t*)(dst + 4 * nn);
+  float* dpe = (float*)(dind + nn);
+  float* dpth = dpe + nn;
+  float* du = dpth + nn;
+  int32_t* dof = (int32_t*)(du + nu * nn);
+  std::vector<float> soa(4 * nn);
+  std::vector<int32_t> course_of(nn);
+  for (size_t i = 0; i < nn; ++i) {
+    soa[i] = st[i].x; soa[nn + i] = st[i].y; soa[2 * nn + i] = st[i].yaw; soa[3 * nn + i] = st[i].v;
+    course_of[i] = (int32_t)i;
+  }
+  crb::check(crb_memcpy_h2d(ctx, dst, soa.data(), soa.size() * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dind, ind, nn * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dpe, pe, nn * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dpth, pth_e, nn * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, dof, course_of.data(), nn * 4), "crb_memcpy_h2d");
+  crb::check(crb_memcpy_h2d(ctx, doff, off.data(), (nn + 1) * 8), "crb_memcpy_h2d");
+  crb_lqr_track_params prm;
+  crb_lqr_track_default_params(&prm, nx);
+  crb::check(crb_lqr_steering_control_many_batched(ctx, (int64_t)nn, nx, dst, base, base + np, base + 2 * np,
+                                                   base + 3 * np, sp ? base + 4 * np : nullptr, doff, (int32_t)nn,
+                                                   (int64_t)np, dof, &prm, dind, dpe, dpth, du, nullptr, nullptr,
+                                                   nullptr),
+             "crb_lqr_steering_control_many_batched");
   crb::check(crb_memcpy_d2h(ctx, ind, dind, nn * 4), "crb_memcpy_d2h");
   crb::check(crb_memcpy_d2h(ctx, pe, dpe, nn * 4), "crb_memcpy_d2h");
   crb::check(crb_memcpy_d2h(ctx, pth_e, dpth, nn * 4), "crb_memcpy_d2h");
@@ -980,6 +1041,20 @@ inline Vec_f lqr_steering_control(const std::vector<State>& states, const Vec_f&
   for (size_t i = 0; i < n; ++i) ind[i] = i32[i];
   return delta;
 }
+// a fleet with a course per vehicle: state i follows (cx[i], cy[i], cyaw[i], ck[i]); ind (course-local), pe, pth_e
+// one per state (in/out); returns delta per state
+inline Vec_f lqr_steering_control(const std::vector<State>& states, const std::vector<Vec_f>& cx,
+                                  const std::vector<Vec_f>& cy, const std::vector<Vec_f>& cyaw,
+                                  const std::vector<Vec_f>& ck, std::vector<int>& ind, Vec_f& pe, Vec_f& pth_e) {
+  const size_t n = states.size();
+  if (ind.size() != n || pe.size() != n || pth_e.size() != n)
+    throw std::runtime_error("lqr_steering_control: ind, pe and pth_e need one value per state");
+  std::vector<int32_t> i32(ind.begin(), ind.end());
+  Vec_f delta(n);
+  detail::lqr_control_many(4, states, cx, cy, cyaw, ck, nullptr, i32.data(), pe.data(), pth_e.data(), delta.data());
+  for (size_t i = 0; i < n; ++i) ind[i] = i32[i];
+  return delta;
+}
 // :136-146
 inline void update(State& state, float a, float delta) {
   std::vector<State> s(1, state);
@@ -1008,6 +1083,22 @@ inline std::vector<Vec_f> lqr_steering_control(const std::vector<State>& states,
   std::vector<int32_t> ind(n, 0);
   Vec_f u(2 * n);
   detail::lqr_control(5, states, cx, cy, cyaw, ck, &sp, ind.data(), pe.data(), pth_e.data(), u.data());
+  std::vector<Vec_f> out(n);
+  for (size_t i = 0; i < n; ++i) out[i] = Vec_f{u[i], u[n + i]};
+  return out;
+}
+// a fleet with a course per vehicle: state i follows (cx[i], cy[i], cyaw[i], ck[i], sp[i]); pe, pth_e one per state
+// (in/out); returns {ai, delta} per state
+inline std::vector<Vec_f> lqr_steering_control(const std::vector<State>& states, const std::vector<Vec_f>& cx,
+                                               const std::vector<Vec_f>& cy, const std::vector<Vec_f>& cyaw,
+                                               const std::vector<Vec_f>& ck, const std::vector<Vec_f>& sp, Vec_f& pe,
+                                               Vec_f& pth_e) {
+  const size_t n = states.size();
+  if (pe.size() != n || pth_e.size() != n)
+    throw std::runtime_error("lqr_steering_control: pe and pth_e need one value per state");
+  std::vector<int32_t> ind(n, 0);
+  Vec_f u(2 * n);
+  detail::lqr_control_many(5, states, cx, cy, cyaw, ck, &sp, ind.data(), pe.data(), pth_e.data(), u.data());
   std::vector<Vec_f> out(n);
   for (size_t i = 0; i < n; ++i) out[i] = Vec_f{u[i], u[n + i]};
   return out;

@@ -10,8 +10,18 @@ the worst case).  Each cell is timed with CUDA events over --reps launches after
 ms per launch, calls/s, the mean and max DARE iterations, the same launch on a 1-point course (the DARE without the
 scan), achieved FP32 FLOP/s with the flops counted from the executed iterations and the course length, against
 crb_probe_fp32_peak measured in the same run, the checker's calls/s on every host core (on 2^16 vehicles) and whether
-the GPU outputs are bit-identical to it.  The card's name and power limit are read in the same run.  Needs a CUDA
-device: there is no CPU fallback."""
+the GPU outputs are bit-identical to it.
+
+Many-course cells (crb_lqr_steering_control_many_batched, a course per vehicle), both nx, 2^16 and 2^20 vehicles at the
+demo speeds: "one_course" (every vehicle on the demo-shaped course, timed next to the shared-course entry point on the
+same inputs), "4096x430" (4096 demo-length courses, the demo course rotated and moved) and "64x8192" (64 courses of the
+8192-point course, rotated and moved), vehicles shuffled across the courses.  Reported per cell: ms per launch and
+calls/s, the same fleet as one shared-course launch per course (the host loop a caller would otherwise write), and
+whether the outputs are bitwise those per-course launches.  Then the MPC lookup
+(crb_mpc_calc_ref_trajectory_many_batched, T = 20) at 2^20 agents on the 4096 courses, next to the single-course lookup
+on one course.
+
+The card's name and power limit are read in the same run.  Needs a CUDA device: there is no CPU fallback."""
 import argparse
 import ctypes as C
 import json
@@ -59,6 +69,136 @@ def same(a, b):
         return np.array_equal(a, b)
     na, nb = np.isnan(a), np.isnan(b)
     return np.array_equal(na, nb) and np.array_equal(a[~na].view(np.uint32), b[~nb].view(np.uint32))
+
+
+def moved(course, rng):
+    """course rotated by a random angle (cyaw turns with it) and moved by up to 500 m."""
+    th = rng.uniform(-np.pi, np.pi)
+    tx, ty = rng.uniform(-500.0, 500.0, 2)
+    x, y = course[0].astype(np.float64), course[1].astype(np.float64)
+    return tuple(np.ascontiguousarray(v, np.float32) for v in (
+        np.cos(th) * x - np.sin(th) * y + tx, np.sin(th) * x + np.cos(th) * y + ty,
+        course[2].astype(np.float64) + th, course[3], course[4]))
+
+
+def event_ms(fn, reps):
+    import torch
+    fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(torch.cuda.current_stream())
+    for _ in range(reps):
+        fn()
+    e1.record(torch.cuda.current_stream())
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+def many_courses(a, eng, res, dev, base):
+    """The many-course cells (see the module docstring)."""
+    import torch
+    rng = np.random.default_rng(0x4A7)
+    sets = {"one_course": [base["demo"]],
+            "4096x430": [moved(base["demo"], rng) for _ in range(4096)],
+            "64x8192": [moved(base["course8192"], rng) for _ in range(64)]}
+    res["many_cells"] = []
+    for cname, courses in sets.items():
+        packed = synth.pack_courses(courses)
+        dpk = [torch.from_numpy(x).to(dev) for x in packed]
+        dsingle = [[torch.from_numpy(x).to(dev) for x in c] for c in courses]
+        for nx in (4, 5):
+            nu = 1 if nx == 4 else 2
+            dcs = dpk[:4] + dpk[5:] if nx == 4 else dpk
+            for log2n in (16, 20):
+                n = 1 << log2n
+                course_of = rng.integers(0, len(courses), n).astype(np.int32)
+                st = np.zeros((4, n), np.float32)
+                ind, pe, pth = np.zeros(n, np.int32), np.zeros(n, np.float32), np.zeros(n, np.float32)
+                groups = [np.nonzero(course_of == c)[0] for c in range(len(courses))]
+                for c, sel in enumerate(groups):
+                    if sel.size:
+                        st[:, sel], ind[sel], pe[sel], pth[sel] = synth.lqr_track_inputs(sel.size, courses[c],
+                                                                                         seed=log2n * 10007 + c)
+                dst, dof = torch.from_numpy(st).to(dev), torch.from_numpy(course_of).to(dev)
+                dind, dpe, dpth = (torch.from_numpy(x.copy()).to(dev) for x in (ind, pe, pth))
+                u = torch.empty((nu, n), dtype=torch.float32, device=dev)
+                it = torch.empty(n, dtype=torch.int32, device=dev)
+                stt = torch.empty(n, dtype=torch.int32, device=dev)
+                # the scan and the DARE depend on x only; ind, pe, pth_e are replaced by every call
+                ms = event_ms(lambda: eng.lqr_steering_control_many(nx, dst, dcs, dof, dind, dpe, dpth, u=u, iters=it,
+                                                                    status=stt), a.reps)
+                # the same fleet, one shared-course launch per course on that course's vehicles (gathered beforehand)
+                per = []
+                for c, sel in enumerate(groups):
+                    if sel.size:
+                        ts = [torch.from_numpy(np.ascontiguousarray(x)).to(dev)
+                              for x in (st[:, sel], ind[sel], pe[sel], pth[sel])]
+                        per.append((c, sel, ts, torch.empty((nu, sel.size), dtype=torch.float32, device=dev),
+                                    torch.empty(sel.size, dtype=torch.int32, device=dev),
+                                    torch.empty(sel.size, dtype=torch.int32, device=dev)))
+
+                def per_course():
+                    for c, sel, ts, pu, pit, pst in per:
+                        eng.lqr_steering_control(nx, ts[0], dsingle[c][: 4 if nx == 4 else 5], ts[1], ts[2], ts[3],
+                                                 u=pu, iters=pit, status=pst)
+                ms_per = event_ms(per_course, max(1, a.reps // 5))
+                # bitwise: one fresh call of each on the original inputs
+                dind, dpe, dpth = (torch.from_numpy(x.copy()).to(dev) for x in (ind, pe, pth))
+                eng.lqr_steering_control_many(nx, dst, dcs, dof, dind, dpe, dpth, u=u, iters=it, status=stt)
+                for c, sel, ts, pu, pit, pst in per:
+                    for t, x in zip(ts[1:], (ind[sel], pe[sel], pth[sel])):
+                        t.copy_(torch.from_numpy(x))
+                per_course()
+                torch.cuda.synchronize()
+                got = [x.cpu().numpy() for x in (u, dind, dpe, dpth, it, stt)]
+                want = [np.zeros_like(x) for x in got]
+                for c, sel, ts, pu, pit, pst in per:
+                    for w, x in zip(want, (pu, ts[1], ts[2], ts[3], pit, pst)):
+                        w[..., sel] = x.cpu().numpy()
+                cell = dict(nx=nx, courses=cname, n_courses=len(courses), points=int(packed[0].size), n=n, ms=ms,
+                            calls_per_s=n / (ms * 1e-3), ms_launch_per_course=ms_per,
+                            launches_per_course=len(per),
+                            bit_identical_to_per_course=bool(all(same(g, w) for g, w in zip(got, want))))
+                if cname == "one_course":
+                    ms1 = event_ms(lambda: eng.lqr_steering_control(nx, dst, dsingle[0][: 4 if nx == 4 else 5], dind,
+                                                                    dpe, dpth, u=u, iters=it, status=stt), a.reps)
+                    cell.update(ms_shared_course_kernel=ms1, shared_course_calls_per_s=n / (ms1 * 1e-3))
+                res["many_cells"].append(cell)
+                print(json.dumps(cell), flush=True)
+    # the MPC lookup at 2^20 agents on the 4096 courses, next to the single-course lookup on the demo course
+    T, n = 20, 1 << 20
+    courses = sets["4096x430"]
+    packed = synth.pack_courses(courses)
+    dpk = [torch.from_numpy(x).to(dev) for x in packed]
+    course_of = rng.integers(0, len(courses), n).astype(np.int32)
+    lens = np.diff(packed[5])
+    local = rng.integers(0, lens[course_of]).astype(np.int32)
+    gidx = packed[5][course_of] + local
+    st = np.stack([packed[0][gidx] + rng.uniform(-1, 1, n), packed[1][gidx] + rng.uniform(-1, 1, n),
+                   packed[2][gidx], rng.uniform(0, 5, n)]).astype(np.float32)
+    dst, dof = torch.from_numpy(st).to(dev), torch.from_numpy(course_of).to(dev)
+    ti0 = torch.from_numpy(np.maximum(local - 3, 0).astype(np.int32)).to(dev)
+    dti = ti0.clone()
+    xr = torch.empty((4 * T, n), dtype=torch.float32, device=dev)
+    stt = torch.empty(n, dtype=torch.int32, device=dev)
+
+    def many():
+        dti.copy_(ti0)
+        eng.calc_ref_trajectory_many(dst, (dpk[0], dpk[1], dpk[2], dpk[4], dpk[5]), dof, 1.0, dti, xr, T, status=stt)
+    d1 = [torch.from_numpy(x).to(dev) for x in base["demo"]]
+    st1 = st.copy()
+    st1[:2] -= packed[0][gidx] - base["demo"][0][local], packed[1][gidx] - base["demo"][1][local]
+    dst1 = torch.from_numpy(np.ascontiguousarray(st1)).to(dev)
+
+    def single():
+        dti.copy_(ti0)
+        eng.calc_ref_trajectory(dst1, d1[0], d1[1], d1[2], d1[4], 1.0, dti, xr, T)
+    copy_ms = event_ms(lambda: dti.copy_(ti0), a.reps)
+    ms_many, ms_single = event_ms(many, a.reps) - copy_ms, event_ms(single, a.reps) - copy_ms
+    cell = dict(kernel="mpc_lookup", T=T, n=n, n_courses=len(courses), ms=ms_many, calls_per_s=n / (ms_many * 1e-3),
+                ms_single_course=ms_single, single_course_calls_per_s=n / (ms_single * 1e-3))
+    res["mpc_lookup"] = cell
+    print(json.dumps(cell), flush=True)
 
 
 def main():
@@ -133,6 +273,7 @@ def main():
                                         (r["iters"], "iters"), (r["status"], "status")))))
                     res["cells"].append(cell)
                     print(json.dumps(cell), flush=True)
+    many_courses(a, eng, res, dev, courses)
     eng.close()
     path = os.path.join(a.out, "lqr_track_bench.json")
     with open(path, "w") as f:
