@@ -23,6 +23,7 @@ CRB_DWA_MAX_OBSTACLES = 256
 CRB_DWA_MAX_SPEED_SAMPLES = 64
 CRB_DWA_MAX_YAWRATE_SAMPLES = 512
 CRB_DWA_MAX_STEPS = 1000
+CRB_DWA_OK, CRB_DWA_BAD_OBSTACLES = 0, 1
 CRB_MPTG_MAX_ITER = 1000
 CRB_MPTG_MAX_STEPS = 16384
 CRB_MPTG_CONVERGED = 0
@@ -54,6 +55,7 @@ CRB_RRT_MAX_ITER = 16384
 CRB_RRT_FOUND = 0
 CRB_RRT_MAX_ITER_REACHED = 1
 CRB_RRT_BAD_INPUT = 2
+CRB_RRT_BAD_OBSTACLES = 3
 
 c_f32p = C.POINTER(C.c_float)
 c_i32p = C.POINTER(C.c_int32)
@@ -178,6 +180,9 @@ PROTOTYPES = {
     "crb_dwa_rollout_points": (C.c_int, [C.POINTER(DwaParams), C.POINTER(C.c_int)]),
     "crb_dwa_control_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_int, C.POINTER(DwaParams), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "crb_dwa_control_many_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p,
+                                               C.POINTER(DwaParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "crb_dwa_motion_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float]),
     "crb_mptg_default_params": (None, [C.POINTER(MptgParams)]),
     "crb_mptg_optimize_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -203,6 +208,10 @@ PROTOTYPES = {
     "crb_rrt_plan_batched": (C.c_int, [C.c_void_p, C.POINTER(RrtParams), C.c_void_p, C.c_int32, C.c_int64, C.c_void_p,
                                        C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "crb_rrt_plan_many_batched": (C.c_int, [C.c_void_p, C.POINTER(RrtParams), C.c_void_p, C.c_int64, C.c_void_p,
+                                            C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,
+                                            C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]),
     "crb_lqr_track_default_params": (None, [C.POINTER(LqrTrackParams), C.c_int]),
     "crb_lqr_steering_control_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,

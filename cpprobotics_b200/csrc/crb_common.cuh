@@ -162,6 +162,25 @@ static inline cudaError_t crb_launch_pdl(void (*kernel)(KArgs...), unsigned grid
 
 static inline int crb_grid_for(int64_t n, int block) { return (int)((n + block - 1) / block); }
 
+// The obstacle list of agent i in an obstacle store (crb.h): rows [b, e) of ob, checked before any row is read.
+// ob_of NULL means one list, [0, n_rows), for every agent (a shared-list entry point, whose n_rows the host checked).
+// Otherwise ob_of[i] must lie in [0, n_sets) and 0 <= ob_off[s] <= ob_off[s + 1] <= n_rows with at most cap rows;
+// false for a reference that fails (b = e = 0 then).  Empty lists are valid.
+__device__ __forceinline__ bool crb_obstacle_list(int64_t i, const int64_t* __restrict__ ob_off, int32_t n_sets,
+                                                  const int32_t* __restrict__ ob_of, int64_t n_rows, int64_t cap,
+                                                  int64_t& b, int64_t& e) {
+  b = 0;
+  e = ob_of ? 0 : n_rows;
+  if (!ob_of) return true;
+  const int32_t s = ob_of[i];
+  if (s < 0 || s >= n_sets) return false;
+  const int64_t lo = ob_off[s], hi = ob_off[s + 1];
+  if (lo < 0 || lo > hi || hi > n_rows || hi - lo > cap) return false;
+  b = lo;
+  e = hi;
+  return true;
+}
+
 // Streaming (evict-first) global accesses for data that is touched exactly once per launch.
 __device__ __forceinline__ float ld_stream(const float* p) { return __ldcs(p); }
 __device__ __forceinline__ void st_stream(float* p, float v) { __stcs(p, v); }

@@ -1,5 +1,5 @@
-// crb_rrt.cu — RRT::planning (include/rrt.h:75-159) for many seeded start / goal queries on one obstacle list, for
-// sm_90a.
+// crb_rrt.cu — RRT::planning (include/rrt.h:75-159) for many seeded start / goal queries, on one obstacle list or on
+// an obstacle list per query (crb.h's obstacle store), for sm_90a.
 //
 // Bit-exact with the reference built for x86-64 with GCC 13 / libstdc++ and glibc 2.39, after goal_gen.seed(seed):
 //   - goal_gen, a std::mt19937: libstdc++'s seeding, twist and tempering.  Both distributions draw from it (area_gen
@@ -17,7 +17,9 @@
 // keeps the first minimum), the obstacle test (lane-strided, then a vote) and the generator's twist (20 steps of 32
 // words, in the order that keeps every read of the sequential twist).  The draws, atan2f and sincosf are computed by
 // every lane alike, so control flow stays uniform.  Warps are persistent: one warp per block, each takes its next query
-// from an atomic counter, because query lengths differ by 2x and more.
+// from an atomic counter, because query lengths differ by 2x and more.  Both entry points run the same kernel: a
+// query's obstacles are rows [b, e) of the store (every query on [0, n_ob) for the shared list), read lane-strided
+// from global memory through its own base pointer, and checked finite once per query.
 //
 // Shared memory per warp (dynamic, sized from max_iter): the generator's 624 words, then node coordinates (float2) and
 // parent indices (int16) for max_iter + 1 nodes.  Parents stay in shared memory rather than only in the optional global
@@ -35,7 +37,10 @@ struct RrtArgs {
   float rand_min, rand_max, e;
   int32_t gsr, max_iter;
   const float* ob;
-  int32_t n_ob;
+  int64_t n_rows;
+  const int64_t* ob_off;  // NULL: every query on rows [0, n_rows)
+  int32_t n_sets;
+  const int32_t* ob_of;
   int64_t n;
   const float* se;
   const uint32_t* seed;
@@ -109,7 +114,9 @@ __device__ __forceinline__ double sq2(float dx, float dy) {
 
 }  // namespace
 
-__global__ void __launch_bounds__(32) crb_rrt_plan_kernel(const RrtArgs a) {
+// Launched with 32 threads per block.  The query's obstacle base and count, held in registers through the loop, would
+// take ptxas from 58 to 64 registers; the cap keeps 58 with no spill.
+__global__ void __maxnreg__(58) crb_rrt_plan_kernel(const RrtArgs a) {
   extern __shared__ __align__(16) uint32_t smem[];
   uint32_t* mt = smem;
   float2* node = (float2*)(smem + kMtN);
@@ -117,16 +124,20 @@ __global__ void __launch_bounds__(32) crb_rrt_plan_kernel(const RrtArgs a) {
   const int lane = threadIdx.x;
   const int64_t n = a.n;
   const float e = a.e;
-  // every obstacle value finite, or every query is BAD_INPUT
-  bool ob_ok = true;
-  for (int j = lane; j < 3 * a.n_ob; j += 32) ob_ok &= isfinite(__ldg(a.ob + j));
-  ob_ok = __all_sync(kFull, ob_ok);
   for (;;) {
     unsigned long long qq = 0;
     if (lane == 0) qq = atomicAdd(a.counter, 1ull);
     const int64_t q = (int64_t)__shfl_sync(kFull, qq, 0);
     if (q >= n) return;
     const float sx = a.se[q], sy = a.se[n + q], gx = a.se[2 * n + q], gy = a.se[3 * n + q];
+    // the query's obstacles, then every value of them finite, or the query is BAD_INPUT
+    int64_t ob0, ob1;
+    const bool ref_ok = crb_obstacle_list(q, a.ob_off, a.n_sets, a.ob_of, a.n_rows, INT32_MAX / 3, ob0, ob1);
+    const float* ob = a.ob + 3 * ob0;
+    const int32_t n_ob = (int32_t)(ob1 - ob0);
+    bool ob_ok = true;
+    for (int j = lane; j < 3 * n_ob; j += 32) ob_ok &= isfinite(__ldg(ob + j));
+    ob_ok = __all_sync(kFull, ob_ok);
     // goal_gen.seed(s): every lane runs the recurrence, lane k % 32 stores word k
     {
       uint32_t v = a.seed[q];
@@ -139,7 +150,9 @@ __global__ void __launch_bounds__(32) crb_rrt_plan_kernel(const RrtArgs a) {
     }
     int p = kMtN;
     int32_t st = CRB_RRT_MAX_ITER_REACHED, nn = 0, it = 0;
-    if (!(ob_ok && isfinite(sx) && isfinite(sy) && isfinite(gx) && isfinite(gy))) {
+    if (!ref_ok) {
+      st = CRB_RRT_BAD_OBSTACLES;
+    } else if (!(ob_ok && isfinite(sx) && isfinite(sy) && isfinite(gx) && isfinite(gy))) {
       st = CRB_RRT_BAD_INPUT;
     } else {
       if (lane == 0) {
@@ -187,8 +200,8 @@ __global__ void __launch_bounds__(32) crb_rrt_plan_kernel(const RrtArgs a) {
         const float px = __fadd_rn(nb.x, __fmul_rn(e, cs)), py = __fadd_rn(nb.y, __fmul_rn(e, sn));
         // CollisionCheck: the new point only
         bool hit = false;
-        for (int j = lane; j < a.n_ob; j += 32) {
-          const float ox = __ldg(a.ob + 3 * j), oy = __ldg(a.ob + 3 * j + 1), r = __ldg(a.ob + 3 * j + 2);
+        for (int j = lane; j < n_ob; j += 32) {
+          const float ox = __ldg(ob + 3 * j), oy = __ldg(ob + 3 * j + 1), r = __ldg(ob + 3 * j + 2);
           hit |= __dsqrt_rn(sq2(__fsub_rn(ox, px), __fsub_rn(oy, py))) <= (double)r;
         }
         if (__any_sync(kFull, hit)) continue;
@@ -251,25 +264,33 @@ void crb_rrt_default_params(crb_rrt_params* p) {
   p->max_iter = 500;
 }
 
-int crb_rrt_plan_batched(crb_ctx* ctx, const crb_rrt_params* prm, const float* ob, int32_t n_ob, int64_t n,
-                         const float* se, const uint32_t* seed, int32_t max_pts, float* path, int32_t* path_len,
-                         int32_t max_nodes, float* tree, int32_t* parent, int32_t* n_nodes, int32_t* n_iter,
-                         int32_t* status) {
+}  // extern "C"
+
+// The argument checks both entry points share (everything but the obstacles).
+static int rrt_check_args(crb_ctx* ctx, const crb_rrt_params* prm, int64_t n, const float* se, const uint32_t* seed,
+                          int32_t max_pts, int32_t max_nodes) {
   CRB_REQUIRE(ctx != nullptr && prm != nullptr, "ctx or prm is NULL");
   CRB_REQUIRE(isfinite(prm->rand_min) && isfinite(prm->rand_max) && prm->rand_min <= prm->rand_max,
               "rand_min and rand_max must be finite with rand_min <= rand_max");
   CRB_REQUIRE(isfinite(prm->expand_dis), "expand_dis must be finite");
   CRB_REQUIRE(prm->max_iter >= 1 && prm->max_iter <= CRB_RRT_MAX_ITER, "max_iter must be in [1, CRB_RRT_MAX_ITER]");
-  CRB_REQUIRE(n_ob >= 0 && n_ob <= INT32_MAX / 3, "n_ob out of range");
   CRB_REQUIRE(n >= 0 && n <= INT64_MAX / 4, "n out of range");
   CRB_REQUIRE(max_pts >= 0 && max_nodes >= 0, "max_pts and max_nodes must be >= 0");
   CRB_REQUIRE(n <= INT64_MAX / 2 / ((max_pts > max_nodes ? max_pts : max_nodes) + 1), "n * max_pts out of range");
-  CRB_REQUIRE(n == 0 || (se && seed && (n_ob == 0 || ob)), "se, seed or ob is NULL");
+  CRB_REQUIRE(n == 0 || (se && seed), "se or seed is NULL");
+  return CRB_OK;
+}
+
+// No device, no computation (no CPU fallback); then the launch, n > 0.
+static int rrt_launch(crb_ctx* ctx, const char* fn, const crb_rrt_params* prm, const float* ob, int64_t n_rows,
+                      const int64_t* ob_off, int32_t n_sets, const int32_t* ob_of, int64_t n, const float* se,
+                      const uint32_t* seed, int32_t max_pts, float* path, int32_t* path_len, int32_t max_nodes,
+                      float* tree, int32_t* parent, int32_t* n_nodes, int32_t* n_iter, int32_t* status) {
   int count = 0;
   const cudaError_t ce = cudaGetDeviceCount(&count);
   if (ce != cudaSuccess || count == 0) {
     cudaGetLastError();
-    crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", __func__);
+    crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", fn);
     return CRB_ERR_NO_DEVICE;
   }
   if (n == 0) return CRB_OK;
@@ -287,7 +308,10 @@ int crb_rrt_plan_batched(crb_ctx* ctx, const crb_rrt_params* prm, const float* o
   a.gsr = prm->goal_sample_rate;
   a.max_iter = prm->max_iter;
   a.ob = ob;
-  a.n_ob = n_ob;
+  a.n_rows = n_rows;
+  a.ob_off = ob_off;
+  a.n_sets = n_sets;
+  a.ob_of = ob_of;
   a.n = n;
   a.se = se;
   a.seed = seed;
@@ -306,6 +330,32 @@ int crb_rrt_plan_batched(crb_ctx* ctx, const crb_rrt_params* prm, const float* o
   CRB_CUDA(cudaGetLastError());
   ctx->launches++;
   return CRB_OK;
+}
+
+extern "C" {
+
+int crb_rrt_plan_batched(crb_ctx* ctx, const crb_rrt_params* prm, const float* ob, int32_t n_ob, int64_t n,
+                         const float* se, const uint32_t* seed, int32_t max_pts, float* path, int32_t* path_len,
+                         int32_t max_nodes, float* tree, int32_t* parent, int32_t* n_nodes, int32_t* n_iter,
+                         int32_t* status) {
+  int rc = rrt_check_args(ctx, prm, n, se, seed, max_pts, max_nodes);
+  if (rc != CRB_OK) return rc;
+  CRB_REQUIRE(n_ob >= 0 && n_ob <= INT32_MAX / 3, "n_ob out of range");
+  CRB_REQUIRE(n == 0 || n_ob == 0 || ob, "ob is NULL");
+  return rrt_launch(ctx, __func__, prm, ob, n_ob, nullptr, 1, nullptr, n, se, seed, max_pts, path, path_len, max_nodes,
+                    tree, parent, n_nodes, n_iter, status);
+}
+
+int crb_rrt_plan_many_batched(crb_ctx* ctx, const crb_rrt_params* prm, const float* ob, int64_t n_rows,
+                              const int64_t* ob_off, int32_t n_sets, const int32_t* ob_of, int64_t n, const float* se,
+                              const uint32_t* seed, int32_t max_pts, float* path, int32_t* path_len, int32_t max_nodes,
+                              float* tree, int32_t* parent, int32_t* n_nodes, int32_t* n_iter, int32_t* status) {
+  int rc = rrt_check_args(ctx, prm, n, se, seed, max_pts, max_nodes);
+  if (rc != CRB_OK) return rc;
+  CRB_REQUIRE(n_sets >= 1 && n_rows >= 0, "n_sets must be >= 1 and n_rows >= 0");
+  CRB_REQUIRE(n == 0 || (ob_off && ob_of && (ob || n_rows == 0)), "ob, ob_off or ob_of is NULL");
+  return rrt_launch(ctx, __func__, prm, ob, n_rows, ob_off, n_sets, ob_of, n, se, seed, max_pts, path, path_len,
+                    max_nodes, tree, parent, n_nodes, n_iter, status);
 }
 
 }  // extern "C"

@@ -10,6 +10,7 @@ Method names follow the reference functions they replace:
   Engine.calc_ref_trajectory <- calc_ref_trajectory()   src/model_predictive_control.cpp:130-170
   Engine.calc_ref_trajectory_many <- the same, each agent on its own course (synth.pack_courses)
   Engine.dwa_control         <- dwa_control()           src/dynamic_window_approach.cpp:148-155
+  Engine.dwa_control_many    <- the same, each robot among its own obstacles (synth.pack_obstacles)
   Engine.dwa_motion          <- motion()                src/dynamic_window_approach.cpp:43-50
   Engine.mptg_optimize       <- TrajectoryOptimizer::optimizer_traj()  include/trajectory_optimizer.h:53-128
   Engine.mptg_generate_trajectory <- MotionModel::generate_trajectory() include/motion_model.h:110-131
@@ -21,6 +22,7 @@ Method names follow the reference functions they replace:
   Engine.grid_obstacle_map   <- calc_obstacle_map()                              src/a_star.cpp:48-78
   Engine.grid_plan           <- a_star_planning() / dijkstra_star_planning()     src/a_star.cpp:110-244, src/dijkstra.cpp
   Engine.rrt_plan            <- RRT::planning()                                  include/rrt.h:75-159
+  Engine.rrt_plan_many       <- the same, each query among its own obstacles (synth.pack_obstacles)
   Engine.lqr_steering_control <- lqr_steering_control() (+ calc_nearest_index)   src/lqr_steer_control.cpp:98-133,
                                                                                  src/lqr_speed_steer_control.cpp:108-151
   Engine.lqr_steering_control_many <- the same, each vehicle on its own course (synth.pack_courses)
@@ -478,6 +480,38 @@ class Engine:
             _ptr(cost, np.float32, device=True, name="cost"), _ptr(best, np.int32, device=True, name="best"),
             _ptr(traj, np.float32, device=True, name="traj")), "crb_dwa_control_batched")
 
+    def dwa_control_many(self, x, u, goal, obstacles, ob_of, params: Optional[DwaParams] = None, cost=None, best=None,
+                         traj=None, status=None):
+        """dwa_control() for n robots, each among its own obstacles.  obstacles (ob, ob_off): the lists' rows ob
+        [n_rows, 2] float32 back to back and ob_off [n_sets + 1] int64 (synth.pack_obstacles); ob_of [n] int32, the list
+        of each robot.  Everything else as dwa_control; status [n] int32 (CRB_DWA_*) is allocated when not given.
+        Returns status.  CUDA tensors; only enqueues."""
+        n = int(x.shape[-1])
+        _shape(x, 5, n, "x"); _shape(u, 2, n, "u"); _shape(goal, 2, n, "goal"); _shape(ob_of, 1, n, "ob_of")
+        ob, off = obstacles
+        if ob.dim() != 2 or int(ob.shape[1]) != 2:
+            raise ValueError(f"ob: expected shape (n_rows, 2), got {tuple(ob.shape)}")
+        if off.dim() != 1:
+            raise ValueError(f"ob_off: expected shape (n_sets + 1,), got {tuple(off.shape)}")
+        prm = params if params is not None else dwa_default_params()
+        if cost is not None:
+            _shape(cost, 1, n, "cost")
+        if best is not None:
+            _shape(best, 1, n, "best")
+        if traj is not None:
+            _shape(traj, 5 * self.dwa_rollout_points(prm), n, "traj")
+        status = status if status is not None else torch.empty(n, dtype=torch.int32, device=x.device)
+        _shape(status, 1, n, "status")
+        check(self.lib.crb_dwa_control_many_batched(
+            self.ctx, n, _ptr(x, np.float32, device=True, name="x"), _ptr(u, np.float32, device=True, name="u"),
+            _ptr(goal, np.float32, device=True, name="goal"), _ptr(ob, np.float32, device=True, name="ob"),
+            int(ob.shape[0]), _ptr(off, np.int64, device=True, name="ob_off"), int(off.shape[0]) - 1,
+            _ptr(ob_of, np.int32, device=True, name="ob_of"), C.byref(prm),
+            _ptr(cost, np.float32, device=True, name="cost"), _ptr(best, np.int32, device=True, name="best"),
+            _ptr(traj, np.float32, device=True, name="traj"), _ptr(status, np.int32, device=True, name="status")),
+            "crb_dwa_control_many_batched")
+        return status
+
     def dwa_rollout_points(self, params: Optional[DwaParams] = None) -> int:
         """Points per rollout (steps + 1): 32 for the reference's Config."""
         k = C.c_int(0)
@@ -742,6 +776,55 @@ class Engine:
             _ptr(parent, np.int32, device=True, name="parent"), _ptr(n_nodes, np.int32, device=True, name="n_nodes"),
             _ptr(n_iter, np.int32, device=True, name="n_iter"), _ptr(status, np.int32, device=True, name="status")),
             "crb_rrt_plan_batched")
+        return dict(path=path, path_len=path_len, tree=tree, parent=parent, n_nodes=n_nodes, n_iter=n_iter,
+                    status=status)
+
+    def rrt_plan_many(self, obstacles, ob_of, se, seed, params: Optional[RrtParams] = None, max_pts: int = 0,
+                      max_nodes: int = 0, path=None, path_len=None, tree=None, parent=None, n_nodes=None, n_iter=None,
+                      status=None):
+        """RRT::planning() for n seeded queries, each among its own obstacles.  obstacles (ob, ob_off): the lists' rows
+        ob [n_rows, 3] float32 (x, y, r) back to back and ob_off [n_sets + 1] int64 (synth.pack_obstacles); ob_of [n]
+        int32, the list of each query.  Everything else, and the returned dict, as rrt_plan; status may be
+        CRB_RRT_BAD_OBSTACLES."""
+        n = int(se.shape[-1])
+        _shape(se, 4, n, "se")
+        _shape(seed, 1, n, "seed")
+        _shape(ob_of, 1, n, "ob_of")
+        ob, off = obstacles
+        if ob.dim() != 2 or int(ob.shape[1]) != 3:
+            raise ValueError(f"ob: expected shape (n_rows, 3), got {tuple(ob.shape)}")
+        if off.dim() != 1:
+            raise ValueError(f"ob_off: expected shape (n_sets + 1,), got {tuple(off.shape)}")
+        if seed.dtype not in (torch.int32, torch.uint32):
+            raise TypeError(f"seed: expected int32 or uint32, got {seed.dtype}")
+        if not seed.is_cuda or not seed.is_contiguous():
+            raise ValueError("seed: expected a contiguous CUDA tensor")
+        prm = params if params is not None else rrt_default_params()
+        dev = se.device
+        full = lambda rows, v, dt: torch.full((rows, n), v, dtype=dt, device=dev)  # noqa: E731
+        if path is None and max_pts > 0:
+            path = full(2 * max_pts, float("nan"), torch.float32)
+        if tree is None and max_nodes > 0:
+            tree = full(2 * max_nodes, float("nan"), torch.float32)
+        if parent is None and max_nodes > 0:
+            parent = full(max_nodes, -1, torch.int32)
+        for a, rows, name in ((path, 2 * max_pts, "path"), (tree, 2 * max_nodes, "tree"), (parent, max_nodes, "parent")):
+            if a is not None:
+                _shape(a, rows, n, name)
+        i32 = lambda a: a if a is not None else torch.empty(n, dtype=torch.int32, device=dev)  # noqa: E731
+        path_len, n_nodes, n_iter, status = i32(path_len), i32(n_nodes), i32(n_iter), i32(status)
+        for a, name in ((path_len, "path_len"), (n_nodes, "n_nodes"), (n_iter, "n_iter"), (status, "status")):
+            _shape(a, 1, n, name)
+        check(self.lib.crb_rrt_plan_many_batched(
+            self.ctx, C.byref(prm), _ptr(ob, np.float32, device=True, name="ob"), int(ob.shape[0]),
+            _ptr(off, np.int64, device=True, name="ob_off"), int(off.shape[0]) - 1,
+            _ptr(ob_of, np.int32, device=True, name="ob_of"), n, _ptr(se, np.float32, device=True, name="se"),
+            seed.data_ptr(), int(max_pts), _ptr(path, np.float32, device=True, name="path"),
+            _ptr(path_len, np.int32, device=True, name="path_len"), int(max_nodes),
+            _ptr(tree, np.float32, device=True, name="tree"), _ptr(parent, np.int32, device=True, name="parent"),
+            _ptr(n_nodes, np.int32, device=True, name="n_nodes"), _ptr(n_iter, np.int32, device=True, name="n_iter"),
+            _ptr(status, np.int32, device=True, name="status")),
+            "crb_rrt_plan_many_batched")
         return dict(path=path, path_len=path_len, tree=tree, parent=parent, n_nodes=n_nodes, n_iter=n_iter,
                     status=status)
 

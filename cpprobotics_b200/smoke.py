@@ -255,5 +255,51 @@ def run() -> None:
         assert wt == th[i] and same_nan(xh[:, i], wx.reshape(-1)), "many-course MPC lookup is not the checker"
     print("smoke MANY  257 vehicles on 8 courses, LQR control (4 and 5 states) and the MPC lookup: bit-identical to "
           "the checker")
+    # an obstacle list per robot: 257 DWA robots and 65 RRT queries in random order over 8 lists each (empty, 1-row
+    # and 256-row lists among the DWA ones), every output as the checker run list by list
+    dls = synth.dwa_fleet_obstacles(8, seed=0x5A3)
+    dob, doff = synth.pack_obstacles(dls, 2)
+    dof = np.random.default_rng(0x5A4).integers(0, 8, 257).astype(np.int32)
+    xw, uw, gw = synth.dwa_inputs(257, seed=0x5A5)
+    uwd = torch.from_numpy(uw).to(dev)
+    cw = torch.empty(257, dtype=torch.float32, device=dev)
+    bw = torch.empty(257, dtype=torch.int32, device=dev)
+    tw = torch.empty((5 * n_pts, 257), dtype=torch.float32, device=dev)
+    sw = eng.dwa_control_many(torch.from_numpy(xw).to(dev), uwd, torch.from_numpy(gw).to(dev),
+                              (torch.from_numpy(dob).to(dev), torch.from_numpy(doff).to(dev)),
+                              torch.from_numpy(dof).to(dev), cost=cw, best=bw, traj=tw)
+    torch.cuda.synchronize()
+    ok = bool((sw == 0).all().item())
+    for s in range(8):
+        sel = np.nonzero(dof == s)[0]
+        rw = OD.dwa_control(xw[:, sel], uw[:, sel], gw[:, sel], dls[s])
+        sel_t = torch.from_numpy(sel)
+        ok = ok and all(same_nan(g[..., sel_t], rw[k]) for g, k in ((uwd.cpu(), "u"), (cw.cpu(), "cost"),
+                                                                    (bw.cpu(), "best"), (tw.cpu(), "traj")))
+    assert ok, "many-list DWA GPU result is not bit-identical to the checker"
+    rls = synth.rrt_fleet_obstacles(8, seed=0x5A6, lo=rd["rand_min"], hi=rd["rand_max"])
+    rob_, roff = synth.pack_obstacles(rls, 3)
+    rof = np.random.default_rng(0x5A7).integers(0, 8, 65).astype(np.int32)
+    rse = np.zeros((4, 65), np.float32)
+    rseed = np.zeros(65, np.uint32)
+    for s in range(8):
+        sel = np.nonzero(rof == s)[0]
+        rse[:, sel], rseed[sel] = synth.rrt_inputs(sel.size, rls[s], rd["rand_min"], rd["rand_max"], seed=s)
+    rr = eng.rrt_plan_many((torch.from_numpy(rob_).to(dev), torch.from_numpy(roff).to(dev)),
+                           torch.from_numpy(rof).to(dev), torch.from_numpy(rse).to(dev),
+                           torch.from_numpy(rseed.view(np.int32)).to(dev), rp, max_pts=64, max_nodes=512)
+    torch.cuda.synchronize()
+    ok = True
+    for s in range(8):
+        sel = np.nonzero(rof == s)[0]
+        ro = OR.plan(dict(rand_min=rp.rand_min, rand_max=rp.rand_max, expand_dis=rp.expand_dis,
+                          goal_sample_rate=rp.goal_sample_rate, max_iter=rp.max_iter), rls[s], rse[:, sel], rseed[sel],
+                     max_pts=64, max_nodes=512)
+        sel_t = torch.from_numpy(sel)
+        ok = ok and all(same_nan(rr[k].cpu()[..., sel_t], ro[k]) for k in ("path", "path_len", "tree", "parent",
+                                                                          "n_nodes", "n_iter", "status"))
+    assert ok, "many-list RRT GPU result is not bit-identical to the checker"
+    print("smoke OBST  257 DWA robots and 65 RRT queries, each among its own obstacles (8 lists each): bit-identical "
+          "to the checker")
     print(f"smoke ok: {eng.launches} kernel launches through libcrb.so")
     eng.close()

@@ -641,3 +641,98 @@ def fleet_courses(n_courses: int, seed: int = 0xF1EE7):
             ct * x - st * y + tx, st * x + ct * y + ty, np.asarray(b[2][s0:s0 + ln], np.float64) + th,
             b[3][s0:s0 + ln], b[4][s0:s0 + ln])))
     return out
+
+
+# ---- an obstacle list per robot: crb_dwa_control_many_batched, crb_rrt_plan_many_batched --------------------------
+def pack_obstacles(lists, k: int):
+    """A list of obstacle lists ([m_s, k] rows each, m_s >= 0) -> (ob, ob_off): every list's rows back to back in list
+    order (float32 [n_rows, k]) and ob_off (int64 [n_sets + 1]), list s being rows [ob_off[s], ob_off[s + 1])."""
+    rows = [np.asarray(o, np.float32).reshape(-1, k) for o in lists]
+    off = np.zeros(len(rows) + 1, np.int64)
+    off[1:] = np.cumsum([len(r) for r in rows])
+    ob = np.concatenate(rows) if rows else np.zeros((0, k), np.float32)
+    return np.ascontiguousarray(ob, np.float32).reshape(-1, k), off
+
+
+def dwa_fleet_obstacles(n_sets: int, seed: int = 0x0B57):
+    """n_sets varied DWA obstacle lists ([m, 2] float32 rows (ox, oy)): list s is empty when s % 16 == 0, one row when
+    s % 16 == 1, CRB_DWA_MAX_OBSTACLES rows when s % 16 == 2, and otherwise 2 to 64 rows.  Each list lies in its own
+    arena: a square of half-width 3 to 30 m around a centre up to 5 m from the demo's (5, 5), so that robots drawn by
+    dwa_inputs see near, sparse and dense obstacles.  Deterministic for a seed."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for s in range(n_sets):
+        m = {0: 0, 1: 1, 2: 256}.get(s % 16, int(rng.integers(2, 65)))
+        h = float(rng.uniform(3.0, 30.0))
+        cx, cy = 5.0 + rng.uniform(-5.0, 5.0, 2)
+        out.append(np.ascontiguousarray(np.stack([rng.uniform(cx - h, cx + h, m), rng.uniform(cy - h, cy + h, m)],
+                                                 axis=1).astype(np.float32).reshape(m, 2)))
+    return out
+
+
+def rrt_fleet_obstacles(n_sets: int, seed: int = 0x5CA7, lo: float = -2.0, hi: float = 15.0, max_k: int = 64):
+    """n_sets scattered RRT maps ([m, 3] float32 rows (x, y, r)) over one planning area [lo, hi)^2: map s has 0 to max_k
+    circles (rrt_scatter_obstacles, radii 0.3 to 1.2) from a seed of its own; every 16th map (s % 16 == 0) is empty.
+    Deterministic for a seed."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for s in range(n_sets):
+        m = 0 if s % 16 == 0 else int(rng.integers(0, max_k + 1))
+        out.append(rrt_scatter_obstacles(m, lo, hi, seed=int(rng.integers(1 << 31))))
+    return out
+
+
+def dwa_neighbour_obstacles(x, static_ob, radius: float, cap: int = 256, chunk: int = 16384):
+    """The obstacle lists of a fleet that avoids itself: robot i's list is the static obstacles static_ob [m, 2], then
+    the positions (x[0], x[1]) of the other robots within `radius` of it (squared distance in float64 <= radius^2),
+    nearest first (ties by robot index), the whole list cut at `cap` rows.  x [5, n] (or [2+, n]) float32.  Returns
+    (ob, ob_off) as pack_obstacles, list i being robot i's (so ob_of = arange(n)).  Built in numpy on a hash grid of
+    radius-sized cells, `chunk` robots at a time: for tests and benchmarks."""
+    px, py = np.asarray(x[0], np.float32), np.asarray(x[1], np.float32)
+    n = px.size
+    st = np.asarray(static_ob, np.float32).reshape(-1, 2)[:cap]
+    room = cap - len(st)
+    pos = np.stack([px, py], axis=1)
+    gx = np.floor(px.astype(np.float64) / radius).astype(np.int64)
+    gy = np.floor(py.astype(np.float64) / radius).astype(np.int64)
+    gx -= gx.min() - 1
+    gy -= gy.min() - 1
+    span = int(gy.max()) + 2
+    key = gx * span + gy
+    order = np.argsort(key, kind="stable")
+    skey = key[order]
+    counts = np.zeros(n, np.int64)
+    nbr = []
+    r2 = float(radius) * float(radius)
+    for c0 in range(0, n, chunk):
+        ii = np.arange(c0, min(n, c0 + chunk))
+        pi, pj = [], []
+        for dx in (-1, 0, 1):
+            for dy in (-1, 0, 1):
+                t = key[ii] + dx * span + dy
+                lo_, hi_ = np.searchsorted(skey, t, "left"), np.searchsorted(skey, t, "right")
+                cnt = hi_ - lo_
+                rep = np.repeat(np.arange(ii.size), cnt)
+                start = np.repeat(lo_ - np.concatenate([[0], np.cumsum(cnt)[:-1]]), cnt)
+                pi.append(ii[rep])
+                pj.append(order[start + np.arange(rep.size)])
+        i, j = np.concatenate(pi), np.concatenate(pj)
+        d2 = (px[j].astype(np.float64) - px[i]) ** 2 + (py[j].astype(np.float64) - py[i]) ** 2
+        keep = (i != j) & (d2 <= r2)
+        i, j, d2 = i[keep], j[keep], d2[keep]
+        o = np.lexsort((j, d2, i))
+        i, j = i[o], j[o]
+        first = np.searchsorted(i, ii, "left")
+        rank = np.arange(i.size) - np.repeat(first, np.bincount(i - c0, minlength=ii.size))
+        take = rank < room
+        counts[ii] = np.minimum(np.bincount(i - c0, minlength=ii.size), max(room, 0))
+        nbr.append(j[take])
+    nbr = np.concatenate(nbr) if nbr else np.zeros(0, np.int64)
+    off = np.zeros(n + 1, np.int64)
+    off[1:] = np.cumsum(counts + len(st))
+    ob = np.empty((int(off[-1]), 2), np.float32)
+    row = np.arange(int(off[-1])) - np.repeat(off[:-1], counts + len(st))
+    is_st = row < len(st)
+    ob[is_st] = st[row[is_st]]
+    ob[~is_st] = pos[nbr]
+    return ob, off

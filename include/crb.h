@@ -21,6 +21,8 @@
  *                                          src/lqr_speed_steer_control.cpp:85-106
  *   crb_dwa_control_batched             <- dwa_control()         src/dynamic_window_approach.cpp:148-155
  *                                         (calc_dynamic_window :52-60, calc_final_input :115-145 and the costs)
+ *   crb_dwa_control_many_batched        <- the same, each robot among its own obstacles (the reference takes ob
+ *                                          per call)
  *   crb_dwa_motion_batched              <- motion()              src/dynamic_window_approach.cpp:43-50
  *   crb_mptg_optimize_batched           <- TrajectoryOptimizer::optimizer_traj()  include/trajectory_optimizer.h:53-200
  *                                         (MotionModel::generate_last_state, quadratic_interpolation,
@@ -37,6 +39,8 @@
  *                                          :31-45), dijkstra_star_planning()  src/dijkstra.cpp
  *   crb_rrt_plan_batched                <- RRT::planning()       include/rrt.h:75-159 (GetNearestNode :161-174,
  *                                          CollisionCheck :176-181)
+ *   crb_rrt_plan_many_batched           <- the same, each query among its own obstacles (the reference's RRT takes
+ *                                          ob_list per planner, :72)
  *   crb_lqr_steering_control_batched    <- lqr_steering_control() src/lqr_steer_control.cpp:98-133 (4 states),
  *                                          src/lqr_speed_steer_control.cpp:108-151 (5 states), with
  *                                          calc_nearest_index() :55-73 / :65-83 and solve_DARE() + dlqr() inside
@@ -402,6 +406,34 @@ int crb_dwa_rollout_points(const crb_dwa_params* p, int* n_pts);
 int crb_dwa_control_batched(crb_ctx* ctx, int64_t n, const float* x, float* u, const float* goal,
                             const float* ob, int n_ob, const crb_dwa_params* prm, float* cost,
                             int32_t* best, float* traj);
+
+/* Obstacle store of crb_dwa_control_many_batched and crb_rrt_plan_many_batched: every obstacle list's rows back to
+ * back, so that each robot or query plans among its own obstacles.
+ *   ob [n_rows][k]  the rows (k = 2: ox, oy for DWA; k = 3: x, y, r for RRT); n_rows is int64_t, ob may be NULL when
+ *                   n_rows = 0
+ *   ob_off [n_sets + 1] int64_t: list s is rows [ob_off[s], ob_off[s + 1])
+ *   ob_of [n] int32_t: the list of each robot or query; lists may be shared, and robots need not be sorted by list
+ * Empty lists are valid and mean no obstacles.  The offsets are device data: each robot's reference is checked on the
+ * device before any row is read (0 <= s < n_sets, 0 <= ob_off[s] <= ob_off[s + 1] <= n_rows, at most the entry point's
+ * per-list cap of rows); one that fails gets its entry point's BAD_OBSTACLES status, and nothing outside the arrays is
+ * read.  CRB_ERR_INVALID_ARG before any device work unless n_sets >= 1, n_rows >= 0 and, for n > 0, ob_off and ob_of
+ * are given and ob is given unless n_rows = 0. */
+
+/* Per-robot status of crb_dwa_control_many_batched. */
+#define CRB_DWA_OK 0
+#define CRB_DWA_BAD_OBSTACLES 1 /* ob_of[i] does not name a list of at most CRB_DWA_MAX_OBSTACLES rows inside
+                                   [0, n_rows): u, cost and traj are NaN and best is -1 */
+
+/* crb_dwa_control_batched with an obstacle list per robot (the obstacle store above, k = 2, at most
+ * CRB_DWA_MAX_OBSTACLES rows per list).  Each robot's u, cost, best and traj are bitwise those of
+ * crb_dwa_control_batched run with its own list.  status [n] int32 CRB_DWA_* is optional (NULL = not written).
+ * CRB_ERR_INVALID_ARG before any device work as crb_dwa_control_batched and for the store's host checks.  One warp
+ * per robot, each staging its robot's list in shared memory.  DEVICE pointers; only enqueues (graph-capturable).
+ * Replaces: dwa_control(x, u, config, goal, ob) :148-155, which takes its obstacles per call. */
+int crb_dwa_control_many_batched(crb_ctx* ctx, int64_t n, const float* x, float* u, const float* goal,
+                                 const float* ob, int64_t n_rows, const int64_t* ob_off, int32_t n_sets,
+                                 const int32_t* ob_of, const crb_dwa_params* prm, float* cost, int32_t* best,
+                                 float* traj, int32_t* status);
 /* x [5][n] in/out, u [2][n] (DEVICE; NULL allowed when n = 0).  dt finite and > 0.
  * Replaces: motion(x, u, dt) :43-50, the plant step of main() :194. */
 int crb_dwa_motion_batched(crb_ctx* ctx, int64_t n, float* x, const float* u, float dt);
@@ -646,6 +678,8 @@ void crb_rrt_default_params(crb_rrt_params* p);
 #define CRB_RRT_MAX_ITER_REACHED 1 /* max_iter passes without reaching the goal (the reference keeps looping) */
 #define CRB_RRT_BAD_INPUT 2        /* a non-finite start, goal or obstacle value, or a nearest-node search with no winner
                                       (every distance NaN or >= FLT_MAX: the reference reads node_list[-1]) */
+#define CRB_RRT_BAD_OBSTACLES 3    /* crb_rrt_plan_many_batched: ob_of[q] does not name a list of at most INT32_MAX / 3
+                                      rows inside [0, n_rows); n_nodes, n_iter and path_len are 0 */
 
 /* RRT::planning for n queries.
  *   prm: shared by the batch (host pointer)
@@ -671,6 +705,16 @@ int crb_rrt_plan_batched(crb_ctx* ctx, const crb_rrt_params* prm, const float* o
                          const float* se, const uint32_t* seed, int32_t max_pts, float* path, int32_t* path_len,
                          int32_t max_nodes, float* tree, int32_t* parent, int32_t* n_nodes, int32_t* n_iter,
                          int32_t* status);
+/* crb_rrt_plan_batched with an obstacle list per query (the obstacle store described above
+ * crb_dwa_control_many_batched, k = 3, at most INT32_MAX / 3 rows per list).  Each query's outputs are bitwise those of
+ * crb_rrt_plan_batched run with its own list and the same seed; a non-finite value in a list makes BAD_INPUT of the
+ * queries on that list only.  Every other argument, the launch and its graph-capture rule are as there.
+ * CRB_ERR_INVALID_ARG before any device work as crb_rrt_plan_batched and for the store's host checks.
+ * Replaces: RRT(start, end, ob_list, ...).planning(), whose constructor takes the obstacles per planner (:72). */
+int crb_rrt_plan_many_batched(crb_ctx* ctx, const crb_rrt_params* prm, const float* ob, int64_t n_rows,
+                              const int64_t* ob_off, int32_t n_sets, const int32_t* ob_of, int64_t n, const float* se,
+                              const uint32_t* seed, int32_t max_pts, float* path, int32_t* path_len, int32_t max_nodes,
+                              float* tree, int32_t* parent, int32_t* n_nodes, int32_t* n_iter, int32_t* status);
 
 /* ---- LQR path tracking (src/lqr_steer_control.cpp, src/lqr_speed_steer_control.cpp) ------------------------------- */
 /* The per-tick functions of the two LQR programs for a fleet on one course; the caller keeps the loop

@@ -382,6 +382,64 @@ inline std::vector<std::array<float, 5>> dwa_control(std::array<float, 5> x, std
   return traj;
 }
 
+// dwa_control for a fleet, each robot among its own obstacles: robot i is dwa_control(x[i], u[i], config, goal[i],
+// ob[i]) (u[i] set, its rollout returned in element i, empty when no sample is admissible), all in one launch of
+// crb_dwa_control_many_batched.  Each ob[i] must have at most CRB_DWA_MAX_OBSTACLES rows.
+template <class Config>
+inline std::vector<std::vector<std::array<float, 5>>> dwa_control(
+    const std::vector<std::array<float, 5>>& x, std::vector<std::array<float, 2>>& u, Config config,
+    const std::vector<std::array<float, 2>>& goal, const std::vector<std::vector<std::array<float, 2>>>& ob) {
+  const size_t n = x.size();
+  if (u.size() != n || goal.size() != n || ob.size() != n)
+    throw std::runtime_error("dwa_control: x, u, goal and ob differ in length");
+  std::vector<std::vector<std::array<float, 5>>> out(n);
+  if (n == 0) return out;
+  crb_ctx* ctx = crb::Session::get();
+  const crb_dwa_params prm = crb::dwa_params_of(config);
+  int n_pts = 0;
+  crb::check(crb_dwa_rollout_points(&prm, &n_pts), "crb_dwa_rollout_points");
+  // host: ob_off [n + 1] int64 | ob_of [n] int32 | x [5][n] | u [2][n] | goal [2][n] | ob [n_rows][2]
+  std::vector<int64_t> off(n + 1, 0);
+  for (size_t i = 0; i < n; ++i) off[i + 1] = off[i] + (int64_t)ob[i].size();
+  const size_t n_rows = (size_t)off[n];
+  std::vector<float> h(2 * (n + 1) + n + 9 * n + 2 * n_rows);
+  std::memcpy(h.data(), off.data(), off.size() * sizeof(int64_t));
+  float* hx = h.data() + 3 * n + 2;
+  for (size_t i = 0; i < n; ++i) {
+    const int32_t s = (int32_t)i;
+    std::memcpy(h.data() + 2 * (n + 1) + i, &s, 4);
+    for (int f = 0; f < 5; ++f) hx[f * n + i] = x[i][f];
+    for (int f = 0; f < 2; ++f) hx[(5 + f) * n + i] = u[i][f];
+    for (int f = 0; f < 2; ++f) hx[(7 + f) * n + i] = goal[i][f];
+    for (size_t k = 0; k < ob[i].size(); ++k) {
+      hx[9 * n + 2 * (off[i] + k)] = ob[i][k][0];
+      hx[9 * n + 2 * (off[i] + k) + 1] = ob[i][k][1];
+    }
+  }
+  // device: the host block | best [n] | traj [5 n_pts][n]; the arena comes from cudaMalloc, so ob_off is aligned
+  float* d = crb::Session::scratch(h.size() + n + 5 * (size_t)n_pts * n);
+  float *dx = d + 3 * n + 2, *dbest = d + h.size(), *dtraj = dbest + n;
+  crb::check(crb_memcpy_h2d(ctx, d, h.data(), h.size() * sizeof(float)), "h2d");
+  crb::check(crb_dwa_control_many_batched(ctx, (int64_t)n, dx, dx + 5 * n, dx + 7 * n, dx + 9 * n, (int64_t)n_rows,
+                                          (const int64_t*)d, (int32_t)n, (const int32_t*)(d + 2 * (n + 1)), &prm,
+                                          nullptr, (int32_t*)dbest, dtraj, nullptr),
+             "crb_dwa_control_many_batched");
+  std::vector<float> hu(2 * n), tr(5 * (size_t)n_pts * n);
+  std::vector<int32_t> best(n);
+  crb::check(crb_memcpy_d2h(ctx, hu.data(), dx + 5 * n, hu.size() * sizeof(float)), "d2h");
+  crb::check(crb_memcpy_d2h(ctx, best.data(), dbest, n * sizeof(int32_t)), "d2h");
+  crb::check(crb_memcpy_d2h(ctx, tr.data(), dtraj, tr.size() * sizeof(float)), "d2h");
+  for (size_t i = 0; i < n; ++i) {
+    u[i][0] = hu[i];
+    u[i][1] = hu[n + i];
+    if (best[i] < 0) continue;
+    out[i].resize((size_t)n_pts);
+    for (int k = 0; k < n_pts; ++k)
+      for (int j = 0; j < 5; ++j) out[i][(size_t)k][(size_t)j] = tr[(size_t)(5 * k + j) * n + i];
+  }
+  return out;
+}
+
 // motion :43-50 (the plant step of main() :194)
 inline std::array<float, 5> motion(std::array<float, 5> x, std::array<float, 2> u, float dt) {
   crb_ctx* ctx = crb::Session::get();
@@ -766,7 +824,8 @@ inline std::vector<std::vector<std::vector<float>>> dijkstra_star_planning(std::
 // reference's after goal_gen.seed(s).  The reference loops until it finds a path and ignores max_iter; here max_iter
 // is raised to CRB_RRT_MAX_ITER and a query that is not FOUND within it (crb.h's CRB_RRT_* statuses) throws.  The
 // batched overload plans every (starts[i], ends[i]) with goal_gen.seed(seeds[i]) on this RRT's obstacles in one
-// launch.  The RRT object owns the nodes it returns (the reference leaks them).
+// launch; the overload with ob_lists plans query i among ob_lists[i] instead (as an RRT constructed with that list),
+// all in one launch of crb_rrt_plan_many_batched.  The RRT object owns the nodes it returns (the reference leaks them).
 namespace cpprobotics {
 class Node {
  public:
@@ -799,6 +858,21 @@ class RRT {
 
   std::vector<std::vector<Node*> > planning(const std::vector<Node*>& starts, const std::vector<Node*>& ends,
                                             const std::vector<uint32_t>& seeds) {
+    return plan(starts, ends, seeds, nullptr);
+  }
+
+  std::vector<std::vector<Node*> > planning(const std::vector<Node*>& starts, const std::vector<Node*>& ends,
+                                            const std::vector<uint32_t>& seeds,
+                                            const std::vector<std::vector<std::vector<float> > >& ob_lists) {
+    if (ob_lists.size() != starts.size()) throw std::runtime_error("RRT: starts and ob_lists differ in length");
+    return plan(starts, ends, seeds, &ob_lists);
+  }
+
+ protected:
+  // lists NULL: every query on ob_list (crb_rrt_plan_batched); else query i on (*lists)[i] (crb_rrt_plan_many_batched)
+  std::vector<std::vector<Node*> > plan(const std::vector<Node*>& starts, const std::vector<Node*>& ends,
+                                        const std::vector<uint32_t>& seeds,
+                                        const std::vector<std::vector<std::vector<float> > >* lists) {
     const size_t n = starts.size();
     if (ends.size() != n || seeds.size() != n) throw std::runtime_error("RRT: starts, ends, seeds differ in length");
     std::vector<std::vector<Node*> > out(n);
@@ -810,11 +884,30 @@ class RRT {
     prm.expand_dis = expand_dis;
     prm.goal_sample_rate = goal_sample_rate;
     prm.max_iter = CRB_RRT_MAX_ITER;
-    const size_t no = ob_list.size();
-    std::vector<float> h(3 * no + 5 * n);  // ob [no][3] | se [4][n] | seed [n]
-    for (size_t j = 0; j < no; ++j) {
-      if (ob_list[j].size() < 3) throw std::runtime_error("RRT: an obstacle needs {x, y, r}");
-      for (int c = 0; c < 3; ++c) h[3 * j + c] = ob_list[j][c];
+    // the rows: ob_list, or every query's list back to back with ob_off [n + 1] (int64) and ob_of [n] = i after them
+    std::vector<const std::vector<std::vector<float> >*> src(1, &ob_list);
+    if (lists) {
+      src.clear();
+      for (size_t i = 0; i < n; ++i) src.push_back(&(*lists)[i]);
+    }
+    std::vector<int64_t> off(1, 0);
+    for (size_t i = 0; i < src.size(); ++i) off.push_back(off.back() + (int64_t)src[i]->size());
+    const size_t no = (size_t)off.back();
+    const size_t store = lists ? 2 * (n + 1) + n : 0;
+    std::vector<float> h(3 * no + 5 * n + store);  // ob [no][3] | se [4][n] | seed [n] | ob_off, ob_of (per query)
+    for (size_t i = 0; i < src.size(); ++i)
+      for (size_t j = 0; j < src[i]->size(); ++j) {
+        const std::vector<float>& o = (*src[i])[j];
+        if (o.size() < 3) throw std::runtime_error("RRT: an obstacle needs {x, y, r}");
+        for (int c = 0; c < 3; ++c) h[3 * (off[i] + j) + c] = o[c];
+      }
+    if (lists) {
+      float* tail = h.data() + 3 * no + 5 * n;
+      std::memcpy(tail, off.data(), off.size() * sizeof(int64_t));
+      for (size_t i = 0; i < n; ++i) {
+        const int32_t s = (int32_t)i;
+        std::memcpy(tail + 2 * (n + 1) + i, &s, 4);
+      }
     }
     for (size_t i = 0; i < n; ++i) {
       h[3 * no + i] = starts[i]->x;
@@ -825,14 +918,26 @@ class RRT {
     }
     int max_pts = 256;
     for (;;) {
-      // ob, se, seed | len, status [2n] | path [2 max_pts n]
-      float* d = crb::Session::scratch(h.size() + 2 * n + 2 * (size_t)max_pts * n);
-      float *dse = d + 3 * no, *dls = dse + 5 * n, *dpath = dls + 2 * n;
-      crb::check(crb_memcpy_h2d(ctx, d, h.data(), h.size() * sizeof(float)), "h2d");
-      crb::check(crb_rrt_plan_batched(ctx, &prm, d, (int32_t)no, (int64_t)n, dse, (const uint32_t*)(dse + 4 * n),
-                                      max_pts, dpath, (int32_t*)dls, 0, nullptr, nullptr, nullptr, nullptr,
-                                      (int32_t*)(dls + n)),
-                 "crb_rrt_plan_batched");
+      // ob [no][3] | ob_off, ob_of | se, seed | len, status [2n] | path [2 max_pts n]; ob_off starts at an even
+      // float index of the (cudaMalloc-aligned) scratch arena, so it is 8-byte aligned
+      const size_t ob_floats = (3 * no + 1) / 2 * 2;
+      float* d = crb::Session::scratch(ob_floats + store + 5 * n + 2 * n + 2 * (size_t)max_pts * n);
+      float *dstore = d + ob_floats, *dse = dstore + store, *dls = dse + 5 * n, *dpath = dls + 2 * n;
+      crb::check(crb_memcpy_h2d(ctx, d, h.data(), 3 * no * sizeof(float)), "h2d");
+      crb::check(crb_memcpy_h2d(ctx, dse, h.data() + 3 * no, 5 * n * sizeof(float)), "h2d");
+      if (lists) {
+        crb::check(crb_memcpy_h2d(ctx, dstore, h.data() + 3 * no + 5 * n, store * sizeof(float)), "h2d");
+        crb::check(crb_rrt_plan_many_batched(ctx, &prm, d, (int64_t)no, (const int64_t*)dstore, (int32_t)n,
+                                             (const int32_t*)(dstore + 2 * (n + 1)), (int64_t)n, dse,
+                                             (const uint32_t*)(dse + 4 * n), max_pts, dpath, (int32_t*)dls, 0,
+                                             nullptr, nullptr, nullptr, nullptr, (int32_t*)(dls + n)),
+                   "crb_rrt_plan_many_batched");
+      } else {
+        crb::check(crb_rrt_plan_batched(ctx, &prm, d, (int32_t)no, (int64_t)n, dse, (const uint32_t*)(dse + 4 * n),
+                                        max_pts, dpath, (int32_t*)dls, 0, nullptr, nullptr, nullptr, nullptr,
+                                        (int32_t*)(dls + n)),
+                   "crb_rrt_plan_batched");
+      }
       std::vector<int32_t> ls(2 * n);
       crb::check(crb_memcpy_d2h(ctx, ls.data(), dls, ls.size() * sizeof(int32_t)), "d2h");
       int longest = 0;
@@ -861,7 +966,6 @@ class RRT {
     }
   }
 
- protected:
   Node* start;
   Node* end;
   const float expand_dis;
