@@ -49,6 +49,8 @@ CRB_GRID_FOUND = 0
 CRB_GRID_NO_PATH = 1
 CRB_GRID_START_OUTSIDE = 2
 CRB_GRID_BAD_POINT = 3
+CRB_GRID_BAD_MAP = 4
+CRB_GRID_MAP_OK, CRB_GRID_MAP_BAD = 0, 1
 CRB_LQR_TRACK_OK, CRB_LQR_TRACK_DARE_MAXITER, CRB_LQR_TRACK_BAD_INDEX, CRB_LQR_TRACK_BAD_COURSE = 0, 1, 2, 3
 CRB_MPC_REF_OK, CRB_MPC_REF_BAD_COURSE = 0, 1
 CRB_RRT_MAX_ITER = 16384
@@ -204,6 +206,13 @@ PROTOTYPES = {
                                         C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p]),
     "crb_grid_plan_slots": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(GridBox), C.c_int64, C.POINTER(C.c_int64)]),
+    "crb_grid_obstacle_map_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64,
+                                             C.c_int64, C.c_void_p, C.c_void_p]),
+    "crb_grid_plan_many_batched": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                             C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
+                                             C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "crb_grid_plan_many_slots": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.POINTER(C.c_int64)]),
     "crb_rrt_default_params": (None, [C.POINTER(RrtParams)]),
     "crb_rrt_plan_batched": (C.c_int, [C.c_void_p, C.POINTER(RrtParams), C.c_void_p, C.c_int32, C.c_int64, C.c_void_p,
                                        C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,

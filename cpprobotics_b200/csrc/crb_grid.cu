@@ -7,6 +7,7 @@
 // the parent's key is greater; pop: the last entry is saved, the hole walks down to a leaf taking the right child
 // unless its key is greater than the left one's, the lone left child of an even-sized heap is taken, and the saved
 // entry sifts back up).  Ties are everywhere on a grid, and which parent a cell keeps is decided by that order.
+// Queries that each plan on their own map: crb_grid_many.cu, on the same device code (crb_grid_common.cuh).
 //
 // Mapping.
 //   crb_grid_map_kernel: one thread per cell; the obstacles are rounded to cells once per block, a tile at a time, in
@@ -19,85 +20,10 @@
 //       g     [cells] float, A*'s path_cost (FLT_MAX = never reached)
 //       state [cells] uint8: bit 7 visited, bit 3 the start, bits 0-2 the move that reached the cell from its parent
 //     and the parent of a cell is cell - offset[move], so no pointer or parent array is kept.
-#include <float.h>
-
-#include "crb_common.cuh"
+#include "crb_grid_common.cuh"
 
 #define GRID_MAP_BLOCK 256
 #define GRID_PLAN_BLOCK 128
-
-namespace {
-
-// get_motion_model :99-108, in its order; the diagonal cost is (float)std::sqrt(2)
-__constant__ int c_mx[8] = {1, 0, -1, 0, -1, -1, 1, 1};
-__constant__ int c_my[8] = {0, 1, 0, -1, -1, 1, -1, 1};
-constexpr float kDiag = 1.41421354f;
-
-__device__ __forceinline__ float grid_nan() { return __int_as_float(0x7fc00000); }
-
-struct Entry {  // one heap element; 8-byte aligned so that an entry moves in one load and one store
-  float key;
-  uint32_t cd;  // cell << 3 | move
-};
-static_assert(sizeof(Entry) == 8, "heap entry is 8 bytes");
-
-// comp(a, b) of the reference's priority_queue: a->key > b->key
-__device__ __forceinline__ void heap_sift_up(Entry* h, int64_t hole, int64_t top, Entry v) {
-  int64_t parent = (hole - 1) / 2;
-  while (hole > top && h[parent].key > v.key) {
-    h[hole] = h[parent];
-    hole = parent;
-    parent = (hole - 1) / 2;
-  }
-  h[hole] = v;
-}
-
-__device__ __forceinline__ void heap_push(Entry* h, int64_t& len, Entry v) {
-  heap_sift_up(h, len, 0, v);
-  ++len;
-}
-
-// pop_heap + pop_back: returns the top, len shrinks by one
-__device__ __forceinline__ Entry heap_pop(Entry* h, int64_t& len) {
-  const Entry top = h[0];
-  --len;
-  if (len > 0) {
-    const Entry v = h[len];
-    int64_t hole = 0, child = 0;
-    while (child < (len - 1) / 2) {
-      child = 2 * (child + 1);
-      if (h[child].key > h[child - 1].key) --child;
-      h[hole] = h[child];
-      hole = child;
-    }
-    if ((len & 1) == 0 && child == (len - 2) / 2) {
-      child = 2 * (child + 1);
-      h[hole] = h[child - 1];
-      hole = child - 1;
-    }
-    heap_sift_up(h, hole, 0, v);
-  }
-  return top;
-}
-
-// (int)std::round(p / reso) with p / reso a float quotient and roundf; false when the result is not a finite value
-// inside the int range (the reference's conversion is undefined there)
-__device__ __forceinline__ bool grid_cell_f(float p, float reso, int& c) {
-  const float r = roundf(__fdiv_rn(p, reso));
-  if (!(r >= -2147483648.0f && r < 2147483648.0f)) return false;
-  c = __float2int_rz(r);
-  return true;
-}
-
-// (int)std::round(o * 1.0 / reso), in double
-__device__ __forceinline__ bool grid_cell_d(float o, float reso, int& c) {
-  const double r = round(__ddiv_rn((double)o, (double)reso));
-  if (!(r >= -2147483648.0 && r < 2147483648.0)) return false;
-  c = __double2int_rz(r);
-  return true;
-}
-
-}  // namespace
 
 __global__ void __launch_bounds__(GRID_MAP_BLOCK)
 crb_grid_map_kernel(int64_t n_obs, const float* __restrict__ ox, const float* __restrict__ oy, float reso, float thr,
@@ -281,7 +207,9 @@ bool grid_box_dims(const crb_grid_box* b, const char* fn, int64_t& W, int64_t& H
 
 bool grid_reso_ok(float reso) { return isfinite(reso) && reso > 0.0f; }
 
-int grid_require_device(const char* fn) {
+}  // namespace
+
+int crb_grid_require_device(const char* fn) {
   int count = 0;
   const cudaError_t e = cudaGetDeviceCount(&count);
   if (e != cudaSuccess || count == 0) {
@@ -291,6 +219,8 @@ int grid_require_device(const char* fn) {
   }
   return CRB_OK;
 }
+
+namespace {
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
@@ -328,8 +258,9 @@ int grid_slots(crb_ctx* ctx, int algo, int64_t cells, int64_t n, int64_t& slots,
 
 }  // namespace
 
-// Grow-only planner workspace of the context (the first 256 bytes hold the query counter).
-static int grid_ws_reserve(crb_ctx* ctx, size_t bytes) {
+// Grow-only planner workspace of the context (the first 256 bytes hold the query counter); crb_grid_many.cu's planner
+// shares it.
+int crb_grid_ws_reserve(crb_ctx* ctx, size_t bytes) {
   if (ctx->grid_ws_cap >= bytes) return CRB_OK;
   if (ctx->grid_ws) {
     CRB_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -381,7 +312,7 @@ int crb_grid_obstacle_map(crb_ctx* ctx, int64_t n_obs, const float* ox, const fl
   int64_t W, H;
   if (!grid_box_dims(box, __func__, W, H)) return CRB_ERR_INVALID_ARG;
   CRB_REQUIRE(map != nullptr && (n_obs == 0 || (ox && oy)), "ox, oy or map is NULL");
-  const int rc = grid_require_device(__func__);
+  const int rc = crb_grid_require_device(__func__);
   if (rc != CRB_OK) return rc;
   CRB_DEVICE_GUARD(ctx);
   const int64_t cells = W * H;
@@ -400,7 +331,7 @@ int crb_grid_plan_slots(crb_ctx* ctx, int algo, const crb_grid_box* box, int64_t
   CRB_REQUIRE(n >= 0, "n must be >= 0");
   int64_t W, H;
   if (!grid_box_dims(box, __func__, W, H)) return CRB_ERR_INVALID_ARG;
-  const int rc = grid_require_device(__func__);
+  const int rc = crb_grid_require_device(__func__);
   if (rc != CRB_OK) return rc;
   CRB_DEVICE_GUARD(ctx);
   size_t sb;
@@ -420,7 +351,7 @@ int crb_grid_plan_batched(crb_ctx* ctx, int algo, const crb_grid_box* box, const
   if (!grid_box_dims(box, __func__, W, H)) return CRB_ERR_INVALID_ARG;
   CRB_REQUIRE(n == 0 || (map && sg), "map or sg is NULL");
   CRB_REQUIRE(n == 0 || max_pts == 0 || path, "path is NULL with max_pts > 0");
-  const int rc = grid_require_device(__func__);
+  const int rc = crb_grid_require_device(__func__);
   if (rc != CRB_OK) return rc;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);
@@ -442,7 +373,7 @@ int crb_grid_plan_batched(crb_ctx* ctx, int algo, const crb_grid_box* box, const
   a.heap_off = offs[0];
   a.g_off = offs[1];
   a.state_off = offs[2];
-  r = grid_ws_reserve(ctx, 256 + (size_t)a.slots * a.slot_bytes);
+  r = crb_grid_ws_reserve(ctx, 256 + (size_t)a.slots * a.slot_bytes);
   if (r != CRB_OK) return r;
   a.counter = (unsigned long long*)ctx->grid_ws;
   a.ws = (char*)ctx->grid_ws + 256;

@@ -21,6 +21,7 @@ Method names follow the reference functions they replace:
   grid_box_of_obstacles      <- a_star_planning() / dijkstra_star_planning() :115-140 (obstacle cells, the box)
   Engine.grid_obstacle_map   <- calc_obstacle_map()                              src/a_star.cpp:48-78
   Engine.grid_plan           <- a_star_planning() / dijkstra_star_planning()     src/a_star.cpp:110-244, src/dijkstra.cpp
+  Engine.grid_obstacle_map_many, Engine.grid_plan_many <- the same, each query on its own map (grid_map_table)
   Engine.rrt_plan            <- RRT::planning()                                  include/rrt.h:75-159
   Engine.rrt_plan_many       <- the same, each query among its own obstacles (synth.pack_obstacles)
   Engine.lqr_steering_control <- lqr_steering_control() (+ calc_nearest_index)   src/lqr_steer_control.cpp:98-133,
@@ -115,6 +116,25 @@ def grid_box_of_obstacles(ox, oy, reso: float) -> GridBox:
     check(load_library().crb_grid_box_of_obstacles(x.size, x.ctypes.data, y.ctypes.data, float(reso), C.byref(b)),
           "crb_grid_box_of_obstacles")
     return b
+
+
+def grid_map_table(boxes, reso):
+    """The map table of grid_obstacle_map_many / grid_plan_many for boxes int [n_maps, 4] (min_x, min_y, max_x, max_y)
+    and reso [n_maps]: (boxes int32 [n_maps, 4], reso float32 [n_maps], map_off int64 [n_maps + 1], max_cells), map m
+    being bytes [map_off[m], map_off[m + 1]) of the store and max_cells the largest W * H.  Host arrays (numpy); a box
+    outside the limits of include/crb.h raises ValueError.  A box per obstacle list comes from grid_box_of_obstacles."""
+    b = np.ascontiguousarray(np.asarray(boxes, np.int64).reshape(-1, 4))
+    r = np.ascontiguousarray(np.asarray(reso, np.float32).reshape(-1))
+    if b.shape[0] < 1 or r.shape != (b.shape[0],):
+        raise ValueError(f"boxes, reso: expected [n_maps, 4] and [n_maps] with n_maps >= 1, got {b.shape}, {r.shape}")
+    W, H = b[:, 2] - b[:, 0], b[:, 3] - b[:, 1]
+    bad = (W < 1) | (H < 1) | (W > _lib.CRB_GRID_MAX_SIDE) | (H > _lib.CRB_GRID_MAX_SIDE) | (
+        W * H > _lib.CRB_GRID_MAX_CELLS)
+    if bad.any():
+        raise ValueError(f"box {int(np.flatnonzero(bad)[0])} is empty or exceeds CRB_GRID_MAX_SIDE / MAX_CELLS")
+    off = np.zeros(b.shape[0] + 1, np.int64)
+    off[1:] = np.cumsum(W * H)
+    return np.ascontiguousarray(b.astype(np.int32)), r, off, int((W * H).max())
 
 
 _libc = None
@@ -727,6 +747,83 @@ class Engine:
             _ptr(path, np.float32, device=True, name="path"), _ptr(path_len, np.int32, device=True, name="path_len"),
             _ptr(cost, np.float32, device=True, name="cost"), _ptr(n_visited, np.int32, device=True, name="n_visited"),
             _ptr(status, np.int32, device=True, name="status")), "crb_grid_plan_batched")
+        return dict(path=path, path_len=path_len, cost=cost, n_visited=n_visited, status=status)
+
+    def grid_obstacle_map_many(self, obstacles, ob_of, rr, table, maps=None, map_status=None):
+        """calc_obstacle_map() for every map of a table in one launch.  obstacles (ob, ob_off): obstacle lists ob
+        [n_rows, 2] float32 rows (ox, oy) back to back and ob_off [n_sets + 1] int64 (synth.pack_obstacles); ob_of
+        [n_maps] int32, the list of each map; rr [n_maps] float32, each map's robot radius; table (boxes int32
+        [n_maps, 4], reso float32 [n_maps], map_off int64 [n_maps + 1], max_cells) from grid_map_table, its arrays on
+        the device.  Returns (maps [n_cells] uint8, map_status [n_maps] int32 CRB_GRID_MAP_*), allocating what is not
+        given (maps zeroed, after one read of map_off[-1]).  CUDA tensors; only enqueues."""
+        boxes, reso, off, max_cells = table
+        n_maps = int(reso.shape[0])
+        ob, ob_off = obstacles
+        if ob.dim() != 2 or int(ob.shape[1]) != 2:
+            raise ValueError(f"ob: expected shape (n_rows, 2), got {tuple(ob.shape)}")
+        if ob_off.dim() != 1:
+            raise ValueError(f"ob_off: expected shape (n_sets + 1,), got {tuple(ob_off.shape)}")
+        self._grid_table_shapes(boxes, reso, off)
+        _shape(ob_of, 1, n_maps, "ob_of"); _shape(rr, 1, n_maps, "rr")
+        if maps is None:
+            maps = torch.zeros(int(off[-1].item()), dtype=torch.uint8, device=reso.device)
+        if map_status is None:
+            map_status = torch.empty(n_maps, dtype=torch.int32, device=reso.device)
+        _shape(map_status, 1, n_maps, "map_status")
+        check(self.lib.crb_grid_obstacle_map_many(
+            self.ctx, _ptr(ob, np.float32, device=True, name="ob"), int(ob.shape[0]),
+            _ptr(ob_off, np.int64, device=True, name="ob_off"), int(ob_off.shape[0]) - 1,
+            _ptr(ob_of, np.int32, device=True, name="ob_of"), _ptr(rr, np.float32, device=True, name="rr"),
+            _ptr(boxes, np.int32, device=True, name="boxes"), _ptr(reso, np.float32, device=True, name="reso"),
+            _ptr(off, np.int64, device=True, name="map_off"), n_maps, int(maps.numel()), int(max_cells),
+            _ptr(maps, np.uint8, device=True, name="maps"), _ptr(map_status, np.int32, device=True, name="map_status")),
+            "crb_grid_obstacle_map_many")
+        return maps, map_status
+
+    @staticmethod
+    def _grid_table_shapes(boxes, reso, off):
+        n_maps = int(reso.shape[0])
+        if tuple(boxes.shape) != (n_maps, 4) or tuple(reso.shape) != (n_maps,) or tuple(off.shape) != (n_maps + 1,):
+            raise ValueError(f"table: expected boxes [n_maps, 4], reso [n_maps], map_off [n_maps + 1], got "
+                             f"{tuple(boxes.shape)}, {tuple(reso.shape)}, {tuple(off.shape)}")
+
+    def grid_plan_many_slots(self, algo: int, max_cells: int, n: int) -> int:
+        """The number of searches grid_plan_many runs at once for n queries on a table with this max_cells."""
+        s = C.c_int64(0)
+        check(self.lib.crb_grid_plan_many_slots(self.ctx, int(algo), int(max_cells), int(n), C.byref(s)),
+              "crb_grid_plan_many_slots")
+        return int(s.value)
+
+    def grid_plan_many(self, algo: int, table, maps, map_of, sg, max_pts: int = 0, path=None, path_len=None,
+                       cost=None, n_visited=None, status=None):
+        """grid_plan with a map per query: query q plans on map map_of[q] (int32 [n]) of the table (grid_map_table's
+        tuple, arrays on the device) and its byte store maps [n_cells] uint8 (grid_obstacle_map_many's).  sg [4, n]
+        float32 in each query's own map's metres.  Returns grid_plan's dict; status may be CRB_GRID_BAD_MAP.  CUDA
+        tensors; only enqueues (the first call at a larger workspace allocates it)."""
+        boxes, reso, off, max_cells = table
+        self._grid_table_shapes(boxes, reso, off)
+        n = int(sg.shape[-1])
+        _shape(sg, 4, n, "sg"); _shape(map_of, 1, n, "map_of")
+        dev = sg.device
+        if path is None and max_pts > 0:
+            path = torch.full((2 * max_pts, n), float("nan"), dtype=torch.float32, device=dev)
+        if path is not None:
+            _shape(path, 2 * max_pts, n, "path")
+        i32 = lambda a: a if a is not None else torch.empty(n, dtype=torch.int32, device=dev)  # noqa: E731
+        path_len, n_visited, status = i32(path_len), i32(n_visited), i32(status)
+        if cost is None:
+            cost = torch.empty(n, dtype=torch.float32, device=dev)
+        for a, name in ((path_len, "path_len"), (cost, "cost"), (n_visited, "n_visited"), (status, "status")):
+            _shape(a, 1, n, name)
+        check(self.lib.crb_grid_plan_many_batched(
+            self.ctx, int(algo), _ptr(boxes, np.int32, device=True, name="boxes"),
+            _ptr(reso, np.float32, device=True, name="reso"), _ptr(off, np.int64, device=True, name="map_off"),
+            int(reso.shape[0]), _ptr(maps, np.uint8, device=True, name="maps"), int(maps.numel()), int(max_cells), n,
+            _ptr(map_of, np.int32, device=True, name="map_of"), _ptr(sg, np.float32, device=True, name="sg"),
+            int(max_pts), _ptr(path, np.float32, device=True, name="path"),
+            _ptr(path_len, np.int32, device=True, name="path_len"), _ptr(cost, np.float32, device=True, name="cost"),
+            _ptr(n_visited, np.int32, device=True, name="n_visited"), _ptr(status, np.int32, device=True, name="status")),
+            "crb_grid_plan_many_batched")
         return dict(path=path, path_len=path_len, cost=cost, n_visited=n_visited, status=status)
 
     # ---- RRT ----------------------------------------------------------------------------------------------------

@@ -301,5 +301,27 @@ def run() -> None:
     assert ok, "many-list RRT GPU result is not bit-identical to the checker"
     print("smoke OBST  257 DWA robots and 65 RRT queries, each among its own obstacles (8 lists each): bit-identical "
           "to the checker")
+    # a map per query: 8 small fleet maps built in one launch, then 129 queries in random order over them per planner,
+    # every map and output as the checker run map by map
+    from oracle import grid_many as OGM  # checker only
+    from .engine import grid_map_table
+    gf = synth.grid_fleet_maps(8, seed=0x5A8)
+    gt = grid_map_table(gf["boxes"], gf["reso"])
+    gob, goff = synth.pack_obstacles(gf["lists"], 2)
+    gdt = tuple(torch.from_numpy(a).to(dev) for a in gt[:3]) + (gt[3],)
+    gmaps, gst = eng.grid_obstacle_map_many((torch.from_numpy(gob).to(dev), torch.from_numpy(goff).to(dev)),
+                                            torch.from_numpy(gf["ob_of"]).to(dev), torch.from_numpy(gf["rr"]).to(dev),
+                                            gdt)
+    gwant, _ = OGM.obstacle_map_many(gob, goff, gf["ob_of"], gf["rr"], *gt[:3], int(gt[2][-1]), gt[3])
+    assert bool((gst == 0).all().item()) and same_nan(gmaps, gwant), "many-map grid build is not the checker"
+    gmof, gmsg = synth.grid_fleet_inputs(129, gt[0], gt[1], gwant, gt[2], seed=0x5A9)
+    for algo in (OG.ASTAR, OG.DIJKSTRA):
+        gr = eng.grid_plan_many(algo, gdt, gmaps, torch.from_numpy(gmof).to(dev), torch.from_numpy(gmsg).to(dev),
+                                max_pts=32)
+        torch.cuda.synchronize()
+        go = OGM.plan_many(algo, *gt[:3], gwant, gt[3], gmof, gmsg, max_pts=32)
+        ok = all(same_nan(gr[k], go[k]) for k in ("path", "path_len", "cost", "n_visited", "status"))
+        assert ok, "many-map grid planner GPU result is not bit-identical to the checker"
+    print("smoke MAPS  8 grid maps in one build, 129 queries over them per planner: bit-identical to the checker")
     print(f"smoke ok: {eng.launches} kernel launches through libcrb.so")
     eng.close()

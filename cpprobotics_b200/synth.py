@@ -736,3 +736,91 @@ def dwa_neighbour_obstacles(x, static_ob, radius: float, cap: int = 256, chunk: 
     ob[is_st] = st[row[is_st]]
     ob[~is_st] = pos[nbr]
     return ob, off
+
+
+# ---- a map per query: crb_grid_obstacle_map_many, crb_grid_plan_many_batched ----------------------------------------
+def _grid_cells(o, reso):
+    """(int)round(o * 1.0 / reso) in double, as the planners round obstacles"""
+    return np.round(np.asarray(o, np.float32).astype(np.float64) * 1.0 / np.float64(np.float32(reso))).astype(np.int64)
+
+
+def grid_fleet_maps(n_maps: int, seed: int = 0x6F1E):
+    """n_maps varied grid maps over shared obstacle lists: dict(lists ([k, 2] float32 rows (ox, oy)), ob_of int32
+    [n_maps], boxes int32 [n_maps, 4], reso float32 [n_maps], rr float32 [n_maps]).  Every list is scattered over a
+    window of up to 60 x 60 cells at a base resolution between 10^-2 and 10^1.7 and offset up to 40 cells from the
+    origin; list s is empty when s % 16 == 0.  About four maps share each list, each at the base resolution or 1.5 or
+    2 times it, with rr 0, 0.5, 1 or 2 times its resolution.  By map index: m % 8 == 1 is a single cell, m % 8 == 2 a
+    rectangular window cut from the list's box, m % 8 == 3 that box grown by 3 cells on each side, otherwise the box of
+    its list's window.  Deterministic for a seed."""
+    rng = np.random.default_rng(seed)
+    n_lists = max(1, (n_maps + 3) // 4)
+    lists, base = [], []
+    for s in range(n_lists):
+        r0 = float(np.float32(10.0 ** rng.uniform(-2.0, 1.69)))
+        W0, H0 = int(rng.integers(2, 61)), int(rng.integers(2, 61))
+        x0, y0 = int(rng.integers(-40, 41)), int(rng.integers(-40, 41))
+        k = 0 if s % 16 == 0 else int(rng.integers(1, max(2, W0 * H0 // 6)))
+        cx, cy = x0 + rng.uniform(0.0, W0, k), y0 + rng.uniform(0.0, H0, k)
+        lists.append(np.ascontiguousarray(np.stack([cx * r0, cy * r0], axis=1).astype(np.float32).reshape(k, 2)))
+        base.append((r0, x0, y0, W0, H0))
+    ob_of = np.zeros(n_maps, np.int32)
+    boxes = np.zeros((n_maps, 4), np.int32)
+    reso = np.zeros(n_maps, np.float32)
+    rr = np.zeros(n_maps, np.float32)
+    for m in range(n_maps):
+        s = int(rng.integers(n_lists)) if m >= n_lists else m
+        r0, x0, y0, W0, H0 = base[s]
+        r = np.float32(r0 * (1.0, 1.0, 1.5, 2.0)[int(rng.integers(4))])
+        bx0, by0 = int(np.floor(x0 * r0 / r)), int(np.floor(y0 * r0 / r))
+        W, H = max(1, int(np.ceil(W0 * r0 / r))), max(1, int(np.ceil(H0 * r0 / r)))
+        kind = m % 8
+        if kind == 1:
+            bx0, by0, W, H = bx0 + int(rng.integers(W)), by0 + int(rng.integers(H)), 1, 1
+        elif kind == 2:
+            w, h = int(rng.integers(1, W + 1)), int(rng.integers(1, H + 1))
+            bx0, by0, W, H = bx0 + int(rng.integers(W - w + 1)), by0 + int(rng.integers(H - h + 1)), w, h
+        elif kind == 3:
+            bx0, by0, W, H = bx0 - 3, by0 - 3, W + 6, H + 6
+        ob_of[m], reso[m] = s, r
+        boxes[m] = (bx0, by0, bx0 + W, by0 + H)
+        rr[m] = np.float32(r * (0.0, 0.5, 1.0, 2.0)[int(rng.integers(4))])
+    return dict(lists=lists, ob_of=ob_of, boxes=boxes, reso=reso, rr=rr)
+
+
+def grid_local_windows(n_robots: int, side: int = 256, win: int = 64, reso: float = 1.0, rr: float = 1.0,
+                       seed: int = 0x10CA):
+    """A fleet in one obstacle field, each robot planning in its own win x win window: the field is
+    grid_scatter_obstacles(side, reso) and every window a box of cells at a seeded offset inside [0, side)^2.  Returns
+    the dict of grid_fleet_maps, with one list that every window shares (ob_of all 0), reso and rr the same for all."""
+    ox, oy = grid_scatter_obstacles(side, reso)
+    rng = np.random.default_rng(seed)
+    x0 = rng.integers(0, side - win + 1, n_robots)
+    y0 = rng.integers(0, side - win + 1, n_robots)
+    boxes = np.ascontiguousarray(np.stack([x0, y0, x0 + win, y0 + win], axis=1).astype(np.int32))
+    return dict(lists=[np.ascontiguousarray(np.stack([ox, oy], axis=1))], ob_of=np.zeros(n_robots, np.int32),
+                boxes=boxes, reso=np.full(n_robots, reso, np.float32), rr=np.full(n_robots, rr, np.float32))
+
+
+def grid_fleet_inputs(n: int, boxes, reso, maps, map_off, seed: int = 0xC0FFEE):
+    """(map_of int32 [n], sg float32 [4, n]) for n queries over the maps of a table (boxes [n_maps, 4], reso, the byte
+    store maps and map_off): every query on a map drawn uniformly, in shuffled order, and the queries of map m
+    grid_inputs(k, boxes[m], map m, reso[m], seed, i0 = (57 + m) % 64), so that each map's first queries are
+    grid_inputs' corner cases.  A map with no free cell takes its queries as if every cell were free.  Deterministic for
+    a seed."""
+    rng = np.random.default_rng(seed)
+    n_maps = len(reso)
+    map_of = rng.integers(0, n_maps, n).astype(np.int32)
+    sg = np.zeros((4, n), np.float32)
+    order = np.argsort(map_of, kind="stable")
+    cuts = np.searchsorted(map_of[order], np.arange(n_maps + 1))
+    for m in range(n_maps):
+        sel = order[cuts[m]:cuts[m + 1]]
+        if sel.size == 0:
+            continue
+        b = boxes[m]
+        W, H = int(b[2]) - int(b[0]), int(b[3]) - int(b[1])
+        mm = np.asarray(maps[int(map_off[m]):int(map_off[m + 1])]).reshape(W, H)
+        if not (mm == 0).any():
+            mm = np.zeros_like(mm)
+        sg[:, sel] = grid_inputs(sel.size, b, mm, float(reso[m]), seed=seed, i0=(57 + m) % 64)
+    return map_of, sg

@@ -617,6 +617,8 @@ int crb_grid_obstacle_map(crb_ctx* ctx, int64_t n_obs, const float* ox, const fl
 #define CRB_GRID_NO_PATH 1       /* the open set emptied first (goal unreachable, blocked or outside the box) */
 #define CRB_GRID_START_OUTSIDE 2 /* the start cell lies outside the box */
 #define CRB_GRID_BAD_POINT 3     /* start or goal is non-finite, or round(p / reso) leaves the int range */
+#define CRB_GRID_BAD_MAP 4       /* crb_grid_plan_many_batched: map_of[q] is outside [0, n_maps) or names an invalid
+                                    table entry (below); takes precedence over BAD_POINT */
 
 /* a_star_planning / dijkstra_star_planning for n queries on one map (the map of crb_grid_obstacle_map, or any
  * uint8 map in its layout, nonzero = blocked).
@@ -645,6 +647,58 @@ int crb_grid_plan_batched(crb_ctx* ctx, int algo, const crb_grid_box* box, const
                           int32_t* n_visited, int32_t* status);
 /* The number of slots (concurrent searches) crb_grid_plan_batched uses for these arguments. */
 int crb_grid_plan_slots(crb_ctx* ctx, int algo, const crb_grid_box* box, int64_t n, int64_t* slots);
+
+/* Map table of crb_grid_obstacle_map_many and crb_grid_plan_many_batched: many maps back to back in one byte store,
+ * each in crb_grid_obstacle_map's layout, so that every robot or query plans on its own map (its own obstacles,
+ * window, resolution or robot radius).
+ *   boxes [n_maps]      crb_grid_box of each map
+ *   reso [n_maps]       float: each map's resolution
+ *   map_off [n_maps + 1] int64_t: map m is bytes [map_off[m], map_off[m + 1]) of maps [n_cells] uint8, cell (x, y) at
+ *                       map_off[m] + (x - min_x) * H + (y - min_y), nonzero = blocked
+ * Host scalars: n_maps >= 1, n_cells >= 0 and max_cells in [1, CRB_GRID_MAX_CELLS], a bound on W * H of every map the
+ * call uses (it sizes the planner's slots, so the host never reads the table).  Entry m is valid when its box is within
+ * the box limits above, W * H <= max_cells, 0 <= map_off[m], map_off[m + 1] - map_off[m] == W * H, map_off[m + 1] <=
+ * n_cells, and reso[m] is finite and > 0.  The table is device data: each entry is checked on the device before
+ * anything it points at is read, and nothing outside a valid entry's bytes is read or written for it.
+ * CRB_ERR_INVALID_ARG before any device work for a scalar out of range or a table pointer that is NULL where the call
+ * needs it. */
+
+/* Status of each map of crb_grid_obstacle_map_many. */
+#define CRB_GRID_MAP_OK 0
+#define CRB_GRID_MAP_BAD 1 /* an invalid table entry, a non-finite rr[m], or an ob_of[m] that does not name a list of
+                              the obstacle store: the map's bytes are left as they were */
+
+/* calc_obstacle_map for every map of a table in one launch.  Map m is built from list ob_of[m] of an obstacle store
+ * (the one described above crb_dwa_control_many_batched, k = 2: rows (ox, oy), no cap on a list's rows) with its own
+ * reso[m] and robot radius rr [n_maps] (float); many maps may share one list.  Every valid map is bitwise
+ * crb_grid_obstacle_map run on its list, box, reso and rr (the threshold is the float quotient rr[m] / reso[m]),
+ * whatever the other entries hold.  map_status [n_maps] int32 CRB_GRID_MAP_* is optional (NULL = not written).
+ * CRB_ERR_INVALID_ARG before any device work for the table's and the store's host checks (n_sets >= 1, n_rows >= 0;
+ * ob may be NULL only when n_rows = 0, maps only when n_cells = 0).  One block per (map, 256-cell tile).  DEVICE
+ * pointers; only enqueues (graph-capturable). */
+int crb_grid_obstacle_map_many(crb_ctx* ctx, const float* ob, int64_t n_rows, const int64_t* ob_off, int32_t n_sets,
+                               const int32_t* ob_of, const float* rr, const crb_grid_box* boxes, const float* reso,
+                               const int64_t* map_off, int32_t n_maps, int64_t n_cells, int64_t max_cells,
+                               uint8_t* maps, int32_t* map_status);
+
+/* crb_grid_plan_batched with a map per query: query q plans on map map_of[q] [n] (int32) of the table above, its start
+ * and goal rounded with that map's reso and its path points cell * reso[map_of[q]].  Each query's outputs are bitwise
+ * those of crb_grid_plan_batched run on its own map (path truncation at max_pts and the untouched tail included).  A
+ * query whose map_of[q] is outside [0, n_maps) or names an invalid entry gets CRB_GRID_BAD_MAP, path_len 0, cost NaN
+ * and n_visited 0; other queries are unaffected.  The slots are sized for max_cells
+ * (crb_grid_plan_many_slots) in the context's workspace that crb_grid_plan_batched uses, with the same graph-capture
+ * rules: the first call at a larger max_cells * slots grows it and cannot be captured, later calls can, and a graph
+ * captured before a call that grew it must not be replayed after.  CRB_ERR_INVALID_ARG before any device work for an
+ * unknown algo, the table's host checks, n or n * max_pts out of range as in crb_grid_plan_batched, a NULL boxes,
+ * reso, map_off, map_of or sg with n > 0, a NULL maps with n > 0 and n_cells > 0, or a NULL path with max_pts > 0.
+ * DEVICE pointers.  Replaces: a_star_planning(sx, sy, gx, gy, ox, oy, reso, rr) / dijkstra_star_planning(...), which
+ * take their map's inputs on every call. */
+int crb_grid_plan_many_batched(crb_ctx* ctx, int algo, const crb_grid_box* boxes, const float* reso,
+                               const int64_t* map_off, int32_t n_maps, const uint8_t* maps, int64_t n_cells,
+                               int64_t max_cells, int64_t n, const int32_t* map_of, const float* sg, int max_pts,
+                               float* path, int32_t* path_len, float* cost, int32_t* n_visited, int32_t* status);
+/* The number of slots crb_grid_plan_many_batched uses for n queries with this max_cells. */
+int crb_grid_plan_many_slots(crb_ctx* ctx, int algo, int64_t max_cells, int64_t n, int64_t* slots);
 
 /* ---- RRT (include/rrt.h) ----------------------------------------------------------------------------------------- */
 /* Many seeded start / goal queries on one obstacle list.  RRT::planning :75-159 loops until a new node lies within

@@ -815,6 +815,114 @@ inline std::vector<std::vector<std::vector<float>>> dijkstra_star_planning(std::
                                                                            float rr) {
   return detail::grid_plan(CRB_GRID_DIJKSTRA, sx, sy, gx, gy, ox_, oy_, reso, rr);
 }
+
+// The same with a map per query: query i is exactly the reference call (sx[i], sy[i], gx[i], gy[i], ox_[i], oy_[i],
+// reso[i], rr[i]).  Every query's map is built in one crb_grid_obstacle_map_many launch and every query planned in one
+// crb_grid_plan_many_batched launch.  Throws as the overloads above do.
+namespace detail {
+inline std::vector<std::vector<std::vector<float>>> grid_plan_many(
+    int algo, const std::vector<float>& sx, const std::vector<float>& sy, const std::vector<float>& gx,
+    const std::vector<float>& gy, const std::vector<std::vector<float>>& ox, const std::vector<std::vector<float>>& oy,
+    const std::vector<float>& reso, const std::vector<float>& rr) {
+  crb_ctx* ctx = crb::Session::get();
+  const size_t n = sx.size();
+  if (sy.size() != n || gx.size() != n || gy.size() != n || ox.size() != n || oy.size() != n || reso.size() != n ||
+      rr.size() != n)
+    throw std::runtime_error("grid planner: the per-query arguments differ in length");
+  std::vector<std::vector<std::vector<float>>> out(n);
+  if (n == 0) return out;
+  // host: map_off [n + 1] | ob_off [n + 1] (int64) | boxes [n][4] | ob_of [n] (int32) | reso | rr | sg [4][n] |
+  // ob [n_rows][2]
+  std::vector<int64_t> moff(n + 1, 0), ooff(n + 1, 0);
+  std::vector<crb_grid_box> boxes(n);
+  int64_t max_cells = 1;
+  for (size_t i = 0; i < n; ++i) {
+    if (ox[i].size() != oy[i].size()) throw std::runtime_error("grid planner: ox and oy differ in length");
+    crb::check(crb_grid_box_of_obstacles((int64_t)ox[i].size(), ox[i].data(), oy[i].data(), reso[i], &boxes[i]),
+               "crb_grid_box_of_obstacles");
+    const int64_t cells = ((int64_t)boxes[i].max_x - boxes[i].min_x) * ((int64_t)boxes[i].max_y - boxes[i].min_y);
+    if (cells > max_cells) max_cells = cells;
+    moff[i + 1] = moff[i] + (cells > 0 ? cells : 0);
+    ooff[i + 1] = ooff[i] + (int64_t)ox[i].size();
+  }
+  const size_t n_rows = (size_t)ooff[n], n_cells = (size_t)moff[n];
+  const size_t o_box = 4 * (n + 1), o_of = o_box + 4 * n, o_reso = o_of + n, o_rr = o_reso + n, o_sg = o_rr + n,
+               o_ob = o_sg + 4 * n;
+  std::vector<float> h(o_ob + 2 * n_rows);
+  std::memcpy(h.data(), moff.data(), moff.size() * sizeof(int64_t));
+  std::memcpy(h.data() + 2 * (n + 1), ooff.data(), ooff.size() * sizeof(int64_t));
+  std::memcpy(h.data() + o_box, boxes.data(), n * sizeof(crb_grid_box));
+  for (size_t i = 0; i < n; ++i) {
+    const int32_t s = (int32_t)i;
+    std::memcpy(h.data() + o_of + i, &s, 4);
+    h[o_reso + i] = reso[i];
+    h[o_rr + i] = rr[i];
+    h[o_sg + i] = sx[i];
+    h[o_sg + n + i] = sy[i];
+    h[o_sg + 2 * n + i] = gx[i];
+    h[o_sg + 3 * n + i] = gy[i];
+    for (size_t k = 0; k < ox[i].size(); ++k) {
+      h[o_ob + 2 * ((size_t)ooff[i] + k)] = ox[i][k];
+      h[o_ob + 2 * ((size_t)ooff[i] + k) + 1] = oy[i][k];
+    }
+  }
+  int max_pts = 256;
+  for (;;) {
+    // device: the host block | len, status [2n] | maps [n_cells bytes] | path [2 max_pts n]
+    const size_t map_f = (n_cells + 3) / 4;
+    float* d = crb::Session::scratch(h.size() + 2 * n + map_f + 2 * (size_t)max_pts * n);
+    float *dls = d + h.size(), *dmap = dls + 2 * n, *dpath = dmap + map_f;
+    const int64_t* dmoff = (const int64_t*)d;
+    const crb_grid_box* dbox = (const crb_grid_box*)(d + o_box);
+    crb::check(crb_memcpy_h2d(ctx, d, h.data(), h.size() * sizeof(float)), "h2d");
+    crb::check(crb_grid_obstacle_map_many(ctx, d + o_ob, (int64_t)n_rows, (const int64_t*)(d + 2 * (n + 1)),
+                                          (int32_t)n, (const int32_t*)(d + o_of), d + o_rr, dbox, d + o_reso, dmoff,
+                                          (int32_t)n, (int64_t)n_cells, max_cells, (uint8_t*)dmap, nullptr),
+               "crb_grid_obstacle_map_many");
+    crb::check(crb_grid_plan_many_batched(ctx, algo, dbox, d + o_reso, dmoff, (int32_t)n, (const uint8_t*)dmap,
+                                          (int64_t)n_cells, max_cells, (int64_t)n, (const int32_t*)(d + o_of),
+                                          d + o_sg, max_pts, dpath, (int32_t*)dls, nullptr, nullptr,
+                                          (int32_t*)(dls + n)),
+               "crb_grid_plan_many_batched");
+    std::vector<int32_t> ls(2 * n);
+    crb::check(crb_memcpy_d2h(ctx, ls.data(), dls, ls.size() * sizeof(int32_t)), "d2h");
+    int longest = 0;
+    for (size_t i = 0; i < n; ++i) {
+      if (ls[n + i] != CRB_GRID_FOUND)
+        throw std::runtime_error("grid planner: no path (status " + std::to_string(ls[n + i]) + ")");
+      if (ls[i] > longest) longest = ls[i];
+    }
+    if (longest > max_pts) {  // again with room for every whole path
+      max_pts = longest;
+      continue;
+    }
+    std::vector<float> p(2 * (size_t)max_pts * n);
+    crb::check(crb_memcpy_d2h(ctx, p.data(), dpath, p.size() * sizeof(float)), "d2h");
+    for (size_t i = 0; i < n; ++i) {
+      std::vector<float> rx, ry;
+      for (int k = 0; k < ls[i]; ++k) {
+        rx.push_back(p[(2 * (size_t)k) * n + i]);
+        ry.push_back(p[(2 * (size_t)k + 1) * n + i]);
+      }
+      out[i] = {rx, ry};
+    }
+    return out;
+  }
+}
+}  // namespace detail
+
+inline std::vector<std::vector<std::vector<float>>> a_star_planning(
+    std::vector<float> sx, std::vector<float> sy, std::vector<float> gx, std::vector<float> gy,
+    std::vector<std::vector<float>> ox_, std::vector<std::vector<float>> oy_, std::vector<float> reso,
+    std::vector<float> rr) {
+  return detail::grid_plan_many(CRB_GRID_ASTAR, sx, sy, gx, gy, ox_, oy_, reso, rr);
+}
+inline std::vector<std::vector<std::vector<float>>> dijkstra_star_planning(
+    std::vector<float> sx, std::vector<float> sy, std::vector<float> gx, std::vector<float> gy,
+    std::vector<std::vector<float>> ox_, std::vector<std::vector<float>> oy_, std::vector<float> reso,
+    std::vector<float> rr) {
+  return detail::grid_plan_many(CRB_GRID_DIJKSTRA, sx, sy, gx, gy, ox_, oy_, reso, rr);
+}
 }  // namespace cpprobotics
 
 // include/rrt.h:21-159.  Node has the reference's members and constructor.  RRT has its constructor (path_resolution is
