@@ -18,6 +18,8 @@ CRB_STATS_LEN = 8
 CRB_COMM_ID_BYTES = 128
 CRB_PF_RESULT_LEN = 24
 CRB_PF_MAX_LANDMARKS = 64
+CRB_PF_FLEET_MAX_NP = 8192
+CRB_PF_FLEET_OK, CRB_PF_FLEET_BAD_OBSERVATIONS = 0, 1
 CRB_MPC_MAX_T = 32
 CRB_DWA_MAX_OBSTACLES = 256
 CRB_DWA_MAX_SPEED_SAMPLES = 64
@@ -155,6 +157,10 @@ PROTOTYPES = {
     "crb_pf_step": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
                               C.c_void_p, C.c_int, C.POINTER(PfParams), C.c_void_p, C.c_uint64, C.c_float,
                               C.c_void_p]),
+    "crb_pf_step_many_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int64, C.c_void_p,
+                                           C.c_int32, C.c_void_p, C.POINTER(PfParams), C.c_void_p, C.c_uint64,
+                                           C.c_float, C.c_void_p, C.c_void_p]),
     "crb_mpc_default_params": (None, [C.POINTER(MpcParams)]),
     "crb_mpc_solve_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.POINTER(MpcParams), C.c_void_p, C.c_void_p,

@@ -37,6 +37,7 @@ struct crb_ctx {
   int mpc_tasks_attr_set;
   int pf_step_attr_set;   // shared-memory carve-out preference of the crb_pf_step kernels (per device)
   int mpc_v0_attr_set;
+  int pf_fleet_attr_set;  // crb_pf_fleet_kernel's dynamic shared-memory limit raised to FLEET_SMEM_MAX
   // NCCL communicator (crb_comm.cu); NULL = single GPU
   void* comm;
   int comm_world, comm_rank;

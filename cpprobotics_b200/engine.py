@@ -364,6 +364,48 @@ class Engine:
             "crb_pf_step")
         return result
 
+    def pf_step_many(self, np_per_robot: int, px, pw, px_next, u, observations, z_of, noise=None,
+                     params: Optional[PfParams] = None, seed: int = 0, uniforms=None, resample_seed: int = 0,
+                     nth: Optional[float] = None, result=None, status=None):
+        """pf_step for a fleet (crb_pf_step_many_batched): n_robots independent filters of np_per_robot particles,
+        robot r in columns [r*np, (r+1)*np) of px [4, n] / pw [n] / px_next [4, n], n = n_robots * np.  u [2, n_robots]
+        holds each robot's control; observations (z, z_off) are the lists' rows z [n_rows, 3] (range, lx, ly) back to
+        back and z_off [n_sets + 1] int64 (synth.pack_obstacles); z_of [n_robots] int32, the list of each robot.
+        nth defaults to np // 2.  Returns the float64 CUDA result tensor [CRB_PF_RESULT_LEN, n_robots]; status
+        [n_robots] int32 (CRB_PF_FLEET_*) is written when given.  Only enqueues."""
+        npr = int(np_per_robot)
+        nr = int(u.shape[-1])
+        n = nr * npr
+        _shape(px, 4, n, "px"); _shape(px_next, 4, n, "px_next"); _shape(pw, 1, n, "pw")
+        _shape(u, 2, nr, "u"); _shape(z_of, 1, nr, "z_of")
+        if noise is not None:
+            _shape(noise, 2, n, "noise")
+        if uniforms is not None:
+            _shape(uniforms, 1, n, "uniforms")
+        z, off = observations
+        if z.dim() != 2 or int(z.shape[1]) != 3:
+            raise ValueError(f"z: expected shape (n_rows, 3), got {tuple(z.shape)}")
+        if off.dim() != 1:
+            raise ValueError(f"z_off: expected shape (n_sets + 1,), got {tuple(off.shape)}")
+        prm = params if params is not None else pf_default_params()
+        if result is None:
+            result = torch.empty((_lib.CRB_PF_RESULT_LEN, nr), dtype=torch.float64, device=px.device)
+        _shape(result, _lib.CRB_PF_RESULT_LEN, nr, "result")
+        if status is not None:
+            _shape(status, 1, nr, "status")
+        check(self.lib.crb_pf_step_many_batched(
+            self.ctx, nr, npr, _ptr(px, np.float32, device=True, name="px"),
+            _ptr(pw, np.float32, device=True, name="pw"), _ptr(px_next, np.float32, device=True, name="px_next"),
+            _ptr(u, np.float32, device=True, name="u"), _ptr(noise, np.float32, device=True, name="noise"),
+            C.c_uint64(int(seed)), _ptr(z, np.float32, device=True, name="z"), int(z.shape[0]),
+            _ptr(off, np.int64, device=True, name="z_off"), int(off.shape[0]) - 1,
+            _ptr(z_of, np.int32, device=True, name="z_of"), C.byref(prm),
+            _ptr(uniforms, np.float32, device=True, name="uniforms"), C.c_uint64(int(resample_seed)),
+            C.c_float(npr // 2 if nth is None else nth), _ptr(result, np.float64, device=True, name="result"),
+            _ptr(status, np.int32, device=True, name="status")),
+            "crb_pf_step_many_batched")
+        return result
+
     # ---- MPC --------------------------------------------------------------------------------------
     def _mpc(self, fn, dev, x0, xref, T, params, u_init, sol, u0, cost, status, iters, hint=None):
         n = int(x0.shape[-1])

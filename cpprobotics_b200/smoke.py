@@ -323,5 +323,26 @@ def run() -> None:
         ok = all(same_nan(gr[k], go[k]) for k in ("path", "path_len", "cost", "n_visited", "status"))
         assert ok, "many-map grid planner GPU result is not bit-identical to the checker"
     print("smoke MAPS  8 grid maps in one build, 129 queries over them per planner: bit-identical to the checker")
+
+    # ---- a particle filter per robot: one fleet step against the checker composed robot by robot ----
+    from oracle import pf_fleet as PFF  # checker only
+    nfr, nfp = 33, 100
+    ff = synth.pf_fleet_inputs(nfr, nfp, seed=0x5F)
+    fx, fw = torch.from_numpy(ff["px"]).to(dev), torch.from_numpy(ff["pw"]).to(dev)
+    fxn = torch.zeros_like(fx)
+    fst = torch.empty(nfr, dtype=torch.int32, device=dev)
+    fres = eng.pf_step_many(nfp, fx, fw, fxn, torch.from_numpy(ff["u"]).to(dev),
+                            (torch.from_numpy(ff["z"]).to(dev), torch.from_numpy(ff["z_off"]).to(dev)),
+                            torch.from_numpy(ff["z_of"]).to(dev), noise=torch.from_numpy(ff["noise"]).to(dev),
+                            uniforms=torch.from_numpy(ff["uniforms"]).to(dev), status=fst)
+    torch.cuda.synchronize()
+    cx, cw, cxn, cres, cst = PFF.step_many(nfp, ff["px"], ff["pw"], ff["u"], ff["z"], ff["z_off"], ff["z_of"],
+                                           ff["noise"], ff["uniforms"])
+    gres = fres.cpu().numpy()
+    assert (fst.cpu().numpy() == cst).all(), "fleet PF status differs from the checker"
+    assert np.abs(fx.cpu().numpy() - cx).max() <= 1e-5, "fleet PF particles differ from the checker"
+    assert np.abs(gres[:4] - cres[:4]).max() <= 1e-4, "fleet PF estimate differs from the checker"
+    print(f"smoke FLEET PF {nfr} robots x {nfp} particles, each with its own u and observations: particles and xEst "
+          f"match the checker, {int(gres[22].sum())} robots resampled")
     print(f"smoke ok: {eng.launches} kernel launches through libcrb.so")
     eng.close()

@@ -824,3 +824,45 @@ def grid_fleet_inputs(n: int, boxes, reso, maps, map_off, seed: int = 0xC0FFEE):
             mm = np.zeros_like(mm)
         sg[:, sel] = grid_inputs(sel.size, b, mm, float(reso[m]), seed=seed, i0=(57 + m) % 64)
     return map_of, sg
+
+
+PF_RFID = ((10.0, 0.0), (10.0, 10.0), (0.0, 15.0), (-5.0, 20.0))   # the demo's tags, src/particle_filter.cpp:192-196
+PF_MAX_RANGE = 20.0                                                  # :20
+
+
+def pf_fleet_inputs(n_robots: int, np_per_robot: int, seed: int = 0xF1EE7, tags=PF_RFID,
+                    max_range: float = PF_MAX_RANGE, spread: float = 10.0):
+    """A fleet of particle filters for crb_pf_step_many_batched: robot r has its own hidden true pose (within `spread`
+    m of the origin), its own particles (a 0.2 m cloud around that pose, random yaw and speed), its own control u
+    (speed 0.5..1.5, yaw rate -0.3..0.3) and its own observation list built as the demo builds z (:257-268): the tags
+    of the shared set `tags` ([k, 2], the demo's four by default) within max_range of the true pose, each as a row
+    (range + 0.04 N(0,1), lx, ly).  Lists are packed with pack_obstacles(lists, 3), one list per robot.
+    Returns dict(px [4,n], pw [n] (= 1/np), u [2,n_robots], z [n_rows,3], z_off [n_robots+1], z_of [n_robots],
+    noise [2,n], uniforms [n] in [1,2), truth [4,n_robots]), float32 / int64 / int32, n = n_robots * np_per_robot."""
+    nr, npr = int(n_robots), int(np_per_robot)
+    n = nr * npr
+    ridx = np.arange(nr, dtype=np.uint64)
+    pidx = np.arange(n, dtype=np.uint64)
+    truth = np.stack([uniform(seed, 70, ridx, -spread, spread), uniform(seed, 71, ridx, -spread, spread),
+                      uniform(seed, 72, ridx, -np.pi, np.pi), uniform(seed, 73, ridx, 0.5, 1.5)])
+    own = np.repeat(np.arange(nr), npr)
+    px = np.empty((4, n), np.float64)
+    px[0] = truth[0, own] + 0.2 * normal(seed, 74, pidx)
+    px[1] = truth[1, own] + 0.2 * normal(seed, 75, pidx)
+    px[2] = uniform(seed, 76, pidx, -np.pi, np.pi)
+    px[3] = uniform(seed, 77, pidx, 0.0, 2.0)
+    u = np.stack([uniform(seed, 78, ridx, 0.5, 1.5), uniform(seed, 79, ridx, -0.3, 0.3)])
+    tg = np.asarray(tags, np.float32).reshape(-1, 2)
+    tx, ty = truth[0].astype(np.float32), truth[1].astype(np.float32)
+    d = np.sqrt((tx[:, None] - tg[None, :, 0]) ** 2 + (ty[:, None] - tg[None, :, 1]) ** 2).astype(np.float32)
+    dn = (d + np.float32(0.04) * normal(seed, 80, np.arange(nr * len(tg), dtype=np.uint64)).reshape(nr, -1)
+          .astype(np.float32)).astype(np.float32)
+    seen = d <= np.float32(max_range)
+    lists = [np.stack([dn[r, seen[r]], tg[seen[r], 0], tg[seen[r], 1]], axis=1) for r in range(nr)]
+    z, z_off = pack_obstacles(lists, 3)
+    f = np.float32
+    return dict(px=np.ascontiguousarray(px.astype(f)), pw=np.full(n, 1.0 / npr, f),
+                u=np.ascontiguousarray(u.astype(f)), z=z, z_off=z_off, z_of=np.arange(nr, dtype=np.int32),
+                noise=np.ascontiguousarray(np.stack([normal(seed, 81, pidx), normal(seed, 82, pidx)]).astype(f)),
+                uniforms=np.ascontiguousarray(uniform(seed, 83, pidx, 1.0, 2.0).astype(f)),
+                truth=np.ascontiguousarray(truth.astype(f)))

@@ -12,6 +12,8 @@
  *   crb_pf_estimate                     <- pf_localization() tail            src/particle_filter.cpp:104-107
  *                                         (calc_covariance :59-71)
  *   crb_pf_resample                     <- resampling() + cumsum()           src/particle_filter.cpp:111-148
+ *   crb_pf_step_many_batched            <- pf_localization() + resampling() per robot, each with its own u and z
+ *                                          src/particle_filter.cpp:73-148, :257-271
  *   crb_mpc_solve_batched[_host]        <- mpc_solve() + FG_EVAL            src/model_predictive_control.cpp:188-346
  *   crb_mpc_plant_update_batched        <- update()                          src/model_predictive_control.cpp:69-81
  *   crb_mpc_calc_ref_trajectory_batched <- calc_ref_trajectory() :130-170 + calc_nearest_index() :107-127
@@ -241,6 +243,44 @@ int crb_pf_resample(crb_ctx* ctx, int64_t n, float* px, float* pw, float* px_tmp
 int crb_pf_step(crb_ctx* ctx, int64_t n, float* px, float* pw, float* px_next, const float* noise,
                 uint64_t seed, const float* landmarks, int n_lm, const crb_pf_params* prm,
                 const float* uniforms, uint64_t resample_seed, float nth, double* result_dev);
+
+/* Per-robot status of crb_pf_step_many_batched. */
+#define CRB_PF_FLEET_OK 0
+#define CRB_PF_FLEET_BAD_OBSERVATIONS 1 /* z_of[r] does not name a list of at most CRB_PF_MAX_LANDMARKS rows inside
+                                           [0, n_rows): the robot's result column is NaN and its px, pw and px_next
+                                           columns are left as they were */
+/* Particles per robot of crb_pf_step_many_batched: the largest power of two whose shared-memory slice (24 bytes per
+ * particle plus 1280) fits the 227 KB of one CTA. */
+#define CRB_PF_FLEET_MAX_NP 8192
+/* crb_pf_step for a fleet: n_robots INDEPENDENT filters of np particles each, one complete iteration of every filter in
+ * ONE launch (one warp per robot).  Robot r owns columns [r*np, (r+1)*np) of the field-major arrays; each robot
+ * normalises, estimates, decides on resampling (Neff < nth, its own) and resamples with its own particles only.
+ *   px [4][n_robots*np], pw [n_robots*np] in/out and px_next [4][n_robots*np] out: as crb_pf_step, per robot
+ *   u [2][n_robots]   each robot's control; prm->u is ignored, every other field of prm is shared by the batch
+ *   z, n_rows, z_off, n_sets, z_of: each robot's observations in the obstacle store described above
+ *                     crb_dwa_control_many_batched, k = 3: rows (range, lx, ly) like the reference's z items
+ *                     (:263-266), at most CRB_PF_MAX_LANDMARKS rows per list; an empty list means no weight update
+ *   noise [2][n_robots*np] or NULL: particle r*np + j then draws Philox4x32-10(seed, r*np + j), the draws
+ *                     crb_pf_predict_weight_batched makes for that particle of the whole array
+ *   uniforms [n_robots*np] in [1, 2) or NULL: Philox(resample_seed, r*np + j); resampleid_j = j/np + U_j/np with
+ *                     the running maximum, the cap at np - 1 and pw = 1/np of crb_pf_step
+ *   result [CRB_PF_RESULT_LEN][n_robots] (f64, field-major): each robot's crb_pf_step result
+ *   status [n_robots] int32 CRB_PF_FLEET_* (optional, NULL = not written)
+ * A robot's px, pw and px_next are bitwise those of crb_pf_predict_weight_batched + crb_pf_step's tail run on that
+ * robot alone with its u in prm and its list as the landmarks, up to the summation order of the weight sum and the
+ * cumulative weights (the reductions run over the robot's particles in a fixed order of their own).  A NaN in one
+ * list or all-zero weights in one robot make only that robot's outputs NaN.  On a context with a communicator the
+ * robots are independent too: there is no collective, each rank steps its own robots as on one GPU.
+ * CRB_ERR_INVALID_ARG before any device work unless 1 <= np <= CRB_PF_FLEET_MAX_NP, n_robots >= 0, prm is given,
+ * the store passes its host checks and, for n_robots > 0, px, pw, px_next, u and result are given and px != px_next.
+ * n_robots = 0 does nothing.  DEVICE pointers; only enqueues (graph-capturable).
+ * Replaces: pf_localization(px, pw, xEst, PEst, z, u) + resampling(px, pw) per robot, src/particle_filter.cpp:73-148,
+ * :270-271. */
+int crb_pf_step_many_batched(crb_ctx* ctx, int64_t n_robots, int32_t np, float* px, float* pw, float* px_next,
+                             const float* u, const float* noise, uint64_t seed, const float* z, int64_t n_rows,
+                             const int64_t* z_off, int32_t n_sets, const int32_t* z_of, const crb_pf_params* prm,
+                             const float* uniforms, uint64_t resample_seed, float nth, double* result,
+                             int32_t* status);
 
 /* ---- MPC -------------------------------------------------------------------------------------- */
 /* Problem constants: src/model_predictive_control.cpp:23-48 (macros), cost weights :202-210 and

@@ -8,6 +8,7 @@
 //   update(state, a, delta)                       src/model_predictive_control.cpp:69-81
 //   calc_ref_trajectory(...)                      src/model_predictive_control.cpp:130-170
 //   resampling(px, pw, gen, uni_d)                src/particle_filter.cpp:120-148
+//   pf_localization_resampling(px, pw, xEst, PEst, z, u, ...)   the demo's tick :270-271 for a fleet, one launch
 //   solve_DARE / dlqr (4x4 and 5x5)               src/lqr_steer_control.cpp:75-96, lqr_speed_steer_control.cpp:85-106
 //   dwa_control(x, u, config, goal, ob), motion(x, u, dt)   src/dynamic_window_approach.cpp:148-155, :43-50
 //   MotionModel, TrajectoryOptimizer::optimizer_traj(...)    include/motion_model.h, include/trajectory_optimizer.h
@@ -289,6 +290,92 @@ inline void resampling(crb::Mat<4, NP>& px, crb::Mat<NP, 1>& pw, std::mt19937 ge
     crb::check(crb_memcpy_d2h(ctx, pw.data(), dpw, NP * sizeof(float)), "d2h");
     for (int ip = 0; ip < NP; ++ip)
       for (int k = 0; k < 4; ++k) px(k, ip) = sx[k * NP + ip];
+  }
+}
+
+// The demo's tick for a fleet: pf_localization(px, pw, xEst, PEst, z, u, Rsim, Q, gen, gaussian_d) followed by
+// resampling(px, pw, gen2, uni_d) (src/particle_filter.cpp:270-271) for every robot r, with its own particles px[r],
+// weights pw[r], observations z[r] and control u[r], in ONE crb_pf_step_many_batched launch.  Each robot's generators
+// are gen[r] and gen2[r], copied like the single-robot overloads take them by value (the caller's are not advanced),
+// and the distributions are copied per robot, so robot r draws exactly what the two single-robot calls would: 2 NP
+// normals from gen[r] (two per particle, :87-88), then NP uniforms from gen2[r] (one per particle, :133).  NTh = NP/2.
+// Each robot's list holds at most CRB_PF_MAX_LANDMARKS rows.
+template <int NP>
+inline void pf_localization_resampling(std::vector<crb::Mat<4, NP>>& px, std::vector<crb::Mat<NP, 1>>& pw,
+                                       std::vector<crb::Vector4f>& xEst, std::vector<crb::Matrix4f>& PEst,
+                                       const std::vector<std::vector<crb::RowVector3f>>& z,
+                                       const std::vector<crb::Vector2f>& u, crb::Matrix2f Rsim, float Q,
+                                       std::vector<std::mt19937> gen, std::normal_distribution<> gaussian_d,
+                                       std::vector<std::mt19937> gen2, std::uniform_real_distribution<> uni_d) {
+  const size_t nr = px.size();
+  if (pw.size() != nr || z.size() != nr || u.size() != nr || gen.size() != nr || gen2.size() != nr)
+    throw std::runtime_error("pf_localization_resampling: px, pw, z, u, gen and gen2 need one entry per robot");
+  xEst.resize(nr);
+  PEst.resize(nr);
+  if (nr == 0) return;
+  crb_ctx* ctx = crb::Session::get();
+  crb_pf_params prm;
+  crb_pf_default_params(&prm);
+  prm.Q = Q;
+  prm.rsim_diag[0] = Rsim(0, 0);
+  prm.rsim_diag[1] = Rsim(1, 1);
+  const size_t n = nr * NP;
+  std::vector<float> sx(4 * n), sw(n), noise(2 * n), un(n), su(2 * nr), rows;
+  std::vector<int64_t> off(nr + 1, 0);
+  std::vector<int32_t> of(nr);
+  for (size_t r = 0; r < nr; ++r) {
+    std::normal_distribution<> gd = gaussian_d;       // pf_localization's by-value arguments
+    std::uniform_real_distribution<> ud = uni_d;      // resampling's
+    for (int ip = 0; ip < NP; ++ip) {
+      const size_t j = r * NP + ip;
+      for (int k = 0; k < 4; ++k) sx[k * n + j] = px[r](k, ip);   // Eigen's 4 x NP (AoS) -> SoA [4][n]
+      sw[j] = pw[r](ip);
+      noise[j] = (float)gd(gen[r]);
+      noise[n + j] = (float)gd(gen[r]);
+    }
+    for (int ip = 0; ip < NP; ++ip) un[r * NP + ip] = (float)ud(gen2[r]);
+    su[r] = u[r](0);
+    su[nr + r] = u[r](1);
+    for (const crb::RowVector3f& zi : z[r])
+      for (int k = 0; k < 3; ++k) rows.push_back(zi(0, k));
+    off[r + 1] = off[r] + (int64_t)z[r].size();
+    of[r] = (int32_t)r;
+  }
+  // device layout (floats): px | px_next | pw | noise | uniforms | u | rows | z_off (int64) | z_of | result (f64)
+  const size_t nrow = rows.size();
+  size_t o_off = 12 * n + 2 * nr + nrow;
+  o_off += o_off & 1;                                   // 8-byte alignment for the int64 offsets
+  const size_t o_of = o_off + 2 * (nr + 1);
+  size_t o_res = o_of + nr;
+  o_res += o_res & 1;
+  float* d = crb::Session::scratch(o_res + 2 * (size_t)CRB_PF_RESULT_LEN * nr);
+  float *dpx = d, *dpxn = d + 4 * n, *dpw = d + 8 * n, *dn = d + 9 * n, *dun = d + 11 * n, *du = d + 12 * n;
+  float* drows = du + 2 * nr;
+  int64_t* doff = (int64_t*)(d + o_off);
+  int32_t* dof = (int32_t*)(d + o_of);
+  double* dres = (double*)(d + o_res);
+  crb::check(crb_memcpy_h2d(ctx, dpx, sx.data(), sx.size() * sizeof(float)), "h2d");
+  crb::check(crb_memcpy_h2d(ctx, dpw, sw.data(), sw.size() * sizeof(float)), "h2d");
+  crb::check(crb_memcpy_h2d(ctx, dn, noise.data(), noise.size() * sizeof(float)), "h2d");
+  crb::check(crb_memcpy_h2d(ctx, dun, un.data(), un.size() * sizeof(float)), "h2d");
+  crb::check(crb_memcpy_h2d(ctx, du, su.data(), su.size() * sizeof(float)), "h2d");
+  if (nrow) crb::check(crb_memcpy_h2d(ctx, drows, rows.data(), nrow * sizeof(float)), "h2d");
+  crb::check(crb_memcpy_h2d(ctx, doff, off.data(), off.size() * sizeof(int64_t)), "h2d");
+  crb::check(crb_memcpy_h2d(ctx, dof, of.data(), of.size() * sizeof(int32_t)), "h2d");
+  crb::check(crb_pf_step_many_batched(ctx, (int64_t)nr, NP, dpx, dpw, dpxn, du, dn, 0, drows, (int64_t)nrow / 3,
+                                      doff, (int32_t)nr, dof, &prm, dun, 0, (float)(NP / 2), dres, nullptr),
+             "crb_pf_step_many_batched");               // :73-148; NTh = NP / 2 is an integer expression (:22)
+  std::vector<double> res((size_t)CRB_PF_RESULT_LEN * nr);
+  crb::check(crb_memcpy_d2h(ctx, sx.data(), dpxn, sx.size() * sizeof(float)), "d2h");   // resampled or a copy
+  crb::check(crb_memcpy_d2h(ctx, sw.data(), dpw, sw.size() * sizeof(float)), "d2h");
+  crb::check(crb_memcpy_d2h(ctx, res.data(), dres, res.size() * sizeof(double)), "d2h");
+  for (size_t r = 0; r < nr; ++r) {
+    for (int ip = 0; ip < NP; ++ip) {
+      for (int k = 0; k < 4; ++k) px[r](k, ip) = sx[k * n + r * NP + ip];
+      pw[r](ip) = sw[r * NP + ip];
+    }
+    for (int k = 0; k < 4; ++k) xEst[r](k) = (float)res[k * nr + r];
+    for (int k = 0; k < 16; ++k) PEst[r].d[k] = (float)res[(4 + k) * nr + r];   // column-major, like Eigen
   }
 }
 
