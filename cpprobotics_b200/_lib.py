@@ -20,6 +20,7 @@ CRB_PF_RESULT_LEN = 24
 CRB_PF_MAX_LANDMARKS = 64
 CRB_PF_FLEET_MAX_NP = 8192
 CRB_PF_FLEET_OK, CRB_PF_FLEET_BAD_OBSERVATIONS = 0, 1
+CRB_EKF_OK, CRB_EKF_BAD_MODEL = 0, 1
 CRB_MPC_MAX_T = 32
 CRB_DWA_MAX_OBSTACLES = 256
 CRB_DWA_MAX_SPEED_SAMPLES = 64
@@ -143,6 +144,10 @@ PROTOTYPES = {
     "crb_ekf_track_sync": (C.c_int, [C.c_void_p, C.c_void_p]),
     "crb_ekf_track_read": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "crb_ekf_track_close": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "crb_ekf_step_many_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_int32, C.c_void_p, C.c_int, C.c_void_p]),
+    "crb_ekf_track_step_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "crb_pf_default_params": (None, [C.POINTER(PfParams)]),
     "crb_pf_predict_weight_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                                 C.c_void_p, C.c_uint64, C.c_void_p, C.c_int,

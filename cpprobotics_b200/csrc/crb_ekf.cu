@@ -22,101 +22,7 @@
 // that input (tests/test_ekf_edges.py).
 #include <stdint.h>
 
-#include "crb_common.cuh"
-
-struct EkfArgs {
-  double dt;
-  float Q[16];
-  float R[4];
-};
-
-// One filter step on register state.  P is column-major: P[r + 4*c].
-__device__ __forceinline__ void ekf_step(float (&x)[4], float (&P)[16], float z0, float z1,
-                                         float u0, float u1, const EkfArgs& a) {
-  // ---- motion_model(xEst, u) :22-36.  B_(0,0) = DT*cos(yaw) is a double product narrowed to float.
-  float s, c;
-  crb_sincosf_libm(x[2], s, c);   // the host libm's bits (crb_common.cuh)
-  const float b00 = (float)(a.dt * (double)c);
-  const float b10 = (float)(a.dt * (double)s);
-  const float b21 = (float)a.dt;
-  float xp[4];
-  xp[0] = x[0] + b00 * u0;
-  xp[1] = x[1] + b10 * u0;
-  xp[2] = x[2] + b21 * u1;
-  xp[3] = x[3] + u0;  // F_(3,3) = 1 and B_(3,0) = 1: v accumulates (reference quirk)
-
-  // ---- jacobF(xPred, u) :38-47: evaluated at the PREDICTED yaw with v = u(0).
-  float s2, c2;
-  crb_sincosf_libm(xp[2], s2, c2);
-  const float j02 = (float)((-a.dt * (double)u0) * (double)s2);
-  const float j03 = (float)(a.dt * (double)c2);
-  const float j12 = (float)((a.dt * (double)u0) * (double)c2);
-  const float j13 = (float)(a.dt * (double)s2);
-
-  // ---- PPred = (jF*P)*jF^T + Q :69.
-  // T = jF*P: rows 2,3 are rows of P; row 0 = (P0j + j02*P2j) + j03*P3j; row 1 likewise.
-  float T[16];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    T[0 + 4 * j] = (P[0 + 4 * j] + j02 * P[2 + 4 * j]) + j03 * P[3 + 4 * j];
-    T[1 + 4 * j] = (P[1 + 4 * j] + j12 * P[2 + 4 * j]) + j13 * P[3 + 4 * j];
-    T[2 + 4 * j] = P[2 + 4 * j];
-    T[3 + 4 * j] = P[3 + 4 * j];
-  }
-  // PP = T*jF^T + Q: columns 2,3 are columns of T; column 0 = (Ti0 + Ti2*j02) + Ti3*j03.
-  float PP[16];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    PP[i + 4 * 0] = ((T[i + 4 * 0] + T[i + 4 * 2] * j02) + T[i + 4 * 3] * j03) + a.Q[i + 4 * 0];
-    PP[i + 4 * 1] = ((T[i + 4 * 1] + T[i + 4 * 2] * j12) + T[i + 4 * 3] * j13) + a.Q[i + 4 * 1];
-    PP[i + 4 * 2] = T[i + 4 * 2] + a.Q[i + 4 * 2];
-    PP[i + 4 * 3] = T[i + 4 * 3] + a.Q[i + 4 * 3];
-  }
-
-  // ---- update :71-77.  zPred = xPred.xy; S = PPred[0:2,0:2] + R; closed-form 2x2 inverse.
-  const float y0 = z0 - xp[0];
-  const float y1 = z1 - xp[1];
-  const float S00 = PP[0] + a.R[0], S10 = PP[1] + a.R[1];
-  const float S01 = PP[4] + a.R[2], S11 = PP[5] + a.R[3];
-  const float det = S00 * S11 - S10 * S01;
-  const float invdet = 1.0f / det;
-  const float i00 = S11 * invdet, i10 = -S10 * invdet;
-  const float i01 = -S01 * invdet, i11 = S00 * invdet;
-  float K0[4], K1[4];  // K = (PPred*jH^T) * S^-1, columns 0 and 1
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    K0[i] = PP[i] * i00 + PP[i + 4] * i10;
-    K1[i] = PP[i] * i01 + PP[i + 4] * i11;
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) x[i] = xp[i] + (K0[i] * y0 + K1[i] * y1);
-  // PEst = (I - K*jH)*PPred: M = I - K*jH has columns (e0-K0, e1-K1, e2, e3).
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float p0 = PP[0 + 4 * j], p1 = PP[1 + 4 * j];
-    P[0 + 4 * j] = (1.0f - K0[0]) * p0 + (0.0f - K1[0]) * p1;
-    P[1 + 4 * j] = (0.0f - K0[1]) * p0 + (1.0f - K1[1]) * p1;
-    P[2 + 4 * j] = ((0.0f - K0[2]) * p0 + (0.0f - K1[2]) * p1) + PP[2 + 4 * j];
-    P[3 + 4 * j] = ((0.0f - K0[3]) * p0 + (0.0f - K1[3]) * p1) + PP[3 + 4 * j];
-  }
-}
-
-// V consecutive floats of one field: one 4-byte (V = 1) or 8-byte (V = 2) streaming access.
-template <int V>
-__device__ __forceinline__ void ld_agents(const float* p, float (&v)[V]) {
-  if constexpr (V == 1) {
-    v[0] = ld_stream(p);
-  } else {
-    const float2 t = __ldcs(reinterpret_cast<const float2*>(p));
-    v[0] = t.x;
-    v[1] = t.y;
-  }
-}
-template <int V>
-__device__ __forceinline__ void st_agents(float* p, const float (&v)[V]) {
-  if constexpr (V == 1) st_stream(p, v[0]);
-  else __stcs(reinterpret_cast<float2*>(p), make_float2(v[0], v[1]));
-}
+#include "crb_ekf_common.cuh"
 
 // count agents, leading dimension ld (>= count) for x/P, ld_zu for z/u (they may live in a staging
 // buffer with a different pitch).  Each thread filters V consecutive agents; V = 2 needs count, ld and ld_zu
@@ -341,11 +247,12 @@ extern "C" int crb_ekf_track_sync(crb_ctx* ctx, crb_ekf_track* t) {
   return CRB_OK;
 }
 
-extern "C" int crb_ekf_track_step(crb_ctx* ctx, crb_ekf_track* t, const float* z_host, const float* u_host,
-                                  const crb_ekf_params* prm, float* x_out_host, int async) {
-  CRB_REQUIRE(ctx != nullptr && t != nullptr && prm != nullptr, "ctx / track / prm is NULL");
-  CRB_REQUIRE(z_host && u_host, "NULL observation / control array");
-  CRB_DEVICE_GUARD(ctx);
+// One step of a track: z, u reach the device (in place when pinned and mapped, else through t->stage), launch(sk, mz,
+// mu) enqueues the step on the track's kernel stream, and x goes out through the snapshot rotation.  The entry points
+// below differ only in that launch.
+template <class Launch>
+static int ekf_track_step_body(crb_ctx* ctx, crb_ekf_track* t, const float* z_host, const float* u_host,
+                               float* x_out_host, int async, Launch&& launch) {
   const int64_t n = t->n;
   const size_t row = (size_t)n * sizeof(float);
   cudaStream_t sk = ctx->pipe_stream[0], sc = ctx->pipe_stream[1];
@@ -359,7 +266,7 @@ extern "C" int crb_ekf_track_step(crb_ctx* ctx, crb_ekf_track* t, const float* z
     mz = t->stage;
     mu = t->stage + 2 * n;
   }
-  int rc = ekf_launch(ctx, sk, n, n, t->x, t->P, mz, mu, n, 1, prm);
+  int rc = launch(sk, mz, mu);
   if (rc) return rc;
   if (x_out_host) {
     // snapshot p was last used two steps ago: its copy must have left before it is overwritten
@@ -377,6 +284,31 @@ extern "C" int crb_ekf_track_step(crb_ctx* ctx, crb_ekf_track* t, const float* z
     CRB_CUDA(cudaStreamSynchronize(sc));
   }
   return CRB_OK;
+}
+
+extern "C" int crb_ekf_track_step(crb_ctx* ctx, crb_ekf_track* t, const float* z_host, const float* u_host,
+                                  const crb_ekf_params* prm, float* x_out_host, int async) {
+  CRB_REQUIRE(ctx != nullptr && t != nullptr && prm != nullptr, "ctx / track / prm is NULL");
+  CRB_REQUIRE(z_host && u_host, "NULL observation / control array");
+  CRB_DEVICE_GUARD(ctx);
+  return ekf_track_step_body(ctx, t, z_host, u_host, x_out_host, async,
+                             [&](cudaStream_t sk, const float* mz, const float* mu) {
+                               return ekf_launch(ctx, sk, t->n, t->n, t->x, t->P, mz, mu, t->n, 1, prm);
+                             });
+}
+
+extern "C" int crb_ekf_track_step_many(crb_ctx* ctx, crb_ekf_track* t, const float* z_host, const float* u_host,
+                                       const crb_ekf_params* models, int32_t n_models, const int32_t* model_of,
+                                       int32_t* status, float* x_out_host, int async) {
+  CRB_REQUIRE(ctx != nullptr && t != nullptr, "ctx / track is NULL");
+  CRB_REQUIRE(z_host && u_host, "NULL observation / control array");
+  CRB_REQUIRE(models && model_of && n_models >= 1, "NULL model table / model_of, or n_models < 1");
+  CRB_DEVICE_GUARD(ctx);
+  return ekf_track_step_body(ctx, t, z_host, u_host, x_out_host, async,
+                             [&](cudaStream_t sk, const float* mz, const float* mu) {
+                               return ekf_many_launch(ctx, sk, t->n, t->n, t->x, t->P, mz, mu, t->n, 1, models,
+                                                      n_models, model_of, status);
+                             });
 }
 
 extern "C" int crb_ekf_track_read(crb_ctx* ctx, crb_ekf_track* t, float* x_host, float* P_host) {

@@ -3,6 +3,7 @@
 Method names follow the reference functions they replace:
 
   Engine.ekf_estimation      <- ekf_estimation()       src/extended_kalman_filter.cpp:64-78
+  Engine.ekf_estimation_many <- the same, each agent with its own Q, R and DT (ekf_models)
   Engine.pf_predict_weight   <- pf_localization() loop  src/particle_filter.cpp:81-102
   Engine.pf_estimate         <- pf_localization() tail  src/particle_filter.cpp:104-107
   Engine.mpc_solve           <- mpc_solve()             src/model_predictive_control.cpp:255-346
@@ -56,6 +57,27 @@ def ekf_default_params() -> EkfParams:
     p = EkfParams()
     load_library().crb_ekf_default_params(C.byref(p))
     return p
+
+
+# one crb_ekf_params record (include/crb.h): a model table is a device array of these
+EKF_MODEL_DTYPE = np.dtype({"names": ["dt", "Q", "R"], "formats": [np.float64, (np.float32, 16), (np.float32, 4)],
+                            "offsets": [EkfParams.dt.offset, EkfParams.Q.offset, EkfParams.R.offset],
+                            "itemsize": C.sizeof(EkfParams)})
+assert EKF_MODEL_DTYPE.itemsize == 88 and [EKF_MODEL_DTYPE.fields[k][1] for k in ("dt", "Q", "R")] == [0, 8, 72]
+
+
+def ekf_models(dt, Q, R) -> np.ndarray:
+    """A model table for ekf_estimation_many / ekf_track_step_many: dt [m], Q [m, 16] and R [m, 4] (column-major, as
+    crb_ekf_params) packed into m 88-byte records.  Returns a host uint8 array [m, 88]; torch.from_numpy(...).cuda()
+    uploads it as it is."""
+    d = np.asarray(dt, np.float64).reshape(-1)
+    q = np.asarray(Q, np.float32).reshape(d.size, 16)
+    r = np.asarray(R, np.float32).reshape(d.size, 4)
+    if d.size < 1:
+        raise ValueError("a model table needs at least one model")
+    t = np.zeros(d.size, EKF_MODEL_DTYPE)
+    t["dt"], t["Q"], t["R"] = d, q, r
+    return t.view(np.uint8).reshape(d.size, EKF_MODEL_DTYPE.itemsize)
 
 
 def pf_default_params() -> PfParams:
@@ -265,6 +287,30 @@ class Engine:
     def ekf_estimation_host(self, x, P, z, u, params: Optional[EkfParams] = None, n_steps: int = 1):
         self._ekf(self.lib.crb_ekf_step_batched_host, False, x, P, z, u, params, n_steps)
 
+    def _ekf_table(self, models, model_of, n, status, dev):
+        if tuple(models.shape[1:]) != (EKF_MODEL_DTYPE.itemsize,) or models.shape[0] < 1:
+            raise ValueError(f"models: expected [n_models >= 1, {EKF_MODEL_DTYPE.itemsize}] bytes (ekf_models), "
+                             f"got {tuple(models.shape)}")
+        _shape(model_of, 1, n, "model_of")
+        if status is not None:
+            _shape(status, 1, n, "status")
+        return (_ptr(models, np.uint8, device=dev, name="models"), int(models.shape[0]),
+                _ptr(model_of, np.int32, device=dev, name="model_of"),
+                _ptr(status, np.int32, device=dev, name="status"))
+
+    def ekf_estimation_many(self, x, P, z, u, models, model_of, n_steps: int = 1, status=None):
+        """ekf_estimation with a noise model per agent: agent i steps with models[model_of[i]].  In place on x [4,n],
+        P [16,n]; z, u [2*n_steps, n]; models uint8 [n_models, 88] (ekf_models); model_of int32 [n]; status int32 [n]
+        or None (CRB_EKF_OK / CRB_EKF_BAD_MODEL).  CUDA tensors."""
+        n = int(x.shape[-1])
+        _shape(x, 4, n, "x"); _shape(P, 16, n, "P")
+        _shape(z, 2 * n_steps, n, "z"); _shape(u, 2 * n_steps, n, "u")
+        tab, nm, mof, st = self._ekf_table(models, model_of, n, status, True)
+        check(self.lib.crb_ekf_step_many_batched(
+            self.ctx, n, _ptr(x, np.float32, device=True, name="x"), _ptr(P, np.float32, device=True, name="P"),
+            _ptr(z, np.float32, device=True, name="z"), _ptr(u, np.float32, device=True, name="u"), tab, nm, mof,
+            int(n_steps), st), "crb_ekf_step_many_batched")
+
     # ---- PF ---------------------------------------------------------------------------------------
     # resident-state tracking: the reference's time loop (:171-183), 16 B in / 16 B out per update
     def ekf_track_open(self, x0, P0):
@@ -282,6 +328,18 @@ class Engine:
                                           _ptr(u, np.float32, device=False, name="u"), C.byref(prm),
                                           _ptr(x_out, np.float32, device=False, name="x_out"), int(bool(async_))),
               "crb_ekf_track_step")
+
+    def ekf_track_step_many(self, trk, z, u, models, model_of, status=None, x_out=None, async_: bool = False):
+        """ekf_track_step with a noise model per agent.  z, u, x_out host arrays as in ekf_track_step; models,
+        model_of and status CUDA tensors as in ekf_estimation_many, complete on the device before the call (the track
+        runs on the context's pipeline streams)."""
+        n = int(model_of.shape[-1])
+        tab, nm, mof, st = self._ekf_table(models, model_of, n, status, True)
+        check(self.lib.crb_ekf_track_step_many(self.ctx, trk, _ptr(z, np.float32, device=False, name="z"),
+                                               _ptr(u, np.float32, device=False, name="u"), tab, nm, mof, st,
+                                               _ptr(x_out, np.float32, device=False, name="x_out"),
+                                               int(bool(async_))),
+              "crb_ekf_track_step_many")
 
     def ekf_track_sync(self, trk):
         check(self.lib.crb_ekf_track_sync(self.ctx, trk), "crb_ekf_track_sync")

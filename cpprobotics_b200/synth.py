@@ -76,6 +76,29 @@ def ekf_inputs(n: int, i0: int = 0, seed: int = 0xC0FFEE, n_steps: int = 1):
             np.ascontiguousarray(z.astype(f)), np.ascontiguousarray(u.astype(f)))
 
 
+def ekf_fleet_inputs(n: int, n_models: int, seed: int = 0xC0FFEE, n_steps: int = 1):
+    """ekf_inputs for a fleet whose agents each name one of n_models noise models.  Returns a dict with x, P, z, u as
+    ekf_inputs gives them and the model table as arrays: dt float64 [m] in [0.02, 0.2], Q float32 [m, 16] and R
+    float32 [m, 4] (column-major, as crb_ekf_params; pack them with engine.ekf_models), and model_of int32 [n], a
+    shuffled assignment that uses every model when n >= n_models.  Q is the reference's diagonal scaled per model,
+    with non-symmetric off-diagonal entries in every other model; R is a per-model diagonal, non-symmetric in every
+    third model."""
+    x, P, z, u = ekf_inputs(n, seed=seed, n_steps=n_steps)
+    rng = np.random.default_rng([seed, n_models, 0xEF])
+    m = int(n_models)
+    dt = rng.uniform(0.02, 0.2, m)
+    Q = np.zeros((m, 16), np.float64)
+    Q[:, [0, 5, 15]] = 0.01 * rng.uniform(0.25, 4.0, (m, 3))
+    Q[:, 10] = (np.pi / 180) ** 2 * rng.uniform(0.25, 4.0, m)
+    off = [1, 2, 3, 4, 6, 7, 8, 9, 11, 12, 13, 14]
+    Q[::2, off] = 1e-3 * rng.uniform(-1.0, 1.0, (len(range(0, m, 2)), len(off)))
+    R = np.zeros((m, 4), np.float64)
+    R[:, [0, 3]] = rng.uniform(0.1, 2.0, (m, 2))
+    R[::3, 1:3] = rng.uniform(-0.05, 0.05, (len(range(0, m, 3)), 2))
+    model_of = (rng.permutation(n) % m).astype(np.int32)
+    return dict(x=x, P=P, z=z, u=u, dt=dt, Q=Q.astype(np.float32), R=R.astype(np.float32), model_of=model_of)
+
+
 # ---- config 3: batched PF predict + weight (SURVEY §8 d-4) -------------------------------------------
 PF_TRUTH = (2.0, -1.0, 0.3, 1.0)
 

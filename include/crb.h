@@ -7,6 +7,8 @@
  *   crb_ekf_step_batched[_host]        <- ekf_estimation()      src/extended_kalman_filter.cpp:64-78
  *                                         (motion_model :22-36, jacobF :38-47, observation_model :50-55,
  *                                          jacobH :57-62 are folded into the same kernel)
+ *   crb_ekf_step_many_batched           <- the same, each agent with its own Q, R and DT (the reference takes Q and R
+ *                                          per call)
  *   crb_pf_predict_weight_batched[_host] <- pf_localization() particle loop  src/particle_filter.cpp:81-102
  *                                         (motion_model :26-40, gauss_likelihood :53-57)
  *   crb_pf_estimate                     <- pf_localization() tail            src/particle_filter.cpp:104-107
@@ -167,6 +169,36 @@ int crb_ekf_track_step(crb_ctx* ctx, crb_ekf_track* trk, const float* z_host, co
 int crb_ekf_track_sync(crb_ctx* ctx, crb_ekf_track* trk);
 int crb_ekf_track_read(crb_ctx* ctx, crb_ekf_track* trk, float* x_host, float* P_host);
 int crb_ekf_track_close(crb_ctx* ctx, crb_ekf_track* trk);
+
+/* A noise model per agent: ekf_estimation(xEst, PEst, z, u, Q, R) takes Q and R per call, and robots with different
+ * sensors, drive trains or filter periods each have their own.  A model is one crb_ekf_params record (88 bytes: dt at
+ * offset 0, Q at 8, R at 72); a model table is a DEVICE array of n_models such records in this struct's own layout,
+ * so a std::vector<crb_ekf_params> is copied up as it is.  model_of [n] (int32, device) names each agent's model.
+ *
+ * crb_ekf_step_many_batched: x, P, z, u and n_steps as in crb_ekf_step_batched; agent i uses models[model_of[i]] for
+ * all n_steps steps of the launch, and its x and P are bitwise those of crb_ekf_step_batched run with
+ * prm = &models[model_of[i]] (also signed zeros, NaN and inf).  status [n] (device) is optional: NULL is not written.
+ * An index outside [0, n_models) reads no record: that agent's x and P are written NaN (a filter whose step did not
+ * run must not look as if it had, also when status is NULL) and its status is CRB_EKF_BAD_MODEL; other agents are
+ * unaffected.  Host arguments are checked before any device work: a NULL ctx, n < 0, n_steps < 1, n_models < 1,
+ * or (n > 0) a NULL x, P, z, u, models or model_of is CRB_ERR_INVALID_ARG; n = 0 is a no-op.  The call only enqueues
+ * on the context's stream and can be captured in a CUDA graph.
+ *
+ * crb_ekf_track_step_many: crb_ekf_track_step with the model table in place of prm (z_host, u_host, x_out_host,
+ * async and the two-deep rotation as there).  models, model_of and status are DEVICE arrays that the caller uploads
+ * once and reuses every tick.  The track runs on the context's pipeline streams, not its main stream, so the table
+ * and model_of must be complete on the device before the call (e.g. after crb_sync), and status is complete when the
+ * step's x_out_host is.
+ *
+ * Agents are independent: a context with a communicator steps its own shard and makes no collective. */
+#define CRB_EKF_OK 0
+#define CRB_EKF_BAD_MODEL 1   /* model_of[i] is outside [0, n_models): x and P of agent i are written NaN */
+int crb_ekf_step_many_batched(crb_ctx* ctx, int64_t n, float* x, float* P, const float* z, const float* u,
+                              const crb_ekf_params* models, int32_t n_models, const int32_t* model_of,
+                              int n_steps, int32_t* status);
+int crb_ekf_track_step_many(crb_ctx* ctx, crb_ekf_track* trk, const float* z_host, const float* u_host,
+                            const crb_ekf_params* models, int32_t n_models, const int32_t* model_of,
+                            int32_t* status, float* x_out_host, int async);
 
 /* ---- particle filter -------------------------------------------------------------------------- */
 /* Constants from src/particle_filter.cpp: DT :18, PI :19 (3.141592653, *not* M_PI), Q :217 (0.01),

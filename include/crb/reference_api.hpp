@@ -2,7 +2,7 @@
 // on top of the C ABI (crb.h).  A CppRobotics main() re-targets to the H100 engine by including this
 // header instead of <Eigen/Eigen> for the hot functions and linking libcrb.so.
 //
-//   ekf_estimation(xEst, PEst, z, u, Q, R)        src/extended_kalman_filter.cpp:64-78
+//   ekf_estimation(xEst, PEst, z, u, Q, R)        src/extended_kalman_filter.cpp:64-78 (also over vectors of robots)
 //   pf_localization(px, pw, xEst, PEst, z, u, Rsim, Q, gen, gaussian_d)   src/particle_filter.cpp:73-109
 //   mpc_solve(x0, traj_ref)                       src/model_predictive_control.cpp:255-346
 //   update(state, a, delta)                       src/model_predictive_control.cpp:69-81
@@ -149,6 +149,48 @@ inline void ekf_estimation(crb::Vector4f& xEst, crb::Matrix4f& PEst, crb::Vector
   crb::check(crb_ekf_step_batched_host(crb::Session::get(), 1, xEst.data(), PEst.data(), z.data(),
                                        u.data(), &prm, 1),
              "crb_ekf_step_batched_host");
+}
+
+// ekf_estimation for a fleet, each robot with its own Q and R: robot i is ekf_estimation(xEst[i], PEst[i], z[i], u[i],
+// Q[i], R[i]) with the reference's DT, all in one launch of crb_ekf_step_many_batched with one model per robot.
+inline void ekf_estimation(std::vector<crb::Vector4f>& xEst, std::vector<crb::Matrix4f>& PEst,
+                           const std::vector<crb::Vector2f>& z, const std::vector<crb::Vector2f>& u,
+                           const std::vector<crb::Matrix4f>& Q, const std::vector<crb::Matrix2f>& R) {
+  const size_t n = xEst.size();
+  if (PEst.size() != n || z.size() != n || u.size() != n || Q.size() != n || R.size() != n)
+    throw std::runtime_error("ekf_estimation: xEst, PEst, z, u, Q and R differ in length");
+  if (n == 0) return;
+  crb_ctx* ctx = crb::Session::get();
+  crb_ekf_params dflt;
+  crb_ekf_default_params(&dflt);
+  // host and device: models [n] (22 floats each) | x [4][n] | P [16][n] | z [2][n] | u [2][n] | model_of [n]
+  const size_t nm = sizeof(crb_ekf_params) / sizeof(float);
+  std::vector<float> h((nm + 25) * n);
+  std::vector<crb_ekf_params> models(n, dflt);
+  float* hx = h.data() + nm * n;
+  for (size_t i = 0; i < n; ++i) {
+    std::memcpy(models[i].Q, Q[i].data(), sizeof(models[i].Q));
+    std::memcpy(models[i].R, R[i].data(), sizeof(models[i].R));
+    for (int f = 0; f < 4; ++f) hx[f * n + i] = xEst[i](f);
+    for (int f = 0; f < 16; ++f) hx[(4 + f) * n + i] = PEst[i].data()[f];
+    for (int f = 0; f < 2; ++f) hx[(20 + f) * n + i] = z[i](f);
+    for (int f = 0; f < 2; ++f) hx[(22 + f) * n + i] = u[i](f);
+    const int32_t m = (int32_t)i;
+    std::memcpy(hx + 24 * n + i, &m, sizeof(m));
+  }
+  std::memcpy(h.data(), models.data(), n * sizeof(crb_ekf_params));
+  float* d = crb::Session::scratch(h.size());
+  float* dx = d + nm * n;
+  crb::check(crb_memcpy_h2d(ctx, d, h.data(), h.size() * sizeof(float)), "crb_memcpy_h2d");
+  crb::check(crb_ekf_step_many_batched(ctx, (int64_t)n, dx, dx + 4 * n, dx + 20 * n, dx + 22 * n,
+                                       (const crb_ekf_params*)d, (int32_t)n, (const int32_t*)(dx + 24 * n), 1,
+                                       nullptr),
+             "crb_ekf_step_many_batched");
+  crb::check(crb_memcpy_d2h(ctx, hx, dx, 20 * n * sizeof(float)), "crb_memcpy_d2h");
+  for (size_t i = 0; i < n; ++i) {
+    for (int f = 0; f < 4; ++f) xEst[i](f) = hx[f * n + i];
+    for (int f = 0; f < 16; ++f) PEst[i].data()[f] = hx[(4 + f) * n + i];
+  }
 }
 
 // src/model_predictive_control.cpp:69-81
