@@ -9,7 +9,7 @@
 // predicted particles, its weights and its cumulative weights in its own slice of dynamic shared memory
 // (pf_fleet_slice_bytes), then runs predict + weight (the two-lane routine of crb_pf_common.cuh, particles 2l and
 // 2l + 1 of each 64-particle round in lane l), the weight sum, normalisation, the estimate moments around the robot's
-// particle 0, Neff, the resampling decision, the cumulative weights and the gather, with warp shuffles and
+// heaviest particle, Neff, the resampling decision, the cumulative weights and the gather, with warp shuffles and
 // __syncwarp only: no global scan, no second launch.  The reductions have a fixed order (lane-sequential, then a
 // fixed shuffle tree), so a robot's outputs do not depend on the launch shape or on the other robots.
 #include "crb_pf_common.cuh"
@@ -77,8 +77,12 @@ crb_pf_fleet_kernel(float* __restrict__ px, float* __restrict__ pw, float* __res
   __syncwarp();
 
   // ---- predict + weight (:81-102): particles j and j + 1 in the two lanes; a lone last particle in both ----
+  // The lane also keeps the heaviest of its raw weights (ties to the lower index; a NaN never wins), the pivot of the
+  // moments below: per round the larger of its pair, and the pair's first particle.
   const float2 one = f2(a.one);
   double sw_d = 0.0;
+  float bw = -INFINITY;
+  int bp = 0;
   for (int p0 = 0; p0 < np; p0 += 64) {
     const int j = p0 + 2 * lane;
     if (j < np) {
@@ -102,6 +106,8 @@ crb_pf_fleet_kernel(float* __restrict__ px, float* __restrict__ pw, float* __res
       s_x[j] = X0.x; s_x[np + j] = X1.x; s_x[2 * np + j] = X2.x; s_x[3 * np + j] = X3.x;
       s_w[j] = Wn.x;
       sw_d += (double)Wn.x;
+      const float w2 = fmaxf(Wn.x, Wn.y);   // Wn.y is particle j again when it is the lone last one
+      if (w2 > bw) { bw = w2; bp = j; }
       if (two) {
         s_x[k] = X0.y; s_x[np + k] = X1.y; s_x[2 * np + k] = X2.y; s_x[3 * np + k] = X3.y;
         s_w[k] = Wn.y;
@@ -109,16 +115,26 @@ crb_pf_fleet_kernel(float* __restrict__ px, float* __restrict__ pw, float* __res
       }
     }
   }
+  // the heaviest particle of the lane: the first of its pair unless that one is lighter (or NaN)
+  int bi = bw > -INFINITY && !(s_w[bp] == bw) ? bp + 1 : bp;
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sw_d += __shfl_down_sync(0xffffffffu, sw_d, o);
+  for (int o = 16; o > 0; o >>= 1) {
+    sw_d += __shfl_down_sync(0xffffffffu, sw_d, o);
+    const float ow = __shfl_xor_sync(0xffffffffu, bw, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ow > bw || (ow == bw && oi < bi)) { bw = ow; bi = oi; }   // the same winner in every lane
+  }
   sw_d = __shfl_sync(0xffffffffu, sw_d, 0);   // pw.sum() before the normalisation, the same bits in every lane
   __syncwarp();
 
-  // ---- normalise (:104), cumulative weights (:111-118), sum of squares (:126), moments around particle 0 ----
+  // ---- normalise (:104), cumulative weights (:111-118), sum of squares (:126), moments around the heaviest
+  // particle: its normalised weight w_max >= 1/np and Var_f >= w_max (x_f - xEst_f)^2, so the pivot lies within
+  // sqrt(np) standard deviations of the mean and the one-pass moments lose at most ~np 2^-52 of each variance to
+  // cancellation, wherever the cloud and its outliers are.  All-zero or NaN weights keep particle 0 (NaN results). ----
   const float sw = (float)sw_d;              // pw.sum() is a float in the reference (:104)
   double piv[4];
 #pragma unroll
-  for (int f = 0; f < 4; ++f) piv[f] = (double)s_x[f * np];
+  for (int f = 0; f < 4; ++f) piv[f] = (double)s_x[f * np + bi];
   double v[15], sq = 0.0, carry = 0.0;
 #pragma unroll
   for (int q = 0; q < 15; ++q) v[q] = 0.0;

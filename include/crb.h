@@ -262,9 +262,11 @@ int crb_pf_resample(crb_ctx* ctx, int64_t n, float* px, float* pw, float* px_tmp
  *                  crb_pf_resample
  *   result_dev [CRB_PF_RESULT_LEN] (device, f64): [0..3] xEst, [4..19] PEst (column-major), [20] sum of the
  *                  un-normalised weights, [21] Neff, [22] 1.0 if resampled, [23] sum of squared weights
- * PEst comes from one pass of double moments centred on particle 0 (rank 0's on a sharded filter), so its accuracy
- * does not depend on the distance from the origin: each entry is within 1e-6 sqrt(P_rr P_cc) of the float64
- * two-pass covariance around xEst (tested with 5 cm clouds up to 10^5 m away).  All-zero weights give NaN.
+ * PEst comes from one pass of double moments centred on particle 0 (rank 0's on a sharded filter).  Its accuracy does
+ * not depend on the distance from the origin, but it does depend on how far particle 0 lies from the cloud: the
+ * cancellation error grows with (that distance / the cloud's spread)^2.  With particle 0 in the cloud each entry is
+ * within 1e-6 sqrt(P_rr P_cc) of the float64 two-pass covariance around xEst (tested with 5 cm clouds up to 10^5 m
+ * away); a light particle 0 kilometres from a centimetre-wide cloud can exceed that.  All-zero weights give NaN.
  * Everything is enqueued on the context's stream (capturable in a CUDA graph).  On a context with a communicator
  * (a filter sharded over GPUs) the weight sum and the moments are all-reduced (one 120-byte all-reduce), every
  * rank gets the global xEst / PEst, weights are normalised globally, and particles are NOT resampled (px_next is
@@ -300,7 +302,11 @@ int crb_pf_step(crb_ctx* ctx, int64_t n, float* px, float* pw, float* px_next, c
  *   status [n_robots] int32 CRB_PF_FLEET_* (optional, NULL = not written)
  * A robot's px, pw and px_next are bitwise those of crb_pf_predict_weight_batched + crb_pf_step's tail run on that
  * robot alone with its u in prm and its list as the landmarks, up to the summation order of the weight sum and the
- * cumulative weights (the reductions run over the robot's particles in a fixed order of their own).  A NaN in one
+ * cumulative weights (the reductions run over the robot's particles in a fixed order of their own).  The estimate's
+ * moments are centred on the robot's heaviest particle (ties to the lower index; particle 0 when no weight is a
+ * number), not on particle 0: its normalised weight is at least 1/np, so it lies within sqrt(np) standard deviations
+ * of the mean and the cancellation costs about np 2^-52 of each variance.  PEst is therefore within
+ * 1e-6 sqrt(P_rr P_cc) of the float64 two-pass covariance wherever particle 0 and the cloud lie.  A NaN in one
  * list or all-zero weights in one robot make only that robot's outputs NaN.  On a context with a communicator the
  * robots are independent too: there is no collective, each rank steps its own robots as on one GPU.
  * CRB_ERR_INVALID_ARG before any device work unless 1 <= np <= CRB_PF_FLEET_MAX_NP, n_robots >= 0, prm is given,

@@ -18,6 +18,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import pf_cases as PC
 from cpprobotics_b200 import _lib, synth
 from oracle import oracle as OO
 from oracle import pf_fleet as PFF
@@ -233,30 +234,6 @@ def _host(t):
     return t.cpu().numpy()
 
 
-@pytest.fixture(scope="module")
-def engine():
-    from cpprobotics_b200 import Engine
-    e = Engine(0)
-    yield e
-    e.close()
-
-
-def grouped_fleet(nr, npr, seed):
-    """A fleet whose robots use one of three lists (0, 1 and 64 rows, shuffled over the robots) and one of two controls,
-    so that each of the six (list, u) groups can be checked with ONE crb_pf_predict_weight_batched call."""
-    f = synth.pf_fleet_inputs(nr, npr, seed=seed)
-    rng = np.random.default_rng(seed)
-    lm64 = synth.pf_landmarks(64, seed=seed)
-    lists = [np.zeros((0, 3), np.float32), lm64[:1], lm64]
-    z, z_off = synth.pack_obstacles(lists, 3)
-    f["z"], f["z_off"], f["z_of"] = z, z_off, rng.integers(0, 3, nr).astype(np.int32)
-    us = np.array([[1.0, 0.1], [0.7, -0.2]], np.float32)
-    g = rng.integers(0, 2, nr)
-    f["u"] = np.ascontiguousarray(us[g].T)
-    f["ugroup"], f["lists"], f["us"] = g, lists, us
-    return f
-
-
 def run_fleet(engine, f, npr, nth=None, noise=True, uniforms=True, status=True):
     import torch
     px, pw = _dev(f["px"]), _dev(f["pw"])
@@ -269,8 +246,10 @@ def run_fleet(engine, f, npr, nth=None, noise=True, uniforms=True, status=True):
     return _host(px), _host(pw), _host(pxn), _host(res), (_host(st) if status else None)
 
 
-CELLS = [(1, 65536), (2, 4096), (31, 7), (100, 65536), (100, 1), (257, 4096), (1024, 7), (1024, 4096), (CAP, 1),
-         (CAP, 7)]
+# (np, n_robots); 1157 is the last np with 8 robots per CTA, 1158 the first with 7, 4789 the last with 2 and 4790 the
+# first with 1, each with a partial last CTA where it can have one
+CELLS = [(1, 65536), (2, 4096), (31, 7), (100, 65536), (100, 1), (257, 4096), (1024, 7), (1024, 4096), (1157, 13),
+         (1158, 13), (4789, 5), (4790, 3), (CAP, 1), (CAP, 7)]
 
 
 @pytest.mark.gpu
@@ -281,7 +260,7 @@ def test_particles_are_the_single_filter_kernel_bitwise(engine, npr, nr):
     its own weight sum (result[20])."""
     import torch
     from cpprobotics_b200 import pf_default_params
-    f = grouped_fleet(nr, npr, seed=npr * 7 + nr)
+    f = PC.grouped_fleet(nr, npr, seed=npr * 7 + nr)
     px, pw, pxn, res, st = run_fleet(engine, f, npr, nth=0.0)
     assert (st == _lib.CRB_PF_FLEET_OK).all()
     assert same(pxn, px) and (res[22] == 0).all()

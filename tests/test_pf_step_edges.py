@@ -13,11 +13,11 @@ GPU against float64 / oracle restatements of the same operations, fed with the G
 import numpy as np
 import pytest
 
+import pf_cases as PC
 from cpprobotics_b200 import Engine, synth
 from oracle import oracle as O
 
 F32 = np.float32
-CHUNK = 2048                # weights per scan block
 FORM_SIZES = (1 << 20, (1 << 21) + 1)   # the three-launch and the seven-launch form
 
 
@@ -55,28 +55,10 @@ def _assert_pf_parity(px_got, pw_got, px_want, pw_want, lm, sigma2=0.01):
         assert (np.abs(pw_got[off].astype(np.float64) - pw_want[off]) <= tol).all()
 
 
-def _philox_u12(seed, n):
-    """crb_oracle_philox_uniform12(seed, j) for j = 0 .. n-1, vectorised: the uniforms in [1, 2) the resampling
-    draws when no uniforms are given."""
-    m32 = np.uint64(0xFFFFFFFF)
-    idx = np.arange(n, dtype=np.uint64)
-    c0, c1 = idx & m32, idx >> np.uint64(32)
-    c2 = np.full(n, 0x5EED5EED, np.uint64)
-    c3 = np.zeros(n, np.uint64)
-    k0, k1 = np.uint64(seed & 0xFFFFFFFF), np.uint64((seed >> 32) & 0xFFFFFFFF)
-    for _ in range(10):
-        p0 = np.uint64(0xD2511F53) * c0
-        p1 = np.uint64(0xCD9E8D57) * c2
-        c0, c1, c2, c3 = (p1 >> np.uint64(32)) ^ c1 ^ k0, p1 & m32, (p0 >> np.uint64(32)) ^ c3 ^ k1, p0 & m32
-        k0 = (k0 + np.uint64(0x9E3779B9)) & m32
-        k1 = (k1 + np.uint64(0xBB67AE85)) & m32
-    return F32(1.0) + (c0 >> np.uint64(9)).astype(F32) * F32(1.1920928955078125e-07)
-
-
 def test_vectorised_philox_uniforms_match_the_oracle():
     seed = 0x9_8765_4321
     idx = [0, 1, 2, 1023, 1024, 999_999, (1 << 21) + 1]
-    u = _philox_u12(seed, idx[-1] + 1)
+    u = PC.philox_u12(seed, idx[-1] + 1)
     assert [float(u[j]) for j in idx] == [O.philox_uniform12(seed, j) for j in idx]
 
 
@@ -96,56 +78,6 @@ def _to_dev(a, offset=False):
 
 def _same(a, b):
     return np.array_equal(a, b, equal_nan=True)
-
-
-def _check_estimate(gx, gw, xe_got, P_got):
-    """xEst within one float ulp of the float64 weighted mean; PEst against the float64 two-pass covariance around
-    that xEst with d = float32(px - xEst), as calc_covariance.  Returns max |dP_rc| / sqrt(P_rr P_cc)."""
-    if not np.isfinite(gw).all():
-        assert np.isnan(xe_got).all() and np.isnan(P_got).all()
-        return 0.0
-    w = gw.astype(np.float64)
-    m = gx.astype(np.float64) @ w
-    xe = xe_got.astype(F32)
-    assert np.array_equal(xe.astype(np.float64), xe_got)
-    assert (np.abs(xe_got - m) <= np.spacing(np.abs(m).astype(F32)).astype(np.float64)).all(), (xe_got, m)
-    d = (gx - xe[:, None]).astype(np.float64)
-    C = (d * w) @ d.T
-    assert np.array_equal(P_got, P_got.T)
-    assert (np.diag(P_got) >= 0).all()
-    scale = np.sqrt(np.outer(np.diag(C), np.diag(C)))
-    err = np.abs(P_got - C)
-    ratio = float(np.max(np.where(scale > 0, err / np.where(scale > 0, scale, 1.0), np.where(err > 0, np.inf, 0.0))))
-    assert ratio <= 1e-6, f"max |dP| / sqrt(P_rr P_cc) = {ratio:.3g}\nGPU\n{P_got}\ntwo-pass\n{C}"
-    return ratio
-
-
-def _assert_same_survivors(nxt, px2, gx, gw, U):
-    """Resampled particles against the oracle, bit for bit, except at ties of the cumulative weight.
-
-    The GPU sums the weights in blocks, the oracle in sequence; both round the double sums to the float wcum.  Where a
-    double prefix sum lies within its rounding error of a float rounding boundary the two wcum can differ by one float
-    ulp, and a resampleid equal to one of them then picks a neighbouring particle (a few per 10^6 particles with
-    synthetic weights).  Every differing slot j must be such a tie: the GPU's particle is one within 64 of the
-    oracle's, and every cumulative weight between the two lies within one float ulp of resampleid_j."""
-    n = gx.shape[1]
-    bad = np.flatnonzero(~(nxt == px2).all(axis=0))
-    if bad.size == 0:
-        return
-    assert bad.size <= max(2, n >> 16), f"{bad.size} resampled particles differ, first at j = {bad[:8]}"
-    w64 = np.cumsum(gw.astype(np.float64))
-    wcum = w64.astype(F32)
-    j = np.arange(n)
-    rid = ((j / n).astype(F32).astype(np.float64) + U / n).astype(F32)
-    rid[1:] = np.maximum(rid[1:], rid[:-1])          # the reference's search index never moves back
-    for jb in bad:
-        i_o = min(int(np.searchsorted(wcum, rid[jb], "left")), n - 1)
-        assert (px2[:, jb] == gx[:, i_o]).all()
-        lo, hi = max(0, i_o - 64), min(n, i_o + 65)
-        ks = lo + np.flatnonzero((gx[:, lo:hi] == nxt[:, [jb]]).all(axis=0))
-        assert ks.size, f"slot {jb}: the GPU's particle is not within 64 of the oracle's {i_o}"
-        tie = lambda k: (np.abs(w64[min(k, i_o):max(k, i_o)] - rid[jb]) <= np.spacing(rid[jb])).all()
-        assert any(tie(int(k)) for k in ks), f"slot {jb}: a different particle without a cumulative-weight tie"
 
 
 def _step(engine, px, pw, noise, lm, nth, uniforms, resample_seed, seed, offset):
@@ -188,7 +120,7 @@ def _check_step(engine, px, pw, noise, lm, *, nth, uniforms=None, resample_seed=
     # the requested threshold: the same estimate, Neff, the decision and the index work
     x1, w1, nxt, r = _step(engine, px, pw, noise, lm, nth, uniforms, resample_seed, seed, offset)
     assert np.array_equal(x1, gx) and _same(r[:22], r0[:22]) and _same(r[23], r0[23])
-    U = (uniforms if uniforms is not None else _philox_u12(resample_seed, n)).astype(np.float64)
+    U = (uniforms if uniforms is not None else PC.philox_u12(resample_seed, n)).astype(np.float64)
     neff_o = O.pf_resample(gx, gw, U, nth=0.0)[3]
     neff = F32(r[21])
     assert (np.isnan(neff) and np.isnan(neff_o)) or abs(neff - F32(neff_o)) <= np.spacing(F32(neff_o)), (neff, neff_o)
@@ -196,11 +128,11 @@ def _check_step(engine, px, pw, noise, lm, *, nth, uniforms=None, resample_seed=
     if r[22]:
         px2, pw2, did, _ = O.pf_resample(gx, gw, U, nth=np.inf)
         assert did
-        _assert_same_survivors(nxt, px2, gx, gw, U)
+        PC.assert_same_survivors(nxt, px2, gx, gw, U)
         assert np.array_equal(w1, pw2)
     else:
         assert np.array_equal(nxt, gx) and _same(w1, gw)
-    ratio = _check_estimate(gx, gw, r0[0:4], r0[4:20].reshape(4, 4).T)
+    ratio = PC.check_estimate(gx, gw, r0[0:4], r0[4:20].reshape(4, 4).T)
     return dict(x=gx, w=gw, r=r, nxt=nxt, w_out=w1, ratio=ratio)
 
 
@@ -249,41 +181,8 @@ def test_pf_step_landmark_counts(engine, n, n_lm):
 
 
 # ---- controlled weights -----------------------------------------------------------------------------------------
-def _weights(kind, n):
-    """Weight families that synthetic likelihoods never produce: one-hot, the NP-1 cap, long zero runs, two levels
-    2^20 apart, and heavy-tailed gamma(0.1) weights clipped to a narrow exponent span with a quarter of them dead."""
-    rng = np.random.default_rng(WEIGHT_KINDS.index(kind))
-    w = np.zeros(n, np.float64)
-    if kind.startswith("onehot"):
-        w[{"onehot_first": 0, "onehot_last": n - 1, "onehot_chunk_end": 100 * CHUNK - 1,
-           "onehot_chunk_start": 100 * CHUNK}[kind]] = 1.0
-    elif kind == "cap":             # all mass on NP-1, tiny weights elsewhere: the reference's cap (:139)
-        w[:] = 2.0 ** -40
-        w[-1] = 1.0
-    elif kind == "zero_run":        # > 4096 zeros between normal weights: both non-staged window searches
-        w[:] = 1.0 + np.floor(rng.random(n) * 64)
-        a = n // 3
-        w[a:a + 5000] = 0.0
-        w[2 * a:2 * a + 9000] = 0.0
-    elif kind == "two_levels":
-        w[:] = np.where(rng.random(n) < 0.5, 1.0, 2.0 ** -20)
-    elif kind == "gamma":           # heavy-tailed, a quarter dead, clipped to a span of 2^(29 - log2 n)
-        g = rng.gamma(0.1, 1.0, n)
-        span = 2.0 ** (29 - int(np.ceil(np.log2(n))))
-        g = np.clip(g, g.max() / span, None)
-        w = g.astype(F32).astype(np.float64)
-        w[rng.integers(0, n, n // 4)] = 0.0
-    elif kind == "all_zero":
-        pass
-    return w.astype(F32)
-
-
-WEIGHT_KINDS = ["onehot_first", "onehot_last", "onehot_chunk_end", "onehot_chunk_start", "cap", "zero_run",
-                "two_levels", "gamma", "all_zero"]
-
-
 @pytest.mark.gpu
-@pytest.mark.parametrize("kind", WEIGHT_KINDS)
+@pytest.mark.parametrize("kind", PC.WEIGHT_KINDS)
 @pytest.mark.parametrize("n", FORM_SIZES)
 def test_pf_step_controlled_weights(engine, n, kind):
     """With no landmarks the weight update is W * exp(0): the weights are what the test sets.  All-zero weights are
@@ -291,7 +190,7 @@ def test_pf_step_controlled_weights(engine, n, kind):
     weights then go through crb_pf_resample, whose gather reads materialised cumulative weights."""
     import torch
     px, _, noise, lm = _inputs(n, 0)
-    pw = _weights(kind, n)
+    pw = PC.weights(kind, n)
     u = (1.0 + np.random.default_rng(3).random(n)).astype(F32)
     st = _check_step(engine, px, pw, noise, lm, nth=float(n), uniforms=u, weights_unchanged=True)
     if kind == "all_zero":
@@ -310,7 +209,7 @@ def test_pf_step_controlled_weights(engine, n, kind):
     assert did == did_o
     assert (np.isnan(neff) and np.isnan(neff_o)) or abs(F32(neff) - F32(neff_o)) <= np.spacing(F32(neff_o))
     if did:
-        _assert_same_survivors(a.cpu().numpy(), px2, gx, gw, u.astype(np.float64))
+        PC.assert_same_survivors(a.cpu().numpy(), px2, gx, gw, u.astype(np.float64))
     else:
         assert _same(a.cpu().numpy(), px2)
     assert _same(b.cpu().numpy(), pw2)
@@ -380,17 +279,6 @@ def test_pf_step_results_do_not_depend_on_earlier_calls(engine):
 
 
 # ---- large coordinates ------------------------------------------------------------------------------------------
-def _far(n, centre, spread=0.05):
-    """synth.pf_inputs moved rigidly to `centre` (with the landmarks) and shrunk to `spread` metres."""
-    px, pw, noise = synth.pf_inputs(n)
-    lm = synth.pf_landmarks(8).astype(np.float64)
-    T = synth.PF_TRUTH
-    for f in (0, 1):
-        px[f] = (centre[f] + (px[f].astype(np.float64) - T[f]) * (spread / 0.2)).astype(F32)
-        lm[:, 1 + f] += centre[f] - T[f]
-    return px, pw, noise, lm.astype(F32)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("centre", [(1e4, -3e4), (1e5, 1e5)], ids=["1e4_-3e4", "1e5_1e5"])
 @pytest.mark.parametrize("n", FORM_SIZES)
@@ -398,7 +286,7 @@ def test_pf_step_covariance_far_from_the_origin(engine, n, centre):
     """A cloud of 5 cm a few km from the origin: PEst must stay at float accuracy.  crb_pf_estimate (two-pass, centred
     on xEst) on the same predicted particles must pass the same gate and agree with crb_pf_step to it."""
     import torch
-    px, pw, noise, lm = _far(n, centre)
+    px, pw, noise, lm = PC.far(n, centre)
     st = _check_step(engine, px, pw, noise, lm, nth=float(n), resample_seed=11)
     a, b = _to_dev(px), _to_dev(pw)
     engine.pf_predict_weight(a, b, _to_dev(noise), lm)
@@ -406,7 +294,7 @@ def test_pf_step_covariance_far_from_the_origin(engine, n, centre):
     torch.cuda.synchronize()
     ex, ew = a.cpu().numpy(), b.cpu().numpy()
     assert np.array_equal(ex, st["x"])
-    _check_estimate(ex, ew, xe.astype(np.float64), Pe.astype(np.float64))
+    PC.check_estimate(ex, ew, xe.astype(np.float64), Pe.astype(np.float64))
     P_step = st["r"][4:20].reshape(4, 4).T
     scale = np.sqrt(np.outer(np.diag(P_step), np.diag(P_step)))
     assert (np.abs(P_step - Pe) <= 1e-6 * scale).all()
