@@ -66,6 +66,9 @@ struct CrbDeviceGuard {
   }
 
 void crb_set_error(const char* fmt, ...);
+// CRB_OK, or CRB_ERR_NO_DEVICE and the error string "<fn>: no usable CUDA device; ..." without a usable CUDA device:
+// an entry point calls it after validating its arguments, as there is no CPU fallback.
+int crb_require_device(const char* fn);
 
 #define CRB_CUDA(call)                                                                      \
   do {                                                                                      \

@@ -12,6 +12,17 @@ void crb_set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+int crb_require_device(const char* fn) {
+  int count = 0;
+  const cudaError_t e = cudaGetDeviceCount(&count);
+  if (e != cudaSuccess || count == 0) {
+    cudaGetLastError();
+    crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", fn);
+    return CRB_ERR_NO_DEVICE;
+  }
+  return CRB_OK;
+}
+
 extern "C" {
 
 int crb_abi_version(void) { return CRB_ABI_VERSION; }

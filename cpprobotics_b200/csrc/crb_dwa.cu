@@ -9,7 +9,8 @@
 // Mapping: one warp per robot.  The robot's speed and yaw-rate grids are built into shared memory, the lanes
 // stride over the Nv x Ny samples in v-major order, each lane rolls its sample out in registers (only the even
 // points and the last one are used, so no trajectory is stored), and a shuffle reduction picks the winner.
-// The winning rollout is computed again, by every lane, to write `traj` when it is requested.
+// The winning rollout is computed again, by every lane, to write `traj` when it is requested.  All of that is one
+// per-robot body, dwa_robot; the two kernels differ only in how they stage the obstacles into shared memory.
 #include <float.h>
 
 #include "crb_common.cuh"
@@ -95,19 +96,15 @@ __device__ __forceinline__ float dwa_obstacle_cost(float dmin, float robot_radiu
   return (float)(1.0 / (double)minr);  // 1 / FLT_MAX is a float subnormal: no flush to zero anywhere here
 }
 
-__global__ void __launch_bounds__(DWA_BLOCK)
-crb_dwa_control_kernel(int64_t n, const float* __restrict__ xg, float* __restrict__ ug,
-                       const float* __restrict__ goalg, const float* __restrict__ obg, int n_ob,
-                       crb_dwa_params p, int n_steps, float* __restrict__ costg, int32_t* __restrict__ bestg,
-                       float* __restrict__ trajg) {
-  __shared__ float2 s_ob[CRB_DWA_MAX_OBSTACLES];
-  __shared__ float s_v[DWA_WARPS][CRB_DWA_MAX_SPEED_SAMPLES];
-  __shared__ float s_w[DWA_WARPS][CRB_DWA_MAX_YAWRATE_SAMPLES];
-  for (int k = threadIdx.x; k < n_ob; k += DWA_BLOCK) s_ob[k] = make_float2(obg[2 * k], obg[2 * k + 1]);
-  __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t i = (int64_t)blockIdx.x * DWA_WARPS + warp;
-  if (i >= n) return;  // whole warps leave together
+// dwa_control for robot i, by the 32 lanes of its warp: the state load, the window, the sample grids in the warp's
+// rows s_v / s_w, every sample's rollout and cost against the n_ob obstacles at ob (shared memory; a slice this warp
+// staged itself is visible after the __syncwarp below), the argmin and the outputs.  status, when not NULL, gets
+// CRB_DWA_OK.
+__device__ __forceinline__ void dwa_robot(int64_t n, int64_t i, int lane, const float2* ob, int n_ob, float* s_v,
+                                          float* s_w, const float* __restrict__ xg, float* __restrict__ ug,
+                                          const float* __restrict__ goalg, crb_dwa_params p, int n_steps,
+                                          float* __restrict__ costg, int32_t* __restrict__ bestg,
+                                          float* __restrict__ trajg, int32_t* __restrict__ statusg) {
   float x[5];
 #pragma unroll
   for (int f = 0; f < 5; ++f) x[f] = xg[(int64_t)f * n + i];
@@ -125,24 +122,24 @@ crb_dwa_control_kernel(int64_t n, const float* __restrict__ xg, float* __restric
   // stores its own entries)
   int nv = 0, nw = 0;
   for (float v = dw0; nv < CRB_DWA_MAX_SPEED_SAMPLES && v <= dw1; v = v + p.v_reso, ++nv)
-    if ((nv & 31) == lane) s_v[warp][nv] = v;
+    if ((nv & 31) == lane) s_v[nv] = v;
   for (float w = dw2; nw < CRB_DWA_MAX_YAWRATE_SAMPLES && w <= dw3; w = w + p.yawrate_reso, ++nw)
-    if ((nw & 31) == lane) s_w[warp][nw] = w;
-  __syncwarp();
+    if ((nw & 31) == lane) s_w[nw] = w;
+  __syncwarp();  // the grids (and a per-warp obstacle slice)
 
-  const float d0 = dwa_min_d2(__int_as_float(0x7fffffff), x[0], x[1], s_ob, n_ob);  // point 0 is x itself
+  const float d0 = dwa_min_d2(__int_as_float(0x7fffffff), x[0], x[1], ob, n_ob);  // point 0 is x itself
   const float gmag = sqrtf(gx * gx + gy * gy);
   float best_c = 10000.0f;  // min_cost's initial value (:120): a cost above it never wins
   int best_s = -1;
   const int ns = nv * nw;
   for (int s = lane; s < ns; s += 32) {
     const int iv = s / nw;
-    const float v = s_v[warp][iv], w = s_w[warp][s - iv * nw];
+    const float v = s_v[iv], w = s_w[s - iv * nw];
     float st[5] = {x[0], x[1], x[2], x[3], x[4]};
     float dmin = d0;
     for (int k = 1; k <= n_steps; ++k) {  // calc_trajectory :63-74; obstacles on points 0, 2, 4, ... (:82)
       crb_dwa_motion(st, v, w, p.dt);
-      if (!(k & 1)) dmin = dwa_min_d2(dmin, st[0], st[1], s_ob, n_ob);
+      if (!(k & 1)) dmin = dwa_min_d2(dmin, st[0], st[1], ob, n_ob);
     }
     // calc_to_goal_cost :103-113: std::pow(float, 2) promotes to double
     const float tmag = (float)sqrt((double)st[0] * (double)st[0] + (double)st[1] * (double)st[1]);
@@ -166,13 +163,14 @@ crb_dwa_control_kernel(int64_t n, const float* __restrict__ xg, float* __restric
     }
   }
   const int biv = best_s >= 0 ? best_s / nw : 0;
-  const float bv = best_s >= 0 ? s_v[warp][biv] : 0.0f;
-  const float bw = best_s >= 0 ? s_w[warp][best_s - biv * nw] : u_prev1;
+  const float bv = best_s >= 0 ? s_v[biv] : 0.0f;
+  const float bw = best_s >= 0 ? s_w[best_s - biv * nw] : u_prev1;
   if (lane == 0) {
     ug[i] = bv;
     ug[n + i] = bw;
     if (costg) costg[i] = best_c;
     if (bestg) bestg[i] = best_s;
+    if (statusg) statusg[i] = CRB_DWA_OK;
   }
   if (trajg) {
     if (best_s < 0) {
@@ -190,12 +188,28 @@ crb_dwa_control_kernel(int64_t n, const float* __restrict__ xg, float* __restric
   }
 }
 
-// dwa_control with an obstacle list per robot (crb.h's obstacle store, checked by crb_obstacle_list).  The
-// same mapping as above, except that each warp stages its own robot's list into its own slice of shared memory, so
-// dwa_min_d2 reads one address across the warp (a broadcast).  A robot whose list reference is bad gets NaN u, cost
-// and traj, best -1 and CRB_DWA_BAD_OBSTACLES; nothing of the store past ob_of[i] and two offsets is read for it.
-// With every robot on one list this kernel took 7.7 % longer than crb_dwa_control_kernel on an H100 (DESIGN.md §3),
-// so the shared-list entry point keeps that kernel.
+__global__ void __launch_bounds__(DWA_BLOCK)
+crb_dwa_control_kernel(int64_t n, const float* __restrict__ xg, float* __restrict__ ug,
+                       const float* __restrict__ goalg, const float* __restrict__ obg, int n_ob,
+                       crb_dwa_params p, int n_steps, float* __restrict__ costg, int32_t* __restrict__ bestg,
+                       float* __restrict__ trajg) {
+  __shared__ float2 s_ob[CRB_DWA_MAX_OBSTACLES];
+  __shared__ float s_v[DWA_WARPS][CRB_DWA_MAX_SPEED_SAMPLES];
+  __shared__ float s_w[DWA_WARPS][CRB_DWA_MAX_YAWRATE_SAMPLES];
+  for (int k = threadIdx.x; k < n_ob; k += DWA_BLOCK) s_ob[k] = make_float2(obg[2 * k], obg[2 * k + 1]);
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t i = (int64_t)blockIdx.x * DWA_WARPS + warp;
+  if (i >= n) return;  // whole warps leave together
+  dwa_robot(n, i, lane, s_ob, n_ob, s_v[warp], s_w[warp], xg, ug, goalg, p, n_steps, costg, bestg, trajg, nullptr);
+}
+
+// dwa_control with an obstacle list per robot (crb.h's obstacle store, checked by crb_obstacle_list): the same body,
+// except that each warp stages its own robot's list into its own slice of shared memory, so dwa_min_d2 reads one
+// address across the warp (a broadcast).  A robot whose list reference is bad gets NaN u, cost and traj, best -1 and
+// CRB_DWA_BAD_OBSTACLES; nothing of the store past ob_of[i] and two offsets is read for it.  With every robot on one
+// list this kernel took 7.7 % longer than crb_dwa_control_kernel on an H100 (DESIGN.md §3), so the shared-list entry
+// point keeps that kernel.
 __global__ void __launch_bounds__(DWA_BLOCK)
 crb_dwa_control_many_kernel(int64_t n, const float* __restrict__ xg, float* __restrict__ ug,
                             const float* __restrict__ goalg, const float* __restrict__ obg, int64_t n_rows,
@@ -225,87 +239,7 @@ crb_dwa_control_many_kernel(int64_t n, const float* __restrict__ xg, float* __re
   const int n_ob = (int)(ob1 - ob0);
   float2* ob = s_ob[warp];
   for (int k = lane; k < n_ob; k += 32) ob[k] = make_float2(obg[2 * (ob0 + k)], obg[2 * (ob0 + k) + 1]);
-  float x[5];
-#pragma unroll
-  for (int f = 0; f < 5; ++f) x[f] = xg[(int64_t)f * n + i];
-  const float gx = goalg[i], gy = goalg[n + i];
-  const float u_prev1 = ug[n + i];
-
-  // calc_dynamic_window :52-60; std::max(a, b) is (a < b) ? b : a and std::min(a, b) is (b < a) ? b : a
-  const float lv = x[3] - p.max_accel * p.dt, hv = x[3] + p.max_accel * p.dt;
-  const float lw = x[4] - p.max_dyawrate * p.dt, hw = x[4] + p.max_dyawrate * p.dt;
-  const float dw0 = (lv < p.min_speed) ? p.min_speed : lv;
-  const float dw1 = (p.max_speed < hv) ? p.max_speed : hv;
-  const float dw2 = (lw < -p.max_yawrate) ? -p.max_yawrate : lw;
-  const float dw3 = (p.max_yawrate < hw) ? p.max_yawrate : hw;
-  // the sample grid :126-127: the k-th value is k sequential float adds (every lane runs the sequence, each
-  // stores its own entries)
-  int nv = 0, nw = 0;
-  for (float v = dw0; nv < CRB_DWA_MAX_SPEED_SAMPLES && v <= dw1; v = v + p.v_reso, ++nv)
-    if ((nv & 31) == lane) s_v[warp][nv] = v;
-  for (float w = dw2; nw < CRB_DWA_MAX_YAWRATE_SAMPLES && w <= dw3; w = w + p.yawrate_reso, ++nw)
-    if ((nw & 31) == lane) s_w[warp][nw] = w;
-  __syncwarp();  // the grids and the obstacle slice
-
-  const float d0 = dwa_min_d2(__int_as_float(0x7fffffff), x[0], x[1], ob, n_ob);  // point 0 is x itself
-  const float gmag = sqrtf(gx * gx + gy * gy);
-  float best_c = 10000.0f;  // min_cost's initial value (:120): a cost above it never wins
-  int best_s = -1;
-  const int ns = nv * nw;
-  for (int s = lane; s < ns; s += 32) {
-    const int iv = s / nw;
-    const float v = s_v[warp][iv], w = s_w[warp][s - iv * nw];
-    float st[5] = {x[0], x[1], x[2], x[3], x[4]};
-    float dmin = d0;
-    for (int k = 1; k <= n_steps; ++k) {  // calc_trajectory :63-74; obstacles on points 0, 2, 4, ... (:82)
-      crb_dwa_motion(st, v, w, p.dt);
-      if (!(k & 1)) dmin = dwa_min_d2(dmin, st[0], st[1], ob, n_ob);
-    }
-    // calc_to_goal_cost :103-113: std::pow(float, 2) promotes to double
-    const float tmag = (float)sqrt((double)st[0] * (double)st[0] + (double)st[1] * (double)st[1]);
-    const float dot = gx * st[0] + gy * st[1];
-    const float to_goal = p.to_goal_cost_gain * crb_dwa_acosf(dot / (gmag * tmag));
-    const float speed = p.speed_cost_gain * (p.max_speed - st[3]);
-    const float cost = to_goal + speed + dwa_obstacle_cost(dmin, p.robot_radius);
-    if (cost <= best_c) {  // `min_cost >= final_cost` (:136): within a lane s increases, so ties go to the later
-      best_c = cost;
-      best_s = s;
-    }
-  }
-  // across lanes: the smaller cost, on a tie the larger index (= the reference's last-wins); NaN never got in
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) {
-    const float oc = __shfl_xor_sync(0xffffffffu, best_c, off);
-    const int os = __shfl_xor_sync(0xffffffffu, best_s, off);
-    if (oc < best_c || (oc == best_c && os > best_s)) {
-      best_c = oc;
-      best_s = os;
-    }
-  }
-  const int biv = best_s >= 0 ? best_s / nw : 0;
-  const float bv = best_s >= 0 ? s_v[warp][biv] : 0.0f;
-  const float bw = best_s >= 0 ? s_w[warp][best_s - biv * nw] : u_prev1;
-  if (lane == 0) {
-    ug[i] = bv;
-    ug[n + i] = bw;
-    if (costg) costg[i] = best_c;
-    if (bestg) bestg[i] = best_s;
-    if (statusg) statusg[i] = CRB_DWA_OK;
-  }
-  if (trajg) {
-    if (best_s < 0) {
-      for (int f = lane; f < 5 * (n_steps + 1); f += 32) trajg[(int64_t)f * n + i] = __int_as_float(0x7fc00000);
-    } else {
-      float st[5] = {x[0], x[1], x[2], x[3], x[4]};
-      for (int k = 0; k <= n_steps; ++k) {
-        if (k > 0) crb_dwa_motion(st, bv, bw, p.dt);
-        if ((k & 31) == lane) {
-#pragma unroll
-          for (int j = 0; j < 5; ++j) trajg[(int64_t)(5 * k + j) * n + i] = st[j];
-        }
-      }
-    }
-  }
+  dwa_robot(n, i, lane, ob, n_ob, s_v[warp], s_w[warp], xg, ug, goalg, p, n_steps, costg, bestg, trajg, statusg);
 }
 
 __global__ void __launch_bounds__(256)
@@ -368,18 +302,6 @@ static int dwa_check_params(const crb_dwa_params* p, int* n_steps) {
   return CRB_OK;
 }
 
-// No device, no computation: the entry points say so after validating their arguments (no CPU fallback).
-static int dwa_require_device(const char* fn) {
-  int count = 0;
-  const cudaError_t e = cudaGetDeviceCount(&count);
-  if (e != cudaSuccess || count == 0) {
-    cudaGetLastError();
-    crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", fn);
-    return CRB_ERR_NO_DEVICE;
-  }
-  return CRB_OK;
-}
-
 extern "C" {
 
 void crb_dwa_default_params(crb_dwa_params* p) {
@@ -419,7 +341,7 @@ int crb_dwa_control_batched(crb_ctx* ctx, int64_t n, const float* x, float* u, c
   int n_steps = 0;
   int rc = dwa_check_params(prm, &n_steps);
   if (rc != CRB_OK) return rc;
-  if ((rc = dwa_require_device(__func__)) != CRB_OK) return rc;
+  if ((rc = crb_require_device(__func__)) != CRB_OK) return rc;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);
   crb_dwa_control_kernel<<<(unsigned)((n + DWA_WARPS - 1) / DWA_WARPS), DWA_BLOCK, 0, ctx->stream>>>(
@@ -441,7 +363,7 @@ int crb_dwa_control_many_batched(crb_ctx* ctx, int64_t n, const float* x, float*
   int n_steps = 0;
   int rc = dwa_check_params(prm, &n_steps);
   if (rc != CRB_OK) return rc;
-  if ((rc = dwa_require_device(__func__)) != CRB_OK) return rc;
+  if ((rc = crb_require_device(__func__)) != CRB_OK) return rc;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);
   crb_dwa_control_many_kernel<<<(unsigned)((n + DWA_WARPS - 1) / DWA_WARPS), DWA_BLOCK, 0, ctx->stream>>>(
@@ -456,7 +378,7 @@ int crb_dwa_motion_batched(crb_ctx* ctx, int64_t n, float* x, const float* u, fl
   CRB_REQUIRE(n >= 0 && (n + 255) / 256 <= 0x7fffffff, "n out of range");
   CRB_REQUIRE(n == 0 || (x && u), "x or u is NULL");
   CRB_REQUIRE(finite_pos(dt), "dt must be finite and > 0");
-  const int rc = dwa_require_device(__func__);
+  const int rc = crb_require_device(__func__);
   if (rc != CRB_OK) return rc;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);

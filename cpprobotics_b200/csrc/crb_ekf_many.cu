@@ -140,14 +140,8 @@ extern "C" int crb_ekf_step_many_batched(crb_ctx* ctx, int64_t n, float* x, floa
   if (n == 0) return CRB_OK;
   CRB_REQUIRE(x && P && z && u, "NULL array");
   CRB_REQUIRE(models && model_of, "NULL model table or model_of");
-  {   // a usable device, or CRB_ERR_NO_DEVICE (valid arguments on a machine without one)
-    int count = 0;
-    if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
-      cudaGetLastError();
-      crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", __func__);
-      return CRB_ERR_NO_DEVICE;
-    }
-  }
+  const int rc = crb_require_device(__func__);
+  if (rc != CRB_OK) return rc;
   CRB_DEVICE_GUARD(ctx);   // ctx->device is current for this call, the caller's device is restored after it
   return ekf_many_launch(ctx, ctx->stream, n, n, x, P, z, u, n, n_steps, models, n_models, model_of, status);
 }

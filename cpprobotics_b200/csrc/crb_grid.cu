@@ -22,9 +22,6 @@
 //     and the parent of a cell is cell - offset[move], so no pointer or parent array is kept.
 #include "crb_grid_common.cuh"
 
-#define GRID_MAP_BLOCK 256
-#define GRID_PLAN_BLOCK 128
-
 __global__ void __launch_bounds__(GRID_MAP_BLOCK)
 crb_grid_map_kernel(int64_t n_obs, const float* __restrict__ ox, const float* __restrict__ oy, float reso, float thr,
                     crb_grid_box box, int64_t cells, uint8_t* __restrict__ map) {
@@ -33,25 +30,7 @@ crb_grid_map_kernel(int64_t n_obs, const float* __restrict__ ox, const float* __
   const int64_t c = (int64_t)blockIdx.x * GRID_MAP_BLOCK + threadIdx.x;
   const int64_t H = (int64_t)box.max_y - box.min_y;
   const int64_t x = c < cells ? box.min_x + c / H : 0, y = c < cells ? box.min_y + c % H : 0;
-  bool blocked = false;
-  for (int64_t k0 = 0; k0 < n_obs; k0 += GRID_MAP_BLOCK) {
-    const int64_t k = k0 + threadIdx.x;
-    int ix = 0, iy = 0;
-    const bool ok = k < n_obs && grid_cell_d(ox[k], reso, ix) && grid_cell_d(oy[k], reso, iy);
-    __syncthreads();  // the previous tile is no longer read
-    s_ob[threadIdx.x] = make_int2(ix, iy);
-    s_ok[threadIdx.x] = ok;
-    __syncthreads();
-    const int m = n_obs - k0 < GRID_MAP_BLOCK ? (int)(n_obs - k0) : GRID_MAP_BLOCK;
-    for (int j = 0; j < m && !blocked; ++j) {
-      if (!s_ok[j]) continue;
-      // std::sqrt(std::pow(ox - x, 2) + std::pow(oy - y, 2)) in double, narrowed to the float d; the squares of
-      // integer differences are exact
-      const double dx = (double)(s_ob[j].x - x), dy = (double)(s_ob[j].y - y);
-      const float d = __double2float_rn(__dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy))));
-      blocked = d <= thr;
-    }
-  }
+  const bool blocked = grid_cell_blocked(x, y, n_obs, ox, oy, 1, reso, thr, s_ob, s_ok);
   if (c < cells) map[c] = blocked ? 1 : 0;
 }
 
@@ -59,14 +38,7 @@ struct GridPlanArgs {
   crb_grid_box box;
   const uint8_t* map;
   float reso;
-  int64_t n;
-  const float* sg;
-  int max_pts;
-  float* path;
-  int32_t* path_len;
-  float* cost;
-  int32_t* n_visited;
-  int32_t* status;
+  GridQueries q;
   unsigned long long* counter;
   char* ws;
   size_t slot_bytes;
@@ -82,105 +54,13 @@ __global__ void __launch_bounds__(GRID_PLAN_BLOCK) crb_grid_plan_kernel(const Gr
   Entry* heap = (Entry*)(slot + a.heap_off);
   float* g = (float*)(slot + a.g_off);
   uint8_t* st = (uint8_t*)(slot + a.state_off);
-  const int64_t n = a.n;
+  const int64_t n = a.q.n;
   const int W = a.box.max_x - a.box.min_x, H = a.box.max_y - a.box.min_y;
   const int64_t cells = (int64_t)W * H;
   for (;;) {
     const int64_t q = (int64_t)atomicAdd(a.counter, 1ull);
     if (q >= n) return;
-    int sx, sy, gx, gy;
-    int32_t status = CRB_GRID_NO_PATH, nvis = 0, plen = 0;
-    float cost = grid_nan();
-    if (!(grid_cell_f(a.sg[q], a.reso, sx) && grid_cell_f(a.sg[n + q], a.reso, sy) &&
-          grid_cell_f(a.sg[2 * n + q], a.reso, gx) && grid_cell_f(a.sg[3 * n + q], a.reso, gy))) {
-      status = CRB_GRID_BAD_POINT;
-    } else {
-      // box-relative cells (64-bit: a cell far outside the box must not wrap into it)
-      const int64_t rsx = (int64_t)sx - a.box.min_x, rsy = (int64_t)sy - a.box.min_y;
-      const int64_t rgx = (int64_t)gx - a.box.min_x, rgy = (int64_t)gy - a.box.min_y;
-      if (rsx < 0 || rsx >= W || rsy < 0 || rsy >= H) {
-        status = CRB_GRID_START_OUTSIDE;
-      } else {
-        const bool goal_in = rgx >= 0 && rgx < W && rgy >= 0 && rgy < H;
-        const int64_t goal_cell = goal_in ? rgx * H + rgy : -1;
-        // fresh cell state (and path costs) for this query, 16 bytes per store
-        {
-          uint4* s4 = (uint4*)st;
-          const int64_t n4 = (cells + 15) / 16;
-          for (int64_t i = 0; i < n4; ++i) s4[i] = make_uint4(0u, 0u, 0u, 0u);
-          if (ALGO == CRB_GRID_ASTAR) {
-            const uint32_t fm = __float_as_uint(FLT_MAX);
-            uint4* g4 = (uint4*)g;
-            const int64_t m4 = (cells + 3) / 4;
-            for (int64_t i = 0; i < m4; ++i) g4[i] = make_uint4(fm, fm, fm, fm);
-          }
-        }
-        const int64_t start = rsx * H + rsy;
-        if (ALGO == CRB_GRID_ASTAR) g[start] = 0.0f;
-        int64_t len = 0;
-        heap_push(heap, len, Entry{0.0f, (uint32_t)start << 3});
-        bool first = true;
-        while (len > 0) {
-          const Entry e = heap_pop(heap, len);
-          const int64_t cell = e.cd >> 3;
-          if (st[cell] & 0x80) continue;  // a duplicate of a visited cell
-          st[cell] = first ? 0x88 : (uint8_t)(0x80 | (e.cd & 7));
-          first = false;
-          ++nvis;
-          if (cell == goal_cell) {
-            status = CRB_GRID_FOUND;
-            cost = e.key;
-            break;
-          }
-          const int cx = (int)(cell / H), cy = (int)(cell - (int64_t)cx * H);
-          float gc = 0.0f, h = 0.0f;
-          if (ALGO == CRB_GRID_ASTAR) {
-            gc = g[cell];
-            // calc_heristic(ngoal, node): w * std::sqrt(pow(dx, 2) + pow(dy, 2)) in double (w = 1), narrowed
-            const double dx = (double)(rgx - cx), dy = (double)(rgy - cy);
-            h = __double2float_rn(__dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy))));
-          }
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int nx = cx + c_mx[i], ny = cy + c_my[i];
-            if (nx < 0 || nx >= W || ny < 0 || ny >= H) continue;  // verify_node: the box
-            const int64_t nc = (int64_t)nx * H + ny;
-            if (__ldg(a.map + nc)) continue;                        // verify_node: the map
-            if (st[nc] & 0x80) continue;                            // visited
-            const float step = i < 4 ? 1.0f : kDiag;
-            if (ALGO == CRB_GRID_ASTAR) {
-              const float ng = __fadd_rn(gc, step);
-              if (ng < g[nc]) {
-                g[nc] = ng;
-                heap_push(heap, len, Entry{__fadd_rn(ng, h), ((uint32_t)nc << 3) | (uint32_t)i});
-              }
-            } else {
-              heap_push(heap, len, Entry{__fadd_rn(e.key, step), ((uint32_t)nc << 3) | (uint32_t)i});
-            }
-          }
-        }
-        if (status == CRB_GRID_FOUND) {
-          // calc_final_path: the goal, then parent after parent down to the start
-          int64_t c = goal_cell;
-          for (;;) {
-            if (a.path && plen < a.max_pts) {
-              const int x = (int)(c / H), y = (int)(c - (c / H) * H);
-              a.path[(2 * (int64_t)plen) * n + q] = __fmul_rn(__int2float_rn(x + a.box.min_x), a.reso);
-              a.path[(2 * (int64_t)plen + 1) * n + q] = __fmul_rn(__int2float_rn(y + a.box.min_y), a.reso);
-            }
-            ++plen;
-            const uint8_t s = st[c];
-            if (s & 0x08) break;
-            c -= (int64_t)c_mx[s & 7] * H + c_my[s & 7];
-          }
-        }
-      }
-    }
-    if (status != CRB_GRID_FOUND) plen = 0;
-    if (a.path_len) a.path_len[q] = plen;
-    if (a.cost) a.cost[q] = cost;
-    if (a.n_visited) a.n_visited[q] = status == CRB_GRID_NO_PATH || status == CRB_GRID_FOUND ? nvis : 0;
-    if (a.status) a.status[q] = status;
+    grid_plan_query<ALGO>(a.q, n, q, true, a.box, W, H, cells, a.reso, a.map, heap, g, st);
   }
 }
 
@@ -207,52 +87,20 @@ bool grid_box_dims(const crb_grid_box* b, const char* fn, int64_t& W, int64_t& H
 
 bool grid_reso_ok(float reso) { return isfinite(reso) && reso > 0.0f; }
 
-}  // namespace
-
-int crb_grid_require_device(const char* fn) {
-  int count = 0;
-  const cudaError_t e = cudaGetDeviceCount(&count);
-  if (e != cudaSuccess || count == 0) {
-    cudaGetLastError();
-    crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", fn);
-    return CRB_ERR_NO_DEVICE;
-  }
-  return CRB_OK;
-}
-
-namespace {
-
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-// slot layout: heap | g (A* only) | state, each 256-byte aligned
-void grid_slot_layout(int algo, int64_t cells, int64_t& heap_off, int64_t& g_off, int64_t& state_off,
-                      size_t& slot_bytes) {
-  heap_off = 0;
-  g_off = (int64_t)align_up((size_t)(8 * cells + 1) * sizeof(Entry), 256);
-  state_off = g_off + (algo == CRB_GRID_ASTAR ? (int64_t)align_up((size_t)cells * sizeof(float), 256) : 0);
-  slot_bytes = align_up((size_t)state_off + (size_t)cells, 256);
-}
-
-int grid_slots(crb_ctx* ctx, int algo, int64_t cells, int64_t n, int64_t& slots, size_t& slot_bytes,
-               int64_t* offs) {
+int grid_slots(crb_ctx* ctx, int algo, int64_t cells, int64_t n, int64_t& slots, int64_t& slot_bytes) {
   int per_sm = 0;
   CRB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(
       &per_sm, algo == CRB_GRID_ASTAR ? (const void*)crb_grid_plan_kernel<CRB_GRID_ASTAR>
                                       : (const void*)crb_grid_plan_kernel<CRB_GRID_DIJKSTRA>,
       GRID_PLAN_BLOCK, 0));
-  int64_t ho, go, so;
-  grid_slot_layout(algo, cells, ho, go, so, slot_bytes);
+  int64_t go, so;
+  grid_slot_layout(algo == CRB_GRID_ASTAR, cells, go, so, slot_bytes);
   const int64_t resident = (int64_t)(per_sm > 0 ? per_sm : 1) * GRID_PLAN_BLOCK * ctx->sm_count;
-  int64_t by_budget = (int64_t)(CRB_GRID_WS_BUDGET / slot_bytes);
+  int64_t by_budget = (int64_t)(CRB_GRID_WS_BUDGET / (size_t)slot_bytes);
   if (by_budget < 1) by_budget = 1;
   slots = n < resident ? n : resident;
   if (slots > by_budget) slots = by_budget;
   if (slots < 1) slots = 1;
-  if (offs) {
-    offs[0] = ho;
-    offs[1] = go;
-    offs[2] = so;
-  }
   return CRB_OK;
 }
 
@@ -312,7 +160,7 @@ int crb_grid_obstacle_map(crb_ctx* ctx, int64_t n_obs, const float* ox, const fl
   int64_t W, H;
   if (!grid_box_dims(box, __func__, W, H)) return CRB_ERR_INVALID_ARG;
   CRB_REQUIRE(map != nullptr && (n_obs == 0 || (ox && oy)), "ox, oy or map is NULL");
-  const int rc = crb_grid_require_device(__func__);
+  const int rc = crb_require_device(__func__);
   if (rc != CRB_OK) return rc;
   CRB_DEVICE_GUARD(ctx);
   const int64_t cells = W * H;
@@ -331,11 +179,11 @@ int crb_grid_plan_slots(crb_ctx* ctx, int algo, const crb_grid_box* box, int64_t
   CRB_REQUIRE(n >= 0, "n must be >= 0");
   int64_t W, H;
   if (!grid_box_dims(box, __func__, W, H)) return CRB_ERR_INVALID_ARG;
-  const int rc = crb_grid_require_device(__func__);
+  const int rc = crb_require_device(__func__);
   if (rc != CRB_OK) return rc;
   CRB_DEVICE_GUARD(ctx);
-  size_t sb;
-  return grid_slots(ctx, algo, W * H, n, *slots, sb, nullptr);
+  int64_t sb;
+  return grid_slots(ctx, algo, W * H, n, *slots, sb);
 }
 
 int crb_grid_plan_batched(crb_ctx* ctx, int algo, const crb_grid_box* box, const uint8_t* map, float reso, int64_t n,
@@ -351,7 +199,7 @@ int crb_grid_plan_batched(crb_ctx* ctx, int algo, const crb_grid_box* box, const
   if (!grid_box_dims(box, __func__, W, H)) return CRB_ERR_INVALID_ARG;
   CRB_REQUIRE(n == 0 || (map && sg), "map or sg is NULL");
   CRB_REQUIRE(n == 0 || max_pts == 0 || path, "path is NULL with max_pts > 0");
-  const int rc = crb_grid_require_device(__func__);
+  const int rc = crb_require_device(__func__);
   if (rc != CRB_OK) return rc;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);
@@ -359,20 +207,13 @@ int crb_grid_plan_batched(crb_ctx* ctx, int algo, const crb_grid_box* box, const
   a.box = *box;
   a.map = map;
   a.reso = reso;
-  a.n = n;
-  a.sg = sg;
-  a.max_pts = max_pts;
-  a.path = max_pts > 0 ? path : nullptr;
-  a.path_len = path_len;
-  a.cost = cost;
-  a.n_visited = n_visited;
-  a.status = status;
-  int64_t offs[3];
-  int r = grid_slots(ctx, algo, W * H, n, a.slots, a.slot_bytes, offs);
+  a.q = GridQueries{n, sg, max_pts, max_pts > 0 ? path : nullptr, path_len, cost, n_visited, status};
+  int64_t slot_bytes;
+  int r = grid_slots(ctx, algo, W * H, n, a.slots, slot_bytes);
   if (r != CRB_OK) return r;
-  a.heap_off = offs[0];
-  a.g_off = offs[1];
-  a.state_off = offs[2];
+  a.slot_bytes = (size_t)slot_bytes;
+  a.heap_off = 0;
+  grid_slot_layout(algo == CRB_GRID_ASTAR, W * H, a.g_off, a.state_off, slot_bytes);
   r = crb_grid_ws_reserve(ctx, 256 + (size_t)a.slots * a.slot_bytes);
   if (r != CRB_OK) return r;
   a.counter = (unsigned long long*)ctx->grid_ws;

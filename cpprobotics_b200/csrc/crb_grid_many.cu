@@ -2,11 +2,11 @@
 // launch, and a_star_planning / dijkstra_star_planning for queries that each name their own map.
 //
 // The maps live back to back in one byte store described by a map table (crb.h): boxes, reso and map_off per map.
-// Every entry is device data, checked on the device before anything it points at is read.  The kernels are
-// crb_grid.cu's, generalised to read their box, resolution and map from the table (the computation, the heap and the
-// rounding are the same code, crb_grid_common.cuh), so each map and each query's outputs are bitwise those of the
-// single-map entry points on that map.  crb_grid.cu's kernels are kept as they were for the single-map entry points:
-// with every query on one map, these kernels took 0.4 % longer on the scatter 128^2 map with Dijkstra, beyond the
+// Every entry is device data, checked on the device before anything it points at is read.  Each kernel runs the same
+// per-cell and per-query body as crb_grid.cu's (grid_cell_blocked and grid_plan_query, crb_grid_common.cuh) and
+// differs only in reading its box, resolution and map from the table, so each map and each query's outputs are
+// bitwise those of the single-map entry points on that map.  The single-map entry points keep their own kernels: with
+// every query on one map, these kernels took 0.4 % longer on the scatter 128^2 map with Dijkstra, beyond the
 // run-to-run spread of 0.2 %, on an H100 (DESIGN.md §3).
 //
 // Mapping.
@@ -15,9 +15,6 @@
 //   crb_grid_plan_many_kernel: crb_grid_plan_kernel's persistent lanes and slots; the slots are sized for the call's
 //     max_cells, and each query lays its slot out (heap 8 * W * H + 1 entries, A*'s g, state) for its own map.
 #include "crb_grid_common.cuh"
-
-#define GRID_MAP_BLOCK 256
-#define GRID_PLAN_BLOCK 128
 
 namespace {
 
@@ -48,15 +45,6 @@ __device__ __forceinline__ bool grid_table_entry(const GridTable& t, int64_t m, 
   return true;
 }
 
-// Slot layout: heap | g (A* only) | state, each 256-byte aligned, for a map of `cells` cells.  A query lays its slot
-// out for its own map; the host sizes the slots for the largest map a call may use.
-__host__ __device__ __forceinline__ void grid_slot_layout(bool astar, int64_t cells, int64_t& g_off, int64_t& state_off,
-                                                          int64_t& slot_bytes) {
-  g_off = ((8 * cells + 1) * (int64_t)sizeof(Entry) + 255) / 256 * 256;
-  state_off = g_off + (astar ? (cells * (int64_t)sizeof(float) + 255) / 256 * 256 : 0);
-  slot_bytes = (state_off + cells + 255) / 256 * 256;
-}
-
 }  // namespace
 
 struct GridMapArgs {
@@ -71,7 +59,7 @@ struct GridMapArgs {
   int32_t* map_status;
 };
 
-// crb_grid_map_kernel's computation, block (tile, m) building the cells [256 * tile, 256 * tile + 256) of map m:
+// calc_obstacle_map, block (tile, m) building the cells [256 * tile, 256 * tile + 256) of map m:
 // gridDim.y blocks stride over the maps and block (0, m) writes map m's status.  Blocks past a map's cells, and every
 // block of a bad entry, leave at once; nothing of a map is read before its entry and list reference are checked.
 __global__ void __launch_bounds__(GRID_MAP_BLOCK) crb_grid_map_many_kernel(const GridMapArgs a) {
@@ -95,25 +83,7 @@ __global__ void __launch_bounds__(GRID_MAP_BLOCK) crb_grid_map_many_kernel(const
     const float* ob = a.ob + 2 * ob0;
     const int64_t c = (int64_t)blockIdx.x * GRID_MAP_BLOCK + threadIdx.x;
     const int64_t x = c < cells ? box.min_x + c / H : 0, y = c < cells ? box.min_y + c % H : 0;
-    bool blocked = false;
-    for (int64_t k0 = 0; k0 < n_obs; k0 += GRID_MAP_BLOCK) {
-      const int64_t k = k0 + threadIdx.x;
-      int ix = 0, iy = 0;
-      const bool ok = k < n_obs && grid_cell_d(ob[2 * k], reso, ix) && grid_cell_d(ob[2 * k + 1], reso, iy);
-      __syncthreads();  // the previous tile is no longer read
-      s_ob[threadIdx.x] = make_int2(ix, iy);
-      s_ok[threadIdx.x] = ok;
-      __syncthreads();
-      const int m = n_obs - k0 < GRID_MAP_BLOCK ? (int)(n_obs - k0) : GRID_MAP_BLOCK;
-      for (int j = 0; j < m && !blocked; ++j) {
-        if (!s_ok[j]) continue;
-        // std::sqrt(std::pow(ox - x, 2) + std::pow(oy - y, 2)) in double, narrowed to the float d; the squares of
-        // integer differences are exact
-        const double dx = (double)(s_ob[j].x - x), dy = (double)(s_ob[j].y - y);
-        const float d = __double2float_rn(__dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy))));
-        blocked = d <= thr;
-      }
-    }
+    const bool blocked = grid_cell_blocked(x, y, n_obs, ob, ob + 1, 2, reso, thr, s_ob, s_ok);
     if (c < cells) a.maps[off + c] = blocked ? 1 : 0;
   }
 }
@@ -122,29 +92,22 @@ struct GridPlanManyArgs {
   const uint8_t* maps;
   GridTable t;
   const int32_t* map_of;  // [n] the map of each query
-  int64_t n;
-  const float* sg;
-  int max_pts;
-  float* path;
-  int32_t* path_len;
-  float* cost;
-  int32_t* n_visited;
-  int32_t* status;
+  GridQueries q;
   unsigned long long* counter;
   char* ws;
   int64_t slot_bytes;
   int64_t slots;
 };
 
-// crb_grid_plan_kernel's search, each query on its own map: the entry is checked before the map is read, and the slot
-// (sized by the host for max_cells) is laid out for the query's own W * H.  __maxnreg__(56) (launched with
+// The search, each query on its own map: the entry is checked before the map is read, and the slot (sized by the host
+// for max_cells) is laid out for the query's own W * H.  __maxnreg__(56) (launched with
 // GRID_PLAN_BLOCK threads) keeps A* from the 16-byte spill ptxas otherwise chooses at 48 registers.
 template <int ALGO>
 __global__ void __maxnreg__(56) crb_grid_plan_many_kernel(const GridPlanManyArgs a) {
   const int64_t lane = (int64_t)blockIdx.x * GRID_PLAN_BLOCK + threadIdx.x;
   if (lane >= a.slots) return;
   char* slot = a.ws + lane * a.slot_bytes;
-  const int64_t n = a.n;
+  const int64_t n = a.q.n;
   for (;;) {
     const int64_t q = (int64_t)atomicAdd(a.counter, 1ull);
     if (q >= n) return;
@@ -157,104 +120,8 @@ __global__ void __maxnreg__(56) crb_grid_plan_many_kernel(const GridPlanManyArgs
     const int64_t cells = (int64_t)W * H;
     int64_t g_off, state_off, slot_end;
     grid_slot_layout(ALGO == CRB_GRID_ASTAR, cells, g_off, state_off, slot_end);
-    Entry* heap = (Entry*)slot;
-    float* g = (float*)(slot + g_off);
-    uint8_t* st = (uint8_t*)(slot + state_off);
-    int sx, sy, gx, gy;
-    int32_t status = CRB_GRID_NO_PATH, nvis = 0, plen = 0;
-    float cost = grid_nan();
-    if (!map_ok) {
-      status = CRB_GRID_BAD_MAP;
-    } else if (!(grid_cell_f(a.sg[q], reso, sx) && grid_cell_f(a.sg[n + q], reso, sy) &&
-                 grid_cell_f(a.sg[2 * n + q], reso, gx) && grid_cell_f(a.sg[3 * n + q], reso, gy))) {
-      status = CRB_GRID_BAD_POINT;
-    } else {
-      // box-relative cells (64-bit: a cell far outside the box must not wrap into it)
-      const int64_t rsx = (int64_t)sx - box.min_x, rsy = (int64_t)sy - box.min_y;
-      const int64_t rgx = (int64_t)gx - box.min_x, rgy = (int64_t)gy - box.min_y;
-      if (rsx < 0 || rsx >= W || rsy < 0 || rsy >= H) {
-        status = CRB_GRID_START_OUTSIDE;
-      } else {
-        const bool goal_in = rgx >= 0 && rgx < W && rgy >= 0 && rgy < H;
-        const int64_t goal_cell = goal_in ? rgx * H + rgy : -1;
-        // fresh cell state (and path costs) for this query, 16 bytes per store
-        {
-          uint4* s4 = (uint4*)st;
-          const int64_t n4 = (cells + 15) / 16;
-          for (int64_t i = 0; i < n4; ++i) s4[i] = make_uint4(0u, 0u, 0u, 0u);
-          if (ALGO == CRB_GRID_ASTAR) {
-            const uint32_t fm = __float_as_uint(FLT_MAX);
-            uint4* g4 = (uint4*)g;
-            const int64_t m4 = (cells + 3) / 4;
-            for (int64_t i = 0; i < m4; ++i) g4[i] = make_uint4(fm, fm, fm, fm);
-          }
-        }
-        const int64_t start = rsx * H + rsy;
-        if (ALGO == CRB_GRID_ASTAR) g[start] = 0.0f;
-        int64_t len = 0;
-        heap_push(heap, len, Entry{0.0f, (uint32_t)start << 3});
-        bool first = true;
-        while (len > 0) {
-          const Entry e = heap_pop(heap, len);
-          const int64_t cell = e.cd >> 3;
-          if (st[cell] & 0x80) continue;  // a duplicate of a visited cell
-          st[cell] = first ? 0x88 : (uint8_t)(0x80 | (e.cd & 7));
-          first = false;
-          ++nvis;
-          if (cell == goal_cell) {
-            status = CRB_GRID_FOUND;
-            cost = e.key;
-            break;
-          }
-          const int cx = (int)(cell / H), cy = (int)(cell - (int64_t)cx * H);
-          float gc = 0.0f, h = 0.0f;
-          if (ALGO == CRB_GRID_ASTAR) {
-            gc = g[cell];
-            // calc_heristic(ngoal, node): w * std::sqrt(pow(dx, 2) + pow(dy, 2)) in double (w = 1), narrowed
-            const double dx = (double)(rgx - cx), dy = (double)(rgy - cy);
-            h = __double2float_rn(__dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy))));
-          }
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int nx = cx + c_mx[i], ny = cy + c_my[i];
-            if (nx < 0 || nx >= W || ny < 0 || ny >= H) continue;  // verify_node: the box
-            const int64_t nc = (int64_t)nx * H + ny;
-            if (__ldg(map + nc)) continue;                          // verify_node: the map
-            if (st[nc] & 0x80) continue;                            // visited
-            const float step = i < 4 ? 1.0f : kDiag;
-            if (ALGO == CRB_GRID_ASTAR) {
-              const float ng = __fadd_rn(gc, step);
-              if (ng < g[nc]) {
-                g[nc] = ng;
-                heap_push(heap, len, Entry{__fadd_rn(ng, h), ((uint32_t)nc << 3) | (uint32_t)i});
-              }
-            } else {
-              heap_push(heap, len, Entry{__fadd_rn(e.key, step), ((uint32_t)nc << 3) | (uint32_t)i});
-            }
-          }
-        }
-        if (status == CRB_GRID_FOUND) {
-          // calc_final_path: the goal, then parent after parent down to the start
-          int64_t c = goal_cell;
-          for (;;) {
-            if (a.path && plen < a.max_pts) {
-              const int x = (int)(c / H), y = (int)(c - (c / H) * H);
-              a.path[(2 * (int64_t)plen) * n + q] = __fmul_rn(__int2float_rn(x + box.min_x), reso);
-              a.path[(2 * (int64_t)plen + 1) * n + q] = __fmul_rn(__int2float_rn(y + box.min_y), reso);
-            }
-            ++plen;
-            const uint8_t s = st[c];
-            if (s & 0x08) break;
-            c -= (int64_t)c_mx[s & 7] * H + c_my[s & 7];
-          }
-        }
-      }
-    }
-    if (status != CRB_GRID_FOUND) plen = 0;
-    if (a.path_len) a.path_len[q] = plen;
-    if (a.cost) a.cost[q] = cost;
-    if (a.n_visited) a.n_visited[q] = status == CRB_GRID_NO_PATH || status == CRB_GRID_FOUND ? nvis : 0;
-    if (a.status) a.status[q] = status;
+    grid_plan_query<ALGO>(a.q, n, q, map_ok, box, W, H, cells, reso, map, (Entry*)slot, (float*)(slot + g_off),
+                          (uint8_t*)(slot + state_off));
   }
 }
 
@@ -300,7 +167,7 @@ int crb_grid_obstacle_map_many(crb_ctx* ctx, const float* ob, int64_t n_rows, co
   CRB_REQUIRE(boxes && reso && map_off, "boxes, reso or map_off is NULL");
   CRB_REQUIRE(ob_off && ob_of && rr && (ob || n_rows == 0), "ob, ob_off, ob_of or rr is NULL");
   CRB_REQUIRE(maps || n_cells == 0, "maps is NULL");
-  const int rc = crb_grid_require_device(__func__);
+  const int rc = crb_require_device(__func__);
   if (rc != CRB_OK) return rc;
   CRB_DEVICE_GUARD(ctx);
   GridMapArgs a = {};
@@ -325,7 +192,7 @@ int crb_grid_plan_many_slots(crb_ctx* ctx, int algo, int64_t max_cells, int64_t 
   CRB_REQUIRE(algo == CRB_GRID_ASTAR || algo == CRB_GRID_DIJKSTRA, "algo must be CRB_GRID_ASTAR or CRB_GRID_DIJKSTRA");
   CRB_REQUIRE(n >= 0, "n must be >= 0");
   CRB_REQUIRE(max_cells >= 1 && max_cells <= CRB_GRID_MAX_CELLS, "max_cells must be in [1, CRB_GRID_MAX_CELLS]");
-  const int rc = crb_grid_require_device(__func__);
+  const int rc = crb_require_device(__func__);
   if (rc != CRB_OK) return rc;
   CRB_DEVICE_GUARD(ctx);
   int64_t sb;
@@ -345,7 +212,7 @@ int crb_grid_plan_many_batched(crb_ctx* ctx, int algo, const crb_grid_box* boxes
   CRB_REQUIRE(n == 0 || (boxes && reso && map_off && map_of && sg), "boxes, reso, map_off, map_of or sg is NULL");
   CRB_REQUIRE(n == 0 || n_cells == 0 || maps, "maps is NULL");
   CRB_REQUIRE(n == 0 || max_pts == 0 || path, "path is NULL with max_pts > 0");
-  const int rc = crb_grid_require_device(__func__);
+  const int rc = crb_require_device(__func__);
   if (rc != CRB_OK) return rc;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);
@@ -353,14 +220,7 @@ int crb_grid_plan_many_batched(crb_ctx* ctx, int algo, const crb_grid_box* boxes
   a.maps = maps;
   a.t = GridTable{boxes, reso, map_off, n_maps, n_cells, max_cells};
   a.map_of = map_of;
-  a.n = n;
-  a.sg = sg;
-  a.max_pts = max_pts;
-  a.path = max_pts > 0 ? path : nullptr;
-  a.path_len = path_len;
-  a.cost = cost;
-  a.n_visited = n_visited;
-  a.status = status;
+  a.q = GridQueries{n, sg, max_pts, max_pts > 0 ? path : nullptr, path_len, cost, n_visited, status};
   int r = grid_many_slots(ctx, algo, max_cells, n, a.slots, a.slot_bytes);
   if (r != CRB_OK) return r;
   r = crb_grid_ws_reserve(ctx, 256 + (size_t)a.slots * (size_t)a.slot_bytes);

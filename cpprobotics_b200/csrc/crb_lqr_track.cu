@@ -297,17 +297,6 @@ LqrtC lqrt_constants(const crb_lqr_track_params* prm) {
   return c;
 }
 
-int lqrt_require_device(const char* fn) {
-  int count = 0;
-  const cudaError_t e = cudaGetDeviceCount(&count);
-  if (e != cudaSuccess || count == 0) {
-    cudaGetLastError();
-    crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", fn);
-    return CRB_ERR_NO_DEVICE;
-  }
-  return CRB_OK;
-}
-
 }  // namespace
 
 extern "C" {
@@ -335,7 +324,7 @@ int crb_lqr_steering_control_batched(crb_ctx* ctx, int64_t n, int nx, const floa
   const int rc = lqrt_check_control(nx, n, sp, prm);
   if (rc) return rc;
   CRB_REQUIRE(n == 0 || (state && cx && cy && cyaw && ck && ind && pe && pth_e && u), "NULL array");
-  const int dev = lqrt_require_device(__func__);
+  const int dev = crb_require_device(__func__);
   if (dev) return dev;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);   // ctx->device is current for this call, the caller's device is restored after it
@@ -364,7 +353,7 @@ int crb_lqr_steering_control_many_batched(crb_ctx* ctx, int64_t n, int nx, const
   if (rc) return rc;
   CRB_REQUIRE(n == 0 || (state && cx && cy && cyaw && ck && course_off && course_of && ind && pe && pth_e && u),
               "NULL array");
-  const int dev = lqrt_require_device(__func__);
+  const int dev = crb_require_device(__func__);
   if (dev) return dev;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);
@@ -388,7 +377,7 @@ int crb_lqr_update_batched(crb_ctx* ctx, int64_t n, float* state, const float* a
   const int rc = lqrt_check_plant(prm);
   if (rc) return rc;
   CRB_REQUIRE(n == 0 || (state && a && delta), "NULL array");
-  const int dev = lqrt_require_device(__func__);
+  const int dev = crb_require_device(__func__);
   if (dev) return dev;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);

@@ -312,18 +312,6 @@ static int mptg_check_params(const crb_mptg_params* p, int max_pts) {
   return CRB_OK;
 }
 
-// No device, no computation: the entry points say so after validating their arguments (no CPU fallback).
-static int mptg_require_device(const char* fn) {
-  int count = 0;
-  const cudaError_t e = cudaGetDeviceCount(&count);
-  if (e != cudaSuccess || count == 0) {
-    cudaGetLastError();
-    crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", fn);
-    return CRB_ERR_NO_DEVICE;
-  }
-  return CRB_OK;
-}
-
 extern "C" {
 
 void crb_mptg_default_params(crb_mptg_params* p) {
@@ -345,7 +333,7 @@ int crb_mptg_optimize_batched(crb_ctx* ctx, int64_t n, const float* state, const
   CRB_REQUIRE(n == 0 || (state && target && param), "state, target or param is NULL");
   int rc = mptg_check_params(prm, max_pts);
   if (rc != CRB_OK) return rc;
-  if ((rc = mptg_require_device(__func__)) != CRB_OK) return rc;
+  if ((rc = crb_require_device(__func__)) != CRB_OK) return rc;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);
   crb_mptg_optimize_kernel<<<crb_grid_for(n, MPTG_BLOCK), MPTG_BLOCK, 0, ctx->stream>>>(
@@ -363,7 +351,7 @@ int crb_mptg_generate_trajectory_batched(crb_ctx* ctx, int64_t n, const float* s
   CRB_REQUIRE(n == 0 || (state && param), "state or param is NULL");
   int rc = mptg_check_params(prm, max_pts);
   if (rc != CRB_OK) return rc;
-  if ((rc = mptg_require_device(__func__)) != CRB_OK) return rc;
+  if ((rc = crb_require_device(__func__)) != CRB_OK) return rc;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);
   crb_mptg_generate_kernel<<<crb_grid_for(n, MPTG_BLOCK), MPTG_BLOCK, 0, ctx->stream>>>(

@@ -246,14 +246,8 @@ extern "C" int crb_pf_step_many_batched(crb_ctx* ctx, int64_t n_robots, int32_t 
   CRB_REQUIRE(n_robots == 0 || (z_off && z_of && (z || n_rows == 0)), "z, z_off or z_of is NULL");
   CRB_REQUIRE(n_robots == 0 || (px && pw && px_next && u && result), "NULL array");
   CRB_REQUIRE(n_robots == 0 || px != px_next, "px and px_next must be different arrays");
-  {   // a usable device, or CRB_ERR_NO_DEVICE (valid arguments on a machine without one)
-    int count = 0;
-    if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
-      cudaGetLastError();
-      crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", __func__);
-      return CRB_ERR_NO_DEVICE;
-    }
-  }
+  const int rc = crb_require_device(__func__);
+  if (rc != CRB_OK) return rc;
   if (n_robots == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);
   PfFleetArgs fa;

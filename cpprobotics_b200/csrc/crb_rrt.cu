@@ -281,18 +281,13 @@ static int rrt_check_args(crb_ctx* ctx, const crb_rrt_params* prm, int64_t n, co
   return CRB_OK;
 }
 
-// No device, no computation (no CPU fallback); then the launch, n > 0.
+// No device, no computation (crb_require_device); then the launch, n > 0.
 static int rrt_launch(crb_ctx* ctx, const char* fn, const crb_rrt_params* prm, const float* ob, int64_t n_rows,
                       const int64_t* ob_off, int32_t n_sets, const int32_t* ob_of, int64_t n, const float* se,
                       const uint32_t* seed, int32_t max_pts, float* path, int32_t* path_len, int32_t max_nodes,
                       float* tree, int32_t* parent, int32_t* n_nodes, int32_t* n_iter, int32_t* status) {
-  int count = 0;
-  const cudaError_t ce = cudaGetDeviceCount(&count);
-  if (ce != cudaSuccess || count == 0) {
-    cudaGetLastError();
-    crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", fn);
-    return CRB_ERR_NO_DEVICE;
-  }
+  const int rc = crb_require_device(fn);
+  if (rc != CRB_OK) return rc;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);
   if (ctx->rrt_counter == nullptr) CRB_CUDA(cudaMalloc(&ctx->rrt_counter, sizeof(unsigned long long)));

@@ -214,18 +214,6 @@ static int slp_states(const crb_slp_sampler* s) {
   return (int)S;
 }
 
-// No device, no computation: the entry points say so after validating their arguments (no CPU fallback).
-static int slp_require_device(const char* fn) {
-  int count = 0;
-  const cudaError_t e = cudaGetDeviceCount(&count);
-  if (e != cudaSuccess || count == 0) {
-    cudaGetLastError();
-    crb_set_error("%s: no usable CUDA device; libcrb has no CPU fallback", fn);
-    return CRB_ERR_NO_DEVICE;
-  }
-  return CRB_OK;
-}
-
 extern "C" {
 
 void crb_slp_default_params(crb_mptg_params* p, float* v) {
@@ -252,7 +240,7 @@ int crb_slp_sample_states_batched(crb_ctx* ctx, int64_t n_q, const crb_slp_sampl
   if (S < 0) return CRB_ERR_INVALID_ARG;
   CRB_REQUIRE(n_q <= INT64_MAX / (S > 0 ? S : 1) / 3, "n_q * S out of range");
   CRB_REQUIRE(n_q == 0 || (qp && n_states && (target || S == 0)), "qp, target or n_states is NULL");
-  const int rc = slp_require_device(__func__);
+  const int rc = crb_require_device(__func__);
   if (rc != CRB_OK) return rc;
   if (n_q == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);
@@ -269,7 +257,7 @@ int crb_slp_search_nearest_batched(crb_ctx* ctx, int64_t n, const float* target,
   CRB_REQUIRE(n >= 0 && (n + SLP_BLOCK - 1) / SLP_BLOCK <= 0x7fffffff, "n out of range");
   CRB_REQUIRE(rows >= 1, "rows must be >= 1");
   CRB_REQUIRE(n == 0 || (target && table && param), "target, table or param is NULL");
-  const int rc = slp_require_device(__func__);
+  const int rc = crb_require_device(__func__);
   if (rc != CRB_OK) return rc;
   if (n == 0) return CRB_OK;
   CRB_DEVICE_GUARD(ctx);

@@ -10,7 +10,6 @@ H100 (-m gpu): group-by-group bits at n 1 to 2^20, both launch forms, 1 and 3 st
 and the special values of test_ekf_edges.py against the checker; bad indices; NULL status; graph capture; offsets past
 2^31; the resident track, pinned and pageable; the C++ program against the checker."""
 import ctypes as C
-import hashlib
 import os
 import subprocess
 
@@ -20,6 +19,7 @@ import pytest
 from cpprobotics_b200 import EKF_MODEL_DTYPE, EkfParams, _lib, ekf_models, synth
 from oracle import ekf_many as EM
 from oracle import oracle as O
+from sass_hashes import compile_source, kernel_sass_hashes
 from test_ekf_edges import NAMES, SETS, _assert_same, _params, _special_batch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -138,8 +138,6 @@ def test_composed_checker_on_one_model_is_the_checker():
         assert same(gx[:, cols], xo) and same(gP[:, cols], Po)
 
 
-NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false", "-Xptxas", "-v"]
 # sha256 of each single-model EKF kernel's SASS (cuobjdump -sass, NVCC_FLAGS, CUDA 12.9) as they were before the model
 # table existed: moving their shared code into crb_ekf_common.cuh must not change one instruction
 SINGLE_MODEL_SASS = {
@@ -150,18 +148,9 @@ SINGLE_MODEL_SASS = {
 }
 
 
-def _compile(tmp_path, src):
-    if not os.path.exists(NVCC):
-        pytest.skip("no nvcc")
-    obj = str(tmp_path / (src + ".o"))
-    log = subprocess.run([NVCC] + NVCC_FLAGS + ["-c", os.path.join(ROOT, "cpprobotics_b200", "csrc", src), "-o", obj],
-                         capture_output=True, text=True, check=True).stderr
-    return obj, log
-
-
 def test_model_table_kernels_do_not_spill(tmp_path):
     """Exactly the two launch forms, with no spill and no stack frame in them or in anything they call."""
-    _, log = _compile(tmp_path, "crb_ekf_many.cu")
+    _, log = compile_source(tmp_path, "crb_ekf_many.cu")
     blocks = {b.splitlines()[0].split("'")[1]: b for b in log.split("Compiling entry function")[1:]}
     assert set(blocks) == {"_Z19crb_ekf_many_kernelILi256ELi3ELi1EEvllPfS0_PKfS2_liPK7EkfArgsiPKiPi",
                            "_Z19crb_ekf_many_kernelILi128ELi4ELi2EEvllPfS0_PKfS2_liPK7EkfArgsiPKiPi"}, sorted(blocks)
@@ -174,17 +163,7 @@ def test_model_table_kernels_do_not_spill(tmp_path):
 
 
 def test_single_model_kernels_keep_their_machine_code(tmp_path):
-    ver = subprocess.run([NVCC, "--version"], capture_output=True, text=True).stdout if os.path.exists(NVCC) else ""
-    if "release 12.9" not in ver:
-        pytest.skip("the pinned SASS is CUDA 12.9's")
-    obj, _ = _compile(tmp_path, "crb_ekf.cu")
-    sass = subprocess.check_output([os.path.join(os.path.dirname(NVCC), "cuobjdump"), "-sass", obj], text=True)
-    got = {}
-    for sec in sass.split("Function : ")[1:]:
-        lines = sec.splitlines()
-        body = "\n".join(x for x in lines[1:] if x.strip() and "Fatbin" not in x and "code for" not in x)
-        got[lines[0].strip()] = hashlib.sha256(body.encode()).hexdigest()
-    assert got == SINGLE_MODEL_SASS
+    assert kernel_sass_hashes(tmp_path, "crb_ekf.cu") == SINGLE_MODEL_SASS
 
 
 def _build_api(tmp_path):

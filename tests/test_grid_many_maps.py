@@ -17,6 +17,7 @@ import pytest
 from cpprobotics_b200 import _lib, grid_map_table, synth
 from oracle import grid as OG
 from oracle import grid_many as GM
+from sass_hashes import compile_source, kernel_sass_hashes
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CPP_API = os.path.join(ROOT, "tests", "cpp", "grid_many_ref_api.cpp")
@@ -150,8 +151,6 @@ def test_composed_checker_on_one_map_is_the_checker():
         assert all(same(a[k], b[k]) for k in KEYS)
 
 
-NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false", "-Xptxas", "-v"]
 # sha256 of each single-map kernel's SASS (cuobjdump -sass, NVCC_FLAGS, CUDA 12.9) as they were before the many-map
 # planner existed: moving their shared code into crb_grid_common.cuh must not change one instruction
 SINGLE_MAP_SASS = {
@@ -162,17 +161,8 @@ SINGLE_MAP_SASS = {
 }
 
 
-def _compile(tmp_path, src):
-    if not os.path.exists(NVCC):
-        pytest.skip("no nvcc")
-    obj = str(tmp_path / (src + ".o"))
-    log = subprocess.run([NVCC] + NVCC_FLAGS + ["-c", os.path.join(ROOT, "cpprobotics_b200", "csrc", src), "-o", obj],
-                         capture_output=True, text=True, check=True).stderr
-    return obj, log
-
-
 def test_many_map_kernels_do_not_spill(tmp_path):
-    _, log = _compile(tmp_path, "crb_grid_many.cu")
+    _, log = compile_source(tmp_path, "crb_grid_many.cu")
     regs = {}
     for b in log.split("Compiling entry function")[1:]:
         name = b.splitlines()[0].split("'")[1]
@@ -185,18 +175,7 @@ def test_many_map_kernels_do_not_spill(tmp_path):
 
 
 def test_single_map_kernels_keep_their_machine_code(tmp_path):
-    import hashlib
-    ver = subprocess.run([NVCC, "--version"], capture_output=True, text=True).stdout if os.path.exists(NVCC) else ""
-    if "release 12.9" not in ver:
-        pytest.skip("the pinned SASS is CUDA 12.9's")
-    obj, _ = _compile(tmp_path, "crb_grid.cu")
-    sass = subprocess.check_output([os.path.join(os.path.dirname(NVCC), "cuobjdump"), "-sass", obj], text=True)
-    got = {}
-    for sec in sass.split("Function : ")[1:]:
-        lines = sec.splitlines()
-        body = "\n".join(x for x in lines[1:] if x.strip() and "Fatbin" not in x and "code for" not in x)
-        got[lines[0].strip()] = hashlib.sha256(body.encode()).hexdigest()
-    assert got == SINGLE_MAP_SASS
+    assert kernel_sass_hashes(tmp_path, "crb_grid.cu") == SINGLE_MAP_SASS
 
 
 def _build_api(tmp_path):

@@ -11,7 +11,6 @@ H100 (-m gpu): per-particle bits at np 1 to CRB_PF_FLEET_MAX_NP and up to 65536 
 Philox mode, crb_pf_step per robot, isolation of bad lists / NaN / zero weights, NULL status, n_robots = 0, graph
 capture, a 50-tick closed loop against the checker and the C++ fleet program against the checker."""
 import ctypes as C
-import hashlib
 import os
 import subprocess
 
@@ -22,6 +21,7 @@ import pf_cases as PC
 from cpprobotics_b200 import _lib, synth
 from oracle import oracle as OO
 from oracle import pf_fleet as PFF
+from sass_hashes import compile_source, kernel_sass_hashes
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CPP_API = os.path.join(ROOT, "tests", "cpp", "pf_fleet_ref_api.cpp")
@@ -118,8 +118,6 @@ def test_composed_checker_on_one_robot_is_the_checker():
     assert same(px2, f["px"]) and same(pw2, f["pw"]) and same(pxn2, f["px"])
 
 
-NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false", "-Xptxas", "-v"]
 # sha256 of each single-filter PF kernel's SASS (cuobjdump -sass, NVCC_FLAGS, CUDA 12.9) as they were before the fleet
 # filter existed: moving their shared code into crb_pf_common.cuh must not change one instruction
 SINGLE_FILTER_SASS = {
@@ -174,42 +172,23 @@ SINGLE_FILTER_SASS = {
 }
 
 
-def _compile(tmp_path, src):
-    if not os.path.exists(NVCC):
-        pytest.skip("no nvcc")
-    obj = str(tmp_path / (src + ".o"))
-    log = subprocess.run([NVCC] + NVCC_FLAGS + ["-c", os.path.join(ROOT, "cpprobotics_b200", "csrc", src), "-o", obj],
-                         capture_output=True, text=True, check=True).stderr
-    return obj, log
-
-
 def test_fleet_kernel_does_not_spill(tmp_path):
     """No spill.  The only stack frame is the 32 bytes of CUDA's sincosf large-argument reduction, reached for
     |yaw| > 1e5 on the CRB_PF_TRIG=0 path, which every single-filter predict kernel carries too."""
-    _, log = _compile(tmp_path, "crb_pf_fleet.cu")
+    _, log = compile_source(tmp_path, "crb_pf_fleet.cu")
     blocks = {b.splitlines()[0].split("'")[1]: b for b in log.split("Compiling entry function")[1:]}
     assert list(blocks) == ["_Z19crb_pf_fleet_kernelPfS_S_PKfS1_S1_PKlPKiS1_PdPi11PfFleetArgs"], list(blocks)
     b = next(iter(blocks.values()))
     assert "0 bytes spill stores, 0 bytes spill loads" in b, b
     assert int(b.split(" bytes stack frame")[0].split()[-1]) <= 32, b
     assert int(b.split("Used ")[1].split(" registers")[0]) <= 96, b
-    _, single = _compile(tmp_path, "crb_pf.cu")
+    _, single = compile_source(tmp_path, "crb_pf.cu")
     lean = [x for x in single.split("Compiling entry function")[1:] if "lean_kernel" in x.splitlines()[0]]
     assert lean and all("32 bytes stack frame" in x for x in lean)
 
 
 def test_single_filter_kernels_keep_their_machine_code(tmp_path):
-    ver = subprocess.run([NVCC, "--version"], capture_output=True, text=True).stdout if os.path.exists(NVCC) else ""
-    if "release 12.9" not in ver:
-        pytest.skip("the pinned SASS is CUDA 12.9's")
-    obj, _ = _compile(tmp_path, "crb_pf.cu")
-    sass = subprocess.check_output([os.path.join(os.path.dirname(NVCC), "cuobjdump"), "-sass", obj], text=True)
-    got = {}
-    for sec in sass.split("Function : ")[1:]:
-        lines = sec.splitlines()
-        body = "\n".join(x for x in lines[1:] if x.strip() and "Fatbin" not in x and "code for" not in x)
-        got[lines[0].strip()] = hashlib.sha256(body.encode()).hexdigest()
-    assert got == SINGLE_FILTER_SASS
+    assert kernel_sass_hashes(tmp_path, "crb_pf.cu") == SINGLE_FILTER_SASS
 
 
 def _build_api(tmp_path):
