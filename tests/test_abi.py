@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from cpprobotics_b200 import _lib
+from toolchain import run_layout_probe
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HDR = os.path.join(ROOT, "include", "crb.h")
@@ -33,13 +34,10 @@ def test_library_exports_every_declared_symbol():
 
 
 def test_struct_layouts_match_the_header(tmp_path):
-    src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(){printf("%zu %zu %zu %zu %zu %zu\\n",'
-                   "sizeof(crb_ekf_params),sizeof(crb_pf_params),sizeof(crb_mpc_params),"
-                   "offsetof(crb_ekf_params,R),offsetof(crb_pf_params,u),offsetof(crb_mpc_params,j_tol));return 0;}\n")
-    exe = tmp_path / "sz"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    got = [int(v) for v in subprocess.check_output([str(exe)]).split()]
+    got = run_layout_probe(
+        tmp_path, '#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(){printf("%zu %zu %zu %zu %zu %zu\\n",'
+        "sizeof(crb_ekf_params),sizeof(crb_pf_params),sizeof(crb_mpc_params),"
+        "offsetof(crb_ekf_params,R),offsetof(crb_pf_params,u),offsetof(crb_mpc_params,j_tol));return 0;}\n")
     want = [C.sizeof(_lib.EkfParams), C.sizeof(_lib.PfParams), C.sizeof(_lib.MpcParams),
             _lib.EkfParams.R.offset, _lib.PfParams.u.offset, _lib.MpcParams.j_tol.offset]
     assert got == want

@@ -13,10 +13,10 @@ import dwa_cases as D
 from cpprobotics_b200 import _lib, synth
 from oracle import dwa as OD
 from oracle._load import reference
+from toolchain import build_ref_program, run_layout_probe
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "dwa_golden.npz")
-CPP = os.path.join(ROOT, "tests", "cpp", "dwa_ref_api.cpp")
 
 
 def bits_equal(a, b):
@@ -117,14 +117,11 @@ def test_defaults_are_the_reference_config_and_layout_matches(tmp_path):
     n = C.c_int(0)
     assert _lib.load_library().crb_dwa_rollout_points(C.byref(lp), C.byref(n)) == 0 and n.value == 32
     assert OD.dwa_rollout_points(op) == 32
-    src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(void){printf("%zu %zu %zu '
-                   '%d %d %d %d\\n",sizeof(crb_dwa_params),offsetof(crb_dwa_params,v_reso),'
-                   'offsetof(crb_dwa_params,speed_cost_gain),CRB_DWA_MAX_OBSTACLES,CRB_DWA_MAX_SPEED_SAMPLES,'
-                   'CRB_DWA_MAX_YAWRATE_SAMPLES,CRB_DWA_MAX_STEPS);return 0;}\n')
-    exe = tmp_path / "sz"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    got = [int(v) for v in subprocess.check_output([str(exe)]).split()]
+    got = run_layout_probe(
+        tmp_path, '#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(void){printf("%zu %zu %zu '
+        '%d %d %d %d\\n",sizeof(crb_dwa_params),offsetof(crb_dwa_params,v_reso),'
+        'offsetof(crb_dwa_params,speed_cost_gain),CRB_DWA_MAX_OBSTACLES,CRB_DWA_MAX_SPEED_SAMPLES,'
+        'CRB_DWA_MAX_YAWRATE_SAMPLES,CRB_DWA_MAX_STEPS);return 0;}\n')
     assert got == [C.sizeof(_lib.DwaParams), _lib.DwaParams.v_reso.offset, _lib.DwaParams.speed_cost_gain.offset,
                    _lib.CRB_DWA_MAX_OBSTACLES, _lib.CRB_DWA_MAX_SPEED_SAMPLES, _lib.CRB_DWA_MAX_YAWRATE_SAMPLES,
                    _lib.CRB_DWA_MAX_STEPS]
@@ -180,16 +177,8 @@ def test_validation_needs_no_device():
         assert L.crb_dwa_motion_batched(ctx, 1, d, d, C.c_float(0.1)) == _lib.CRB_ERR_NO_DEVICE
 
 
-def _build_cpp(tmp_path):
-    exe = str(tmp_path / "dwa_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), CPP,
-                           "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
-
-
 def test_reference_style_program_compiles(tmp_path):
-    _build_cpp(tmp_path)
+    build_ref_program(tmp_path, "dwa_ref_api.cpp")
 
 
 # ---- H100 -----------------------------------------------------------------------------------------------------
@@ -299,7 +288,7 @@ def test_gpu_closed_loop_200_steps(engine):
 
 @pytest.mark.gpu
 def test_gpu_reference_style_program_matches_oracle(tmp_path):
-    exe = _build_cpp(tmp_path)
+    exe = build_ref_program(tmp_path, "dwa_ref_api.cpp")
     d = np.load(GOLDEN)
     x, u, g, ob = d["demo_x"], d["demo_u_in"], d["demo_goal"], d["demo_ob"]
     m = x.shape[1]

@@ -5,7 +5,6 @@ deterministic sweep of magnitudes and resolutions; the rollout length at 999, 10
 is bitwise the checker (and the reference text where oracle/_ref exists) at every configuration, in a closed loop, in
 the reference-style C++ program with a non-default Config, and with `traj` offsets past 2^31 elements."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
@@ -15,9 +14,8 @@ import dwa_cases as D
 from cpprobotics_b200 import _lib, synth
 from oracle import dwa as OD
 from oracle._load import reference
+from toolchain import build_ref_program
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CPP = os.path.join(ROOT, "tests", "cpp", "dwa_ref_api.cpp")
 VCAP, WCAP = _lib.CRB_DWA_MAX_SPEED_SAMPLES, _lib.CRB_DWA_MAX_YAWRATE_SAMPLES
 f32 = np.float32
 NAMES = list(D.CONFIGS)
@@ -402,19 +400,11 @@ def test_gpu_traj_offsets_past_2_31_elements(engine):
     assert bits_equal(got, np.ascontiguousarray(oc["traj"][rows]))
 
 
-def _build_cpp(tmp_path):
-    exe = str(tmp_path / "dwa_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), CPP,
-                           "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
-
-
 @pytest.mark.gpu
 def test_gpu_reference_style_program_with_a_non_default_config(tmp_path):
     """dwa_ref_api's third argument sets its Config member by member, so crb::dwa_params_of maps each member by name;
     every member of this configuration differs from every other."""
-    exe = _build_cpp(tmp_path)
+    exe = build_ref_program(tmp_path, "dwa_ref_api.cpp")
     p = D.config("distinct")
     ob = synth.DWA_DEMO_OBSTACLES
     x, u, g = robots("distinct", 40, ob, seed=12)

@@ -2,31 +2,20 @@
 CPU: the two EKF kernels the launcher selects compile for sm_90a, with the build's flags, without spilling to
 local memory.  H100: the two-agent form of the step (even n, 8-byte aligned arrays) gives the same bits as the
 one-agent form, over several steps per launch; crb_probe_ekf_pattern does what include/crb.h says it does."""
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
-import __graft_entry__ as G
 from cpprobotics_b200 import synth
+from toolchain import ptxas_kernels
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
-
-def test_ekf_compiles_only_the_two_launch_forms_without_spill(tmp_path):
-    if not os.path.exists(G.NVCC):
-        pytest.skip("no nvcc")
-    out = subprocess.run([G.NVCC] + G.NVCC_FLAGS + ["-c", os.path.join(G.CSRC, "crb_ekf.cu"),
-                                                    "-o", str(tmp_path / "ekf.o")],
-                         capture_output=True, text=True, check=True).stderr
-    blocks = out.split("Compiling entry function")[1:]
-    kernels = {b.splitlines()[0].split("'")[1]: b for b in blocks if "crb_ekf_step" in b.splitlines()[0]}
+def test_ekf_compiles_only_the_two_launch_forms_without_spill():
+    kernels = {k: f for k, f in ptxas_kernels("crb_ekf.cu").items() if "crb_ekf_step" in k}
     # the two-agent form <128,4,2> and the one-agent form <256,3,1>
     assert set(kernels) == {"_Z19crb_ekf_step_kernelILi128ELi4ELi2EEvllPfS0_PKfS2_li7EkfArgs",
                             "_Z19crb_ekf_step_kernelILi256ELi3ELi1EEvllPfS0_PKfS2_li7EkfArgs"}, sorted(kernels)
-    for name, b in kernels.items():
-        assert "0 bytes spill stores, 0 bytes spill loads" in b, (name, b)
+    for f in kernels.values():
+        assert (f.spill_stores, f.spill_loads) == (0, 0), f
 
 
 @pytest.mark.gpu

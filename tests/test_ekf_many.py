@@ -10,7 +10,6 @@ H100 (-m gpu): group-by-group bits at n 1 to 2^20, both launch forms, 1 and 3 st
 and the special values of test_ekf_edges.py against the checker; bad indices; NULL status; graph capture; offsets past
 2^31; the resident track, pinned and pageable; the C++ program against the checker."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
@@ -19,11 +18,9 @@ import pytest
 from cpprobotics_b200 import EKF_MODEL_DTYPE, EkfParams, _lib, ekf_models, synth
 from oracle import ekf_many as EM
 from oracle import oracle as O
-from sass_hashes import compile_source, kernel_sass_hashes
 from test_ekf_edges import NAMES, SETS, _assert_same, _params, _special_batch
+from toolchain import build_ref_program, kernel_sass_hashes, ptxas_functions
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CPP_API = os.path.join(ROOT, "tests", "cpp", "ekf_many_ref_api.cpp")
 INV = -1
 F32 = np.float32
 
@@ -148,34 +145,21 @@ SINGLE_MODEL_SASS = {
 }
 
 
-def test_model_table_kernels_do_not_spill(tmp_path):
+def test_model_table_kernels_do_not_spill():
     """Exactly the two launch forms, with no spill and no stack frame in them or in anything they call."""
-    _, log = compile_source(tmp_path, "crb_ekf_many.cu")
-    blocks = {b.splitlines()[0].split("'")[1]: b for b in log.split("Compiling entry function")[1:]}
-    assert set(blocks) == {"_Z19crb_ekf_many_kernelILi256ELi3ELi1EEvllPfS0_PKfS2_liPK7EkfArgsiPKiPi",
-                           "_Z19crb_ekf_many_kernelILi128ELi4ELi2EEvllPfS0_PKfS2_liPK7EkfArgsiPKiPi"}, sorted(blocks)
-    for name, b in blocks.items():
-        assert "crb_ekf_step" not in name
-        assert "0 bytes spill stores, 0 bytes spill loads" in b, (name, b)
-    props = [ln for ln in log.splitlines() if "bytes stack frame" in ln]
-    assert props and all(ln.strip().startswith("0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads")
-                         for ln in props), props
+    fns = ptxas_functions("crb_ekf_many.cu")
+    assert {f.name for f in fns if f.entry} == {
+        "_Z19crb_ekf_many_kernelILi256ELi3ELi1EEvllPfS0_PKfS2_liPK7EkfArgsiPKiPi",
+        "_Z19crb_ekf_many_kernelILi128ELi4ELi2EEvllPfS0_PKfS2_liPK7EkfArgsiPKiPi"}, fns
+    assert all((f.stack, f.spill_stores, f.spill_loads) == (0, 0, 0) for f in fns), fns
 
 
-def test_single_model_kernels_keep_their_machine_code(tmp_path):
-    assert kernel_sass_hashes(tmp_path, "crb_ekf.cu") == SINGLE_MODEL_SASS
-
-
-def _build_api(tmp_path):
-    exe = str(tmp_path / "ekf_many_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
-                           CPP_API, "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
+def test_single_model_kernels_keep_their_machine_code():
+    assert kernel_sass_hashes("crb_ekf.cu") == SINGLE_MODEL_SASS
 
 
 def test_reference_style_program_compiles(tmp_path):
-    _build_api(tmp_path)
+    build_ref_program(tmp_path, "ekf_many_ref_api.cpp")
 
 
 # ---- H100 ---------------------------------------------------------------------------------------------------------------
@@ -443,7 +427,8 @@ def test_track_is_the_many_launch(engine, pinned):
 @pytest.mark.gpu
 def test_reference_style_program_matches_the_checker(tmp_path):
     """The C++ fleet (ekf_estimation over vectors of robots, 50 ticks) against the checker fed the program's inputs."""
-    out = subprocess.check_output([_build_api(tmp_path)], text=True).strip().splitlines()
+    exe = build_ref_program(tmp_path, "ekf_many_ref_api.cpp")
+    out = subprocess.check_output([exe], text=True).strip().splitlines()
     head = out[0].split()
     nr, steps = int(head[1]), int(head[3])
     rows = {}

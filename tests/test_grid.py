@@ -16,10 +16,10 @@ import grid_cases as GC
 from grid_cases import same
 from cpprobotics_b200 import _lib, grid_box_of_obstacles, synth
 from oracle import grid as OG
+from toolchain import STRICT_C99, build_ref_program, ptxas_kernels, run_layout_probe
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "grid_golden.npz")
-CPP_API = os.path.join(ROOT, "tests", "cpp", "grid_ref_api.cpp")
 CPP_HEAP = os.path.join(ROOT, "tests", "cpp", "grid_heap_pin.cpp")
 ALGO_IDS = [a for a, _ in GC.ALGOS]
 
@@ -174,16 +174,12 @@ def test_checker_statuses_where_the_reference_is_undefined(algo):
 
 
 def test_box_and_layout_on_the_host(tmp_path):
-    src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(void){printf("%zu %zu %zu %zu '
-                   '%d %d %d %d %d %d %d %d %zu\\n",sizeof(crb_grid_box),offsetof(crb_grid_box,min_y),'
-                   'offsetof(crb_grid_box,max_x),offsetof(crb_grid_box,max_y),CRB_GRID_MAX_SIDE,CRB_GRID_MAX_CELLS,'
-                   'CRB_GRID_ASTAR,CRB_GRID_DIJKSTRA,CRB_GRID_FOUND,CRB_GRID_NO_PATH,CRB_GRID_START_OUTSIDE,'
-                   'CRB_GRID_BAD_POINT,CRB_GRID_WS_BUDGET);return 0;}\n')
-    exe = tmp_path / "sz"
-    subprocess.check_call(["gcc", "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o",
-                           str(exe)])
-    got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
+    got = run_layout_probe(
+        tmp_path, '#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(void){printf("%zu %zu %zu %zu '
+        '%d %d %d %d %d %d %d %d %zu\\n",sizeof(crb_grid_box),offsetof(crb_grid_box,min_y),'
+        'offsetof(crb_grid_box,max_x),offsetof(crb_grid_box,max_y),CRB_GRID_MAX_SIDE,CRB_GRID_MAX_CELLS,'
+        'CRB_GRID_ASTAR,CRB_GRID_DIJKSTRA,CRB_GRID_FOUND,CRB_GRID_NO_PATH,CRB_GRID_START_OUTSIDE,'
+        'CRB_GRID_BAD_POINT,CRB_GRID_WS_BUDGET);return 0;}\n', STRICT_C99)
     B = _lib.GridBox
     assert got[:4] == [C.sizeof(B), B.min_y.offset, B.max_x.offset, B.max_y.offset]
     assert got[4:] == [_lib.CRB_GRID_MAX_SIDE, _lib.CRB_GRID_MAX_CELLS, _lib.CRB_GRID_ASTAR, _lib.CRB_GRID_DIJKSTRA,
@@ -250,30 +246,15 @@ def test_validation_needs_no_device():
         assert L.crb_grid_plan_slots(ctx, 1, C.byref(good), 5, C.byref(C.c_int64())) == nd
 
 
-def _build_api(tmp_path):
-    exe = str(tmp_path / "grid_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
-                           CPP_API, "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
-
-
 def test_reference_style_program_compiles(tmp_path):
-    _build_api(tmp_path)
+    build_ref_program(tmp_path, "grid_ref_api.cpp")
 
 
-def test_new_kernels_do_not_spill(tmp_path):
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc):
-        pytest.skip("no nvcc")
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false",
-                          "-Xptxas", "-v", "-c", os.path.join(ROOT, "cpprobotics_b200", "csrc", "crb_grid.cu"),
-                          "-o", str(tmp_path / "grid.o")], capture_output=True, text=True, check=True).stderr
-    blocks = out.split("Compiling entry function")[1:]
-    kernels = [b for b in blocks if "crb_grid_" in b.splitlines()[0]]
+def test_new_kernels_do_not_spill():
+    kernels = [f for k, f in ptxas_kernels("crb_grid.cu").items() if "crb_grid_" in k]
     assert len(kernels) == 3
-    for b in kernels:
-        assert "0 bytes spill stores, 0 bytes spill loads" in b and "0 bytes stack frame" in b, b
+    for f in kernels:
+        assert (f.stack, f.spill_stores, f.spill_loads) == (0, 0, 0), f
 
 
 # ---- H100 -----------------------------------------------------------------------------------------------------
@@ -430,7 +411,7 @@ def test_gpu_reproduces_the_golden_fixture(engine):
 
 @pytest.mark.gpu
 def test_gpu_reference_style_program_matches_checker(tmp_path):
-    exe = _build_api(tmp_path)
+    exe = build_ref_program(tmp_path, "grid_ref_api.cpp")
     subprocess.check_call([exe, str(tmp_path / "out.bin")])
     out = np.fromfile(tmp_path / "out.bin", np.float32)
     ox, oy, reso, rr, _ = GC.demo()

@@ -8,7 +8,6 @@ H100 (-m gpu): maps at n_maps = 1, 7 and 1024; plans at n = 1 to 65536 in random
 max_pts 0, truncating and long; every way a table entry can be bad; NULL outputs, n = 0, graph capture, a workspace
 shared with the single-map planner; a local-window fleet; the C++ program against the checker."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
@@ -17,10 +16,8 @@ import pytest
 from cpprobotics_b200 import _lib, grid_map_table, synth
 from oracle import grid as OG
 from oracle import grid_many as GM
-from sass_hashes import compile_source, kernel_sass_hashes
+from toolchain import build_ref_program, kernel_sass_hashes, ptxas_kernels
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CPP_API = os.path.join(ROOT, "tests", "cpp", "grid_many_ref_api.cpp")
 INV = -1
 KEYS = ("path", "path_len", "cost", "n_visited", "status")
 
@@ -161,33 +158,21 @@ SINGLE_MAP_SASS = {
 }
 
 
-def test_many_map_kernels_do_not_spill(tmp_path):
-    _, log = compile_source(tmp_path, "crb_grid_many.cu")
-    regs = {}
-    for b in log.split("Compiling entry function")[1:]:
-        name = b.splitlines()[0].split("'")[1]
-        assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in b, b
-        regs[name] = int(b.split("Used ")[1].split(" registers")[0])
-    assert sorted(regs) == ["_Z24crb_grid_map_many_kernel11GridMapArgs",
-                            "_Z25crb_grid_plan_many_kernelILi0EEv16GridPlanManyArgs",
-                            "_Z25crb_grid_plan_many_kernelILi1EEv16GridPlanManyArgs"], regs
-    assert all(r <= 56 for r in regs.values()), regs
+def test_many_map_kernels_do_not_spill():
+    kernels = ptxas_kernels("crb_grid_many.cu")
+    assert sorted(kernels) == ["_Z24crb_grid_map_many_kernel11GridMapArgs",
+                               "_Z25crb_grid_plan_many_kernelILi0EEv16GridPlanManyArgs",
+                               "_Z25crb_grid_plan_many_kernelILi1EEv16GridPlanManyArgs"], kernels
+    for f in kernels.values():
+        assert (f.stack, f.spill_stores, f.spill_loads) == (0, 0, 0) and f.registers <= 56, f
 
 
-def test_single_map_kernels_keep_their_machine_code(tmp_path):
-    assert kernel_sass_hashes(tmp_path, "crb_grid.cu") == SINGLE_MAP_SASS
-
-
-def _build_api(tmp_path):
-    exe = str(tmp_path / "grid_many_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
-                           CPP_API, "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
+def test_single_map_kernels_keep_their_machine_code():
+    assert kernel_sass_hashes("crb_grid.cu") == SINGLE_MAP_SASS
 
 
 def test_reference_style_program_compiles(tmp_path):
-    _build_api(tmp_path)
+    build_ref_program(tmp_path, "grid_many_ref_api.cpp")
 
 
 # ---- H100 ---------------------------------------------------------------------------------------------------------------
@@ -452,7 +437,7 @@ def test_local_windows_against_the_checker(engine):
 
 @pytest.mark.gpu
 def test_reference_style_program_matches_the_checker(tmp_path):
-    exe = _build_api(tmp_path)
+    exe = build_ref_program(tmp_path, "grid_many_ref_api.cpp")
     out = tmp_path / "out.bin"
     subprocess.check_call([exe, str(out)])
     got = np.fromfile(out, np.float32)

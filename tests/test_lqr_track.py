@@ -20,10 +20,10 @@ from cpprobotics_b200 import _lib, lqr_track_default_params, synth
 from oracle import lqrt as OL
 from oracle import oracle as O
 from oracle._load import reference
+from toolchain import build_ref_program, ptxas_functions, ptxas_kernels
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "lqr_track_golden.npz")
-CPP_API = os.path.join(ROOT, "tests", "cpp", "lqr_ref_api.cpp")
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 KP, STOP_SPEED = 1.0, 0.05
 
@@ -345,37 +345,17 @@ def test_validation_needs_no_device():
         assert b"no CPU fallback" in L.crb_last_error_string()
 
 
-def _build_api(tmp_path):
-    exe = str(tmp_path / "lqr_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
-                           CPP_API, "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
-
-
 def test_reference_style_program_compiles(tmp_path):
-    _build_api(tmp_path)
+    build_ref_program(tmp_path, "lqr_ref_api.cpp")
 
 
-def test_new_kernels_do_not_spill(tmp_path):
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc):
-        pytest.skip("no nvcc")
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false",
-                          "-Xptxas", "-v", "-c", os.path.join(ROOT, "cpprobotics_b200", "csrc", "crb_lqr_track.cu"),
-                          "-o", str(tmp_path / "lqrt.o")], capture_output=True, text=True, check=True).stderr
-    blocks = out.split("Compiling entry function")[1:]
-    names = [b.splitlines()[0] for b in blocks]
-    assert sum("crb_lqr_steering_control_kernel" in s for s in names) == 2
-    assert sum("crb_lqr_update_kernel" in s for s in names) == 1
-    for b in out.split("Function properties for")[1:]:   # the kernels and the out-of-line libm pieces
-        assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in b.splitlines()[1], b
-    # the refactored dlqr kernel too
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false",
-                          "-Xptxas", "-v", "-c", os.path.join(ROOT, "cpprobotics_b200", "csrc", "crb_lqr.cu"),
-                          "-o", str(tmp_path / "lqr.o")], capture_output=True, text=True, check=True).stderr
-    for b in out.split("Function properties for")[1:]:
-        assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in b.splitlines()[1], b
+def test_new_kernels_do_not_spill():
+    kernels = list(ptxas_kernels("crb_lqr_track.cu"))
+    assert sum("crb_lqr_steering_control_kernel" in k for k in kernels) == 2
+    assert sum("crb_lqr_update_kernel" in k for k in kernels) == 1
+    # the kernels and the out-of-line libm pieces, and the refactored dlqr kernel too
+    for f in ptxas_functions("crb_lqr_track.cu") + ptxas_functions("crb_lqr.cu"):
+        assert (f.stack, f.spill_stores, f.spill_loads) == (0, 0, 0), f
 
 
 # ---- H100 -----------------------------------------------------------------------------------------------------

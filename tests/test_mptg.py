@@ -15,10 +15,10 @@ import mptg_cases as MC
 from cpprobotics_b200 import _lib, synth
 from oracle import mptg as OM
 from oracle._load import reference
+from toolchain import build_ref_program, run_layout_probe
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "mptg_golden.npz")
-CPP = os.path.join(ROOT, "tests", "cpp", "mptg_ref_api.cpp")
 MAX_PTS = 128  # the golden fixture's
 
 
@@ -153,15 +153,12 @@ def test_defaults_and_layout(tmp_path):
     assert (lp.base_l, lp.ds, lp.max_iter, lp.cost_th, list(lp.h_step)) == \
         (op.base_l, op.ds, op.max_iter, op.cost_th, list(op.h_step))
     assert np.float32(lp.cost_th) == np.float32(0.1) and np.float32(lp.h_step[1]) == np.float32(0.005)
-    src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(void){printf("%zu %zu %zu %zu '
-                   '%d %d %d %d %d %d %d\\n",sizeof(crb_mptg_params),offsetof(crb_mptg_params,max_iter),'
-                   'offsetof(crb_mptg_params,cost_th),offsetof(crb_mptg_params,h_step),CRB_MPTG_MAX_ITER,'
-                   'CRB_MPTG_MAX_STEPS,CRB_MPTG_CONVERGED,CRB_MPTG_MAX_ITER_REACHED,CRB_MPTG_EMPTY_TRAJ,'
-                   'CRB_MPTG_STEP_CAP,CRB_MPTG_OUT_OF_RANGE);return 0;}\n')
-    exe = tmp_path / "sz"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    got = [int(v) for v in subprocess.check_output([str(exe)]).split()]
+    got = run_layout_probe(
+        tmp_path, '#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(void){printf("%zu %zu %zu %zu '
+        '%d %d %d %d %d %d %d\\n",sizeof(crb_mptg_params),offsetof(crb_mptg_params,max_iter),'
+        'offsetof(crb_mptg_params,cost_th),offsetof(crb_mptg_params,h_step),CRB_MPTG_MAX_ITER,'
+        'CRB_MPTG_MAX_STEPS,CRB_MPTG_CONVERGED,CRB_MPTG_MAX_ITER_REACHED,CRB_MPTG_EMPTY_TRAJ,'
+        'CRB_MPTG_STEP_CAP,CRB_MPTG_OUT_OF_RANGE);return 0;}\n')
     M = _lib.MptgParams
     assert got == [C.sizeof(M), M.max_iter.offset, M.cost_th.offset, M.h_step.offset, _lib.CRB_MPTG_MAX_ITER,
                    _lib.CRB_MPTG_MAX_STEPS, _lib.CRB_MPTG_CONVERGED, _lib.CRB_MPTG_MAX_ITER_REACHED,
@@ -223,16 +220,8 @@ def test_validation_needs_no_device():
         assert opt(prm=C.byref(lib_params(p))) == _lib.CRB_ERR_NO_DEVICE
 
 
-def _build_cpp(tmp_path):
-    exe = str(tmp_path / "mptg_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), CPP,
-                           "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
-
-
 def test_reference_style_program_compiles(tmp_path):
-    _build_cpp(tmp_path)
+    build_ref_program(tmp_path, "mptg_ref_api.cpp")
 
 
 # ---- H100 -----------------------------------------------------------------------------------------------------
@@ -347,7 +336,7 @@ def test_gpu_generate_trajectory_alone(engine):
 
 @pytest.mark.gpu
 def test_gpu_reference_style_program_matches_oracle(tmp_path):
-    exe = _build_cpp(tmp_path)
+    exe = build_ref_program(tmp_path, "mptg_ref_api.cpp")
     st, tg, pa = synth.mptg_inputs(300, seed=21)
     keep = np.flatnonzero(OM.optimize(st, tg, pa)["status"] <= OM.MAX_ITER_REACHED)[:40]
     d0 = MC.demo()

@@ -2,23 +2,16 @@
 alone — one host thread and one crb_ctx per device, libcrb's own NCCL communicator (crb_comm_*), one
 crb_gather_stats per call.  CPU: it compiles against the header, links libcrb.so and fails loudly without a GPU.
 GPU (needs >= 2 devices, `gpurun --gpus 2`): it runs and every rank gathers the same table."""
-import os
 import subprocess
 
 import pytest
 
 from cpprobotics_b200 import _lib
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "cpp", "multi_gpu_demo.cpp")
+from toolchain import build_ref_program
 
 
 def build(tmp_path):
-    exe = str(tmp_path / "multi_gpu_demo")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-pthread", "-I", os.path.join(ROOT, "include"),
-                           SRC, "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
+    return build_ref_program(tmp_path, "multi_gpu_demo.cpp", ("-pthread",))
 
 
 def test_compiles_links_and_needs_a_gpu(tmp_path):

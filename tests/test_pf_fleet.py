@@ -11,7 +11,6 @@ H100 (-m gpu): per-particle bits at np 1 to CRB_PF_FLEET_MAX_NP and up to 65536 
 Philox mode, crb_pf_step per robot, isolation of bad lists / NaN / zero weights, NULL status, n_robots = 0, graph
 capture, a 50-tick closed loop against the checker and the C++ fleet program against the checker."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
@@ -21,10 +20,8 @@ import pf_cases as PC
 from cpprobotics_b200 import _lib, synth
 from oracle import oracle as OO
 from oracle import pf_fleet as PFF
-from sass_hashes import compile_source, kernel_sass_hashes
+from toolchain import build_ref_program, kernel_sass_hashes, ptxas_kernels
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CPP_API = os.path.join(ROOT, "tests", "cpp", "pf_fleet_ref_api.cpp")
 INV = -1
 CAP = _lib.CRB_PF_FLEET_MAX_NP
 
@@ -172,35 +169,23 @@ SINGLE_FILTER_SASS = {
 }
 
 
-def test_fleet_kernel_does_not_spill(tmp_path):
+def test_fleet_kernel_does_not_spill():
     """No spill.  The only stack frame is the 32 bytes of CUDA's sincosf large-argument reduction, reached for
     |yaw| > 1e5 on the CRB_PF_TRIG=0 path, which every single-filter predict kernel carries too."""
-    _, log = compile_source(tmp_path, "crb_pf_fleet.cu")
-    blocks = {b.splitlines()[0].split("'")[1]: b for b in log.split("Compiling entry function")[1:]}
-    assert list(blocks) == ["_Z19crb_pf_fleet_kernelPfS_S_PKfS1_S1_PKlPKiS1_PdPi11PfFleetArgs"], list(blocks)
-    b = next(iter(blocks.values()))
-    assert "0 bytes spill stores, 0 bytes spill loads" in b, b
-    assert int(b.split(" bytes stack frame")[0].split()[-1]) <= 32, b
-    assert int(b.split("Used ")[1].split(" registers")[0]) <= 96, b
-    _, single = compile_source(tmp_path, "crb_pf.cu")
-    lean = [x for x in single.split("Compiling entry function")[1:] if "lean_kernel" in x.splitlines()[0]]
-    assert lean and all("32 bytes stack frame" in x for x in lean)
+    kernels = ptxas_kernels("crb_pf_fleet.cu")
+    assert list(kernels) == ["_Z19crb_pf_fleet_kernelPfS_S_PKfS1_S1_PKlPKiS1_PdPi11PfFleetArgs"], list(kernels)
+    f = next(iter(kernels.values()))
+    assert (f.spill_stores, f.spill_loads) == (0, 0) and f.stack <= 32 and f.registers <= 96, f
+    lean = [f for k, f in ptxas_kernels("crb_pf.cu").items() if "lean_kernel" in k]
+    assert lean and all(f.stack == 32 for f in lean), lean
 
 
-def test_single_filter_kernels_keep_their_machine_code(tmp_path):
-    assert kernel_sass_hashes(tmp_path, "crb_pf.cu") == SINGLE_FILTER_SASS
-
-
-def _build_api(tmp_path):
-    exe = str(tmp_path / "pf_fleet_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
-                           CPP_API, "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
+def test_single_filter_kernels_keep_their_machine_code():
+    assert kernel_sass_hashes("crb_pf.cu") == SINGLE_FILTER_SASS
 
 
 def test_reference_style_program_compiles(tmp_path):
-    _build_api(tmp_path)
+    build_ref_program(tmp_path, "pf_fleet_ref_api.cpp")
 
 
 # ---- H100 ---------------------------------------------------------------------------------------------------------------
@@ -491,7 +476,8 @@ def test_closed_loop_against_the_checker(engine):
 def test_reference_style_program_matches_the_checker(tmp_path):
     """The C++ fleet tick (pf_localization_resampling) against the checker fed the program's inputs and the draws the
     reference's loops make with each robot's generators."""
-    out = subprocess.check_output([_build_api(tmp_path)], text=True).strip().splitlines()
+    exe = build_ref_program(tmp_path, "pf_fleet_ref_api.cpp")
+    out = subprocess.check_output([exe], text=True).strip().splitlines()
     head = out[0].split()
     nr, npr = int(head[1]), int(head[3])
     rows = {}

@@ -20,9 +20,8 @@ import rrt_cases as RC
 from cpprobotics_b200 import _lib, rrt_default_params, synth
 from oracle import dwa as OD
 from oracle import rrt as OR
+from toolchain import build_ref_program, ptxas_kernels
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CPP_API = os.path.join(ROOT, "tests", "cpp", "plan_many_ref_api.cpp")
 INV = -1
 DEMO = synth.RRT_DEMO
 RRT_KEYS = ("path", "path_len", "tree", "parent", "n_nodes", "n_iter", "status")
@@ -193,35 +192,19 @@ def test_checker_composed_per_list_is_the_checker_on_one_shared_list():
     assert all(same(r[k], o[k]) for k in RRT_KEYS)
 
 
-def test_changed_kernels_do_not_spill(tmp_path):
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc):
-        pytest.skip("no nvcc")
+def test_changed_kernels_do_not_spill():
     found = []
-    for src, kernel in (("crb_dwa.cu", "crb_dwa_control_many_kernel"), ("crb_rrt.cu", "crb_rrt_plan_kernel")):
-        out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false",
-                              "-Xptxas", "-v", "-c", os.path.join(ROOT, "cpprobotics_b200", "csrc", src),
-                              "-o", str(tmp_path / (src + ".o"))], capture_output=True, text=True, check=True).stderr
-        for b in out.split("Compiling entry function")[1:]:
-            if kernel in b.splitlines()[0]:
+    for src, kernel, max_regs in (("crb_dwa.cu", "crb_dwa_control_many_kernel", 64),
+                                  ("crb_rrt.cu", "crb_rrt_plan_kernel", 58)):
+        for name, f in ptxas_kernels(src).items():
+            if kernel in name:
                 found.append(kernel)
-                props = b.split("Function properties for")[1].splitlines()[1]
-                assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in props, b
-                regs = int(b.split("Used ")[1].split(" registers")[0])
-                assert regs <= (58 if "rrt" in kernel else 64), b
+                assert (f.stack, f.spill_stores, f.spill_loads) == (0, 0, 0) and f.registers <= max_regs, f
     assert sorted(found) == ["crb_dwa_control_many_kernel", "crb_rrt_plan_kernel"]
 
 
-def _build_api(tmp_path):
-    exe = str(tmp_path / "plan_many_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
-                           CPP_API, "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
-
-
 def test_reference_style_program_compiles(tmp_path):
-    _build_api(tmp_path)
+    build_ref_program(tmp_path, "plan_many_ref_api.cpp")
 
 
 # ---- H100 ---------------------------------------------------------------------------------------------------------------
@@ -573,7 +556,7 @@ def test_gpu_rrt_many_launch_forms(engine):
 
 @pytest.mark.gpu
 def test_gpu_reference_style_program_matches_the_checker(tmp_path):
-    exe = _build_api(tmp_path)
+    exe = build_ref_program(tmp_path, "plan_many_ref_api.cpp")
     lists = synth.dwa_fleet_obstacles(6, seed=13)
     m = 6
     x, u, g = synth.dwa_inputs(m, seed=14)

@@ -6,7 +6,7 @@ crb_dwa_control_many_kernel and crb_dwa_motion_kernel are byte-identical to thei
 crb_dwa_control_kernel and the three many-map grid kernels are not: they have the same instruction count and ptxas
 reports the same registers or fewer (crb_dwa_control_kernel 48 where it used 50), no spill and no stack frame, but the
 registers are allocated differently.  Their pins hold them from here on."""
-from sass_hashes import kernel_sass_hashes
+from toolchain import kernel_sass_hashes
 
 DWA_SASS = {
     "_Z21crb_dwa_motion_kernellPfPKff": "e2529eb1cc6f6bdcda66adc34f8c1a0eeed167da825c84c8d1225f846c57f389",
@@ -25,9 +25,9 @@ GRID_MANY_SASS = {
 }
 
 
-def test_dwa_kernels_keep_their_machine_code(tmp_path):
-    assert kernel_sass_hashes(tmp_path, "crb_dwa.cu") == DWA_SASS
+def test_dwa_kernels_keep_their_machine_code():
+    assert kernel_sass_hashes("crb_dwa.cu") == DWA_SASS
 
 
-def test_many_map_grid_kernels_keep_their_machine_code(tmp_path):
-    assert kernel_sass_hashes(tmp_path, "crb_grid_many.cu") == GRID_MANY_SASS
+def test_many_map_grid_kernels_keep_their_machine_code():
+    assert kernel_sass_hashes("crb_grid_many.cu") == GRID_MANY_SASS

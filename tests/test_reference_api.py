@@ -8,20 +8,16 @@ import sys
 import numpy as np
 import pytest
 
-from cpprobotics_b200 import _lib, synth
+from cpprobotics_b200 import synth
 from oracle import oracle as O
+from toolchain import build_ref_program
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "cpp", "ref_api_demo.cpp")
 K, T, NP = 40, 6, 100
 
 
 def build(tmp_path):
-    exe = str(tmp_path / "ref_api_demo")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-I", os.path.join(ROOT, "include"), SRC,
-                           "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
+    return build_ref_program(tmp_path, "ref_api_demo.cpp", werror=False)
 
 
 def make_inputs():
@@ -39,10 +35,7 @@ def make_inputs():
 def test_every_reference_signature_compiles_and_links(tmp_path):
     """ekf_estimation, pf_localization, resampling, mpc_solve, update, calc_ref_trajectory, solve_DARE and dlqr
     (both LQR demos) with the argument types a CppRobotics main() passes: -std=c++11 -Wall -Werror."""
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "ref_api_all_signatures.cpp"), "-L", libdir, "-lcrb",
-                           f"-Wl,-rpath,{libdir}", "-o", str(tmp_path / "ref_sig")])
+    build_ref_program(tmp_path, "ref_api_all_signatures.cpp")
 
 
 def test_compiles_links_and_fails_loudly_without_gpu(tmp_path):

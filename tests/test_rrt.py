@@ -16,10 +16,10 @@ import pytest
 import rrt_cases as RC
 from cpprobotics_b200 import _lib, rrt_default_params, synth
 from oracle import rrt as OR
+from toolchain import STRICT_C99, build_ref_program, ptxas_functions, run_layout_probe
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "rrt_golden.npz")
-CPP_API = os.path.join(ROOT, "tests", "cpp", "rrt_ref_api.cpp")
 CPP_PIN = os.path.join(ROOT, "tests", "cpp", "rrt_dist_pin.cpp")
 DEMO = synth.RRT_DEMO
 KEYS = ("path", "path_len", "tree", "parent", "n_nodes", "n_iter", "status")
@@ -221,25 +221,19 @@ def test_checker_statuses_where_the_reference_is_undefined():
 
 
 def test_params_and_layout_on_the_host(tmp_path):
-    src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(void){crb_rrt_params p;'
-                   'crb_rrt_default_params(&p);printf("%zu %zu %zu %zu %zu %d %d %d %d %g %g %g %d %d\\n",'
-                   'sizeof(crb_rrt_params),offsetof(crb_rrt_params,rand_max),offsetof(crb_rrt_params,expand_dis),'
-                   'offsetof(crb_rrt_params,goal_sample_rate),offsetof(crb_rrt_params,max_iter),CRB_RRT_MAX_ITER,'
-                   'CRB_RRT_FOUND,CRB_RRT_MAX_ITER_REACHED,CRB_RRT_BAD_INPUT,p.rand_min,p.rand_max,p.expand_dis,'
-                   'p.goal_sample_rate,p.max_iter);return 0;}\n')
-    exe = tmp_path / "sz"
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["gcc", "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o",
-                           str(exe), "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}"])
-    got = subprocess.check_output([str(exe)]).split()
+    got = run_layout_probe(
+        tmp_path, '#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(void){crb_rrt_params p;'
+        'crb_rrt_default_params(&p);printf("%zu %zu %zu %zu %zu %d %d %d %d %g %g %g %d %d\\n",'
+        'sizeof(crb_rrt_params),offsetof(crb_rrt_params,rand_max),offsetof(crb_rrt_params,expand_dis),'
+        'offsetof(crb_rrt_params,goal_sample_rate),offsetof(crb_rrt_params,max_iter),CRB_RRT_MAX_ITER,'
+        'CRB_RRT_FOUND,CRB_RRT_MAX_ITER_REACHED,CRB_RRT_BAD_INPUT,p.rand_min,p.rand_max,p.expand_dis,'
+        'p.goal_sample_rate,p.max_iter);return 0;}\n', STRICT_C99, link_crb=True)
     P = _lib.RrtParams
-    assert [int(x) for x in got[:5]] == [C.sizeof(P), P.rand_max.offset, P.expand_dis.offset,
-                                         P.goal_sample_rate.offset, P.max_iter.offset]
-    assert [int(x) for x in got[5:9]] == [_lib.CRB_RRT_MAX_ITER, _lib.CRB_RRT_FOUND, _lib.CRB_RRT_MAX_ITER_REACHED,
-                                          _lib.CRB_RRT_BAD_INPUT]
-    assert [int(x) for x in got[5:9]] == [OR.MAX_ITER_LIMIT, OR.FOUND, OR.MAX_ITER, OR.BAD_INPUT]
-    assert [float(x) for x in got[9:12]] == [-2.0, 15.0, 1.0] and [int(x) for x in got[12:]] == [5, 500]
+    assert got[:5] == [C.sizeof(P), P.rand_max.offset, P.expand_dis.offset, P.goal_sample_rate.offset,
+                       P.max_iter.offset]
+    assert got[5:9] == [_lib.CRB_RRT_MAX_ITER, _lib.CRB_RRT_FOUND, _lib.CRB_RRT_MAX_ITER_REACHED, _lib.CRB_RRT_BAD_INPUT]
+    assert got[5:9] == [OR.MAX_ITER_LIMIT, OR.FOUND, OR.MAX_ITER, OR.BAD_INPUT]
+    assert got[9:] == [-2, 15, 1, 5, 500]   # rand_min, rand_max and expand_dis are whole, so %g prints integers
     p = rrt_default_params()
     assert (p.rand_min, p.rand_max, p.expand_dis, p.goal_sample_rate, p.max_iter) == (-2.0, 15.0, 1.0, 5, 500)
 
@@ -276,31 +270,16 @@ def test_validation_needs_no_device():
         assert b"no CPU fallback" in L.crb_last_error_string()
 
 
-def _build_api(tmp_path):
-    exe = str(tmp_path / "rrt_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
-                           CPP_API, "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
-
-
 def test_reference_style_program_compiles(tmp_path):
-    _build_api(tmp_path)
+    build_ref_program(tmp_path, "rrt_ref_api.cpp")
 
 
-def test_new_kernel_does_not_spill(tmp_path):
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc):
-        pytest.skip("no nvcc")
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false",
-                          "-Xptxas", "-v", "-c", os.path.join(ROOT, "cpprobotics_b200", "csrc", "crb_rrt.cu"),
-                          "-o", str(tmp_path / "rrt.o")], capture_output=True, text=True, check=True).stderr
-    blocks = out.split("Compiling entry function")[1:]
-    kernels = [b for b in blocks if "crb_rrt_plan_kernel" in b.splitlines()[0]]
+def test_new_kernel_does_not_spill():
+    fns = ptxas_functions("crb_rrt.cu")
+    kernels = [f for f in fns if f.entry and "crb_rrt_plan_kernel" in f.name]
     assert len(kernels) == 1
-    assert "0 bytes spill stores, 0 bytes spill loads" in kernels[0] and "0 bytes stack frame" in kernels[0]
-    for b in out.split("Function properties for")[1:]:   # the out-of-line atanf / sin-cos reduction too
-        assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in b.splitlines()[1], b
+    for f in fns:   # the kernel, and the out-of-line atanf / sin-cos reduction too
+        assert (f.stack, f.spill_stores, f.spill_loads) == (0, 0, 0), f
 
 
 # ---- H100 -----------------------------------------------------------------------------------------------------
@@ -519,7 +498,7 @@ def test_gpu_reproduces_the_golden_fixture(engine):
 
 @pytest.mark.gpu
 def test_gpu_reference_style_program_matches_checker(tmp_path):
-    exe = _build_api(tmp_path)
+    exe = build_ref_program(tmp_path, "rrt_ref_api.cpp")
     subprocess.check_call([exe, str(tmp_path / "out.bin")])
     out = np.fromfile(tmp_path / "out.bin", np.float32)
     ob = synth.rrt_demo_obstacles()

@@ -16,10 +16,10 @@ import slp_cases as SC
 from cpprobotics_b200 import _lib, slp_default_params, slp_load_table, synth
 from oracle import mptg as OM
 from oracle import slp as OS
+from toolchain import build_ref_program, ptxas_kernels, run_layout_probe
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "slp_golden.npz")
-CPP = os.path.join(ROOT, "tests", "cpp", "slp_ref_api.cpp")
 NAMES = ((OS.UNIFORM, "uniform"), (OS.BIASED, "biased"), (OS.LANE, "lane"))
 
 
@@ -216,15 +216,12 @@ def test_defaults_and_layout(tmp_path):
     assert (p.base_l, p.ds, p.max_iter, p.cost_th, list(p.h_step), v) == \
         (q.base_l, q.ds, q.max_iter, q.cost_th, list(q.h_step), w)
     assert np.float32(p.h_step[0]) == np.float32(0.5) and np.float32(p.h_step[1]) == np.float32(0.02)
-    src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(void){printf("%zu %zu %zu %zu '
-                   '%zu %d %d %d %d %d %d %d %d %d\\n",sizeof(crb_slp_sampler),offsetof(crb_slp_sampler,nxy),'
-                   'offsetof(crb_slp_sampler,nh),offsetof(crb_slp_sampler,ns),offsetof(crb_slp_sampler,d),'
-                   'CRB_SLP_UNIFORM,CRB_SLP_BIASED,CRB_SLP_LANE,CRB_SLP_MAX_NXY,CRB_SLP_MAX_NH,CRB_SLP_MAX_NS,'
-                   'CRB_SLP_MAX_STATES,CRB_SLP_OK,CRB_SLP_OUT_OF_RANGE);return 0;}\n')
-    exe = tmp_path / "sz"
-    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
+    got = run_layout_probe(
+        tmp_path, '#include <stdio.h>\n#include <stddef.h>\n#include "crb.h"\nint main(void){printf("%zu %zu %zu %zu '
+        '%zu %d %d %d %d %d %d %d %d %d\\n",sizeof(crb_slp_sampler),offsetof(crb_slp_sampler,nxy),'
+        'offsetof(crb_slp_sampler,nh),offsetof(crb_slp_sampler,ns),offsetof(crb_slp_sampler,d),'
+        'CRB_SLP_UNIFORM,CRB_SLP_BIASED,CRB_SLP_LANE,CRB_SLP_MAX_NXY,CRB_SLP_MAX_NH,CRB_SLP_MAX_NS,'
+        'CRB_SLP_MAX_STATES,CRB_SLP_OK,CRB_SLP_OUT_OF_RANGE);return 0;}\n')
     S = _lib.SlpSampler
     assert got[:5] == [C.sizeof(S), S.nxy.offset, S.nh.offset, S.ns.offset, S.d.offset]
     assert got[5:] == [_lib.CRB_SLP_UNIFORM, _lib.CRB_SLP_BIASED, _lib.CRB_SLP_LANE, _lib.CRB_SLP_MAX_NXY,
@@ -279,30 +276,15 @@ def test_validation_needs_no_device():
             assert samp(s=C.byref(_lib.SlpSampler(*s))) == _lib.CRB_ERR_NO_DEVICE
 
 
-def _build_cpp(tmp_path):
-    exe = str(tmp_path / "slp_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), CPP,
-                           "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
-
-
 def test_reference_style_program_compiles(tmp_path):
-    _build_cpp(tmp_path)
+    build_ref_program(tmp_path, "slp_ref_api.cpp")
 
 
-def test_new_kernels_do_not_spill(tmp_path):
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc):
-        pytest.skip("no nvcc")
-    out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false",
-                          "-Xptxas", "-v", "-c", os.path.join(ROOT, "cpprobotics_b200", "csrc", "crb_slp.cu"),
-                          "-o", str(tmp_path / "slp.o")], capture_output=True, text=True, check=True).stderr
-    blocks = out.split("Compiling entry function")[1:]
-    kernels = [b for b in blocks if "crb_slp_" in b.splitlines()[0]]
+def test_new_kernels_do_not_spill():
+    kernels = [f for k, f in ptxas_kernels("crb_slp.cu").items() if "crb_slp_" in k]
     assert len(kernels) == 2
-    for b in kernels:
-        assert "0 bytes spill stores, 0 bytes spill loads" in b, b
+    for f in kernels:
+        assert (f.spill_stores, f.spill_loads) == (0, 0), f
 
 
 # ---- H100 -----------------------------------------------------------------------------------------------------
@@ -431,7 +413,7 @@ def test_gpu_n_zero_is_a_no_op(engine):
 
 @pytest.mark.gpu
 def test_gpu_reference_style_program_matches_oracle(tmp_path):
-    exe = _build_cpp(tmp_path)
+    exe = build_ref_program(tmp_path, "slp_ref_api.cpp")
     tb = SC.table()
     tb.tofile(tmp_path / "table.bin")
     subprocess.check_call([exe, str(tmp_path / "table.bin"), str(tmp_path / "out.bin")])

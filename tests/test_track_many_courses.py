@@ -8,7 +8,6 @@ H100 (-m gpu): the equivalence at n = 1, 33, 4097 and 65536 on 1-point, demo, 50
 vehicles in random order; NULL outputs, n = 0 and graph capture; bad course references; ind persisting per course,
 BAD_INDEX and target_ind outside the course; a 300-tick closed loop against the checker."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
@@ -18,9 +17,8 @@ from cpprobotics_b200 import _lib, lqr_track_default_params, synth
 from oracle import lqrt as OL
 from oracle import oracle as O
 from test_lqr_track import ALL, _bits_equal, assert_same, nondefault_params
+from toolchain import build_ref_program, ptxas_kernels
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CPP_API = os.path.join(ROOT, "tests", "cpp", "track_many_ref_api.cpp")
 INV = -1
 KP, STOP_SPEED = 1.0, 0.05
 
@@ -109,33 +107,18 @@ def test_fleet_courses_is_deterministic_and_varied():
         assert all(len(f) == len(x[0]) and f.dtype == np.float32 for f in x)
 
 
-def test_new_kernels_do_not_spill(tmp_path):
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc):
-        pytest.skip("no nvcc")
+def test_new_kernels_do_not_spill():
     found = []
     for src, kernel in (("crb_lqr_track.cu", "crb_lqr_track_many_kernel"), ("crb_mpc.cu", "crb_mpc_lookup_many_kernel")):
-        out = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false",
-                              "-Xptxas", "-v", "-c", os.path.join(ROOT, "cpprobotics_b200", "csrc", src),
-                              "-o", str(tmp_path / (src + ".o"))], capture_output=True, text=True, check=True).stderr
-        for b in out.split("Compiling entry function")[1:]:
-            if kernel in b.splitlines()[0]:
+        for name, f in ptxas_kernels(src).items():
+            if kernel in name:
                 found.append(kernel)
-                props = b.split("Function properties for")[1].splitlines()[1]
-                assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in props, b
+                assert (f.stack, f.spill_stores, f.spill_loads) == (0, 0, 0), f
     assert found.count("crb_lqr_track_many_kernel") == 2 and found.count("crb_mpc_lookup_many_kernel") == 1
 
 
-def _build_api(tmp_path):
-    exe = str(tmp_path / "track_many_ref_api")
-    libdir = os.path.dirname(_lib.LIB_PATH)
-    subprocess.check_call(["g++", "-std=c++11", "-O1", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
-                           CPP_API, "-L", libdir, "-lcrb", f"-Wl,-rpath,{libdir}", "-o", exe])
-    return exe
-
-
 def test_reference_style_program_compiles(tmp_path):
-    _build_api(tmp_path)
+    build_ref_program(tmp_path, "track_many_ref_api.cpp")
 
 
 # ---- H100 ---------------------------------------------------------------------------------------------------------------
@@ -616,6 +599,6 @@ def test_gpu_reference_style_program_runs(tmp_path):
     import torch
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
-    out = subprocess.check_output([_build_api(tmp_path)], text=True)
+    out = subprocess.check_output([build_ref_program(tmp_path, "track_many_ref_api.cpp")], text=True)
     lines = out.strip().splitlines()
     assert len(lines) == 2 and lines[0].startswith("lqr_steer_control") and "nan" not in out
