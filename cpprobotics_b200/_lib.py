@@ -26,7 +26,7 @@ CRB_DWA_MAX_OBSTACLES = 256
 CRB_DWA_MAX_SPEED_SAMPLES = 64
 CRB_DWA_MAX_YAWRATE_SAMPLES = 512
 CRB_DWA_MAX_STEPS = 1000
-CRB_DWA_OK, CRB_DWA_BAD_OBSTACLES = 0, 1
+CRB_DWA_OK, CRB_DWA_BAD_OBSTACLES, CRB_DWA_BAD_CONFIG = 0, 1, 2
 CRB_MPTG_MAX_ITER = 1000
 CRB_MPTG_MAX_STEPS = 16384
 CRB_MPTG_CONVERGED = 0
@@ -197,6 +197,11 @@ PROTOTYPES = {
                                                C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p,
                                                C.POINTER(DwaParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "crb_dwa_motion_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_float]),
+    "crb_dwa_control_fleet_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                                C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_void_p]),
+    "crb_dwa_motion_fleet_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "crb_mptg_default_params": (None, [C.POINTER(MptgParams)]),
     "crb_mptg_optimize_batched": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.POINTER(MptgParams), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -13,6 +13,7 @@ Method names follow the reference functions they replace:
   Engine.dwa_control         <- dwa_control()           src/dynamic_window_approach.cpp:148-155
   Engine.dwa_control_many    <- the same, each robot among its own obstacles (synth.pack_obstacles)
   Engine.dwa_motion          <- motion()                src/dynamic_window_approach.cpp:43-50
+  Engine.dwa_control_fleet, Engine.dwa_motion_fleet <- the same two, each robot with its own Config (dwa_config_table)
   Engine.mptg_optimize       <- TrajectoryOptimizer::optimizer_traj()  include/trajectory_optimizer.h:53-128
   Engine.mptg_generate_trajectory <- MotionModel::generate_trajectory() include/motion_model.h:110-131
   Engine.slp_sample_states   <- calc_{uniform_polar,biased_polar,lane}_states()  src/state_lattice_planner.cpp:29-113
@@ -96,6 +97,19 @@ def dwa_default_params() -> DwaParams:
     p = DwaParams()
     load_library().crb_dwa_default_params(C.byref(p))
     return p
+
+
+DWA_CONFIG_FIELDS = tuple(name for name, _ in DwaParams._fields_)   # one crb_dwa_params record: 12 float32
+
+
+def dwa_config_table(params) -> np.ndarray:
+    """A config table for dwa_control_fleet: a sequence of DwaParams packed into float32 [m, 12], one 48-byte
+    crb_dwa_params record per row in the struct's order.  Returns a host array; torch.from_numpy(...).cuda() uploads it
+    as it is.  Records are not checked here: the kernel gives a robot on a refused record CRB_DWA_BAD_CONFIG."""
+    rows = [[getattr(p, k) for k in DWA_CONFIG_FIELDS] for p in params]
+    if not rows:
+        raise ValueError("a config table needs at least one record")
+    return np.ascontiguousarray(np.asarray(rows, np.float32).reshape(len(rows), len(DWA_CONFIG_FIELDS)))
 
 
 def mptg_default_params() -> MptgParams:
@@ -647,6 +661,66 @@ class Engine:
         check(self.lib.crb_dwa_motion_batched(self.ctx, n, _ptr(x, np.float32, device=True, name="x"),
                                               _ptr(u, np.float32, device=True, name="u"), C.c_float(d)),
               "crb_dwa_motion_batched")
+
+    def dwa_max_rollout_points(self, configs) -> int:
+        """The largest dwa_rollout_points over the records of a config table (float32 [m, 12]; copied to the host when
+        on the device), refused records left out; 0 when every record is refused."""
+        rows = configs.cpu().numpy() if torch is not None and isinstance(configs, torch.Tensor) else configs
+        best = 0
+        for row in np.asarray(rows, np.float32).reshape(-1, len(DWA_CONFIG_FIELDS)):
+            k = C.c_int(0)
+            if self.lib.crb_dwa_rollout_points(C.byref(DwaParams(*(float(v) for v in row))), C.byref(k)) == 0:
+                best = max(best, int(k.value))
+        return best
+
+    def dwa_control_fleet(self, x, u, goal, obstacles, ob_of, configs, config_of, max_pts: Optional[int] = None,
+                          cost=None, best=None, traj=None, traj_len=None, status=None):
+        """dwa_control() for a fleet whose robots each have their own Config and obstacle list: robot i plans with
+        configs[config_of[i]] among its list ob_of[i].  configs float32 [n_configs, 12] (dwa_config_table), config_of
+        int32 [n]; x, u, goal, obstacles and ob_of as dwa_control_many.  Optional outputs cost [n], best [n] int32,
+        traj [5*max_pts, n] (the first min(traj_len[i], max_pts) points of robot i's rollout are written), traj_len
+        [n] int32 (each robot's point count); status [n] int32 (CRB_DWA_*) is allocated when not given.  max_pts
+        defaults to the largest point count in the table (read from it on the host).  Returns status.  CUDA tensors;
+        only enqueues when max_pts is given or traj is None."""
+        n = int(x.shape[-1])
+        _shape(x, 5, n, "x"); _shape(u, 2, n, "u"); _shape(goal, 2, n, "goal"); _shape(ob_of, 1, n, "ob_of")
+        _shape(config_of, 1, n, "config_of")
+        ob, off = obstacles
+        if ob.dim() != 2 or int(ob.shape[1]) != 2:
+            raise ValueError(f"ob: expected shape (n_rows, 2), got {tuple(ob.shape)}")
+        if off.dim() != 1:
+            raise ValueError(f"ob_off: expected shape (n_sets + 1,), got {tuple(off.shape)}")
+        if configs.dim() != 2 or int(configs.shape[1]) != len(DWA_CONFIG_FIELDS):
+            raise ValueError(f"configs: expected shape (n_configs, 12) (dwa_config_table), got {tuple(configs.shape)}")
+        if max_pts is None:
+            max_pts = self.dwa_max_rollout_points(configs) if traj is not None else 0
+        if traj is not None:
+            _shape(traj, 5 * int(max_pts), n, "traj")
+        for a, name in ((cost, "cost"), (best, "best"), (traj_len, "traj_len")):
+            if a is not None:
+                _shape(a, 1, n, name)
+        status = status if status is not None else torch.empty(n, dtype=torch.int32, device=x.device)
+        _shape(status, 1, n, "status")
+        check(self.lib.crb_dwa_control_fleet_batched(
+            self.ctx, n, _ptr(x, np.float32, device=True, name="x"), _ptr(u, np.float32, device=True, name="u"),
+            _ptr(goal, np.float32, device=True, name="goal"), _ptr(ob, np.float32, device=True, name="ob"),
+            int(ob.shape[0]), _ptr(off, np.int64, device=True, name="ob_off"), int(off.shape[0]) - 1,
+            _ptr(ob_of, np.int32, device=True, name="ob_of"), _ptr(configs, np.float32, device=True, name="configs"),
+            int(configs.shape[0]), _ptr(config_of, np.int32, device=True, name="config_of"), int(max_pts),
+            _ptr(cost, np.float32, device=True, name="cost"), _ptr(best, np.int32, device=True, name="best"),
+            _ptr(traj, np.float32, device=True, name="traj"), _ptr(traj_len, np.int32, device=True, name="traj_len"),
+            _ptr(status, np.int32, device=True, name="status")), "crb_dwa_control_fleet_batched")
+        return status
+
+    def dwa_motion_fleet(self, x, u, dt):
+        """motion() in place on x [5,n] with u [2,n] and each robot's own dt [n] float32 (for example
+        configs[:, DWA_CONFIG_FIELDS.index("dt")][config_of]), applied as given.  CUDA tensors; only enqueues."""
+        n = int(x.shape[-1])
+        _shape(x, 5, n, "x"); _shape(u, 2, n, "u"); _shape(dt, 1, n, "dt")
+        check(self.lib.crb_dwa_motion_fleet_batched(self.ctx, n, _ptr(x, np.float32, device=True, name="x"),
+                                                    _ptr(u, np.float32, device=True, name="u"),
+                                                    _ptr(dt, np.float32, device=True, name="dt")),
+              "crb_dwa_motion_fleet_batched")
 
     # ---- model-predictive trajectory generation ---------------------------------------------------------
     @staticmethod

@@ -693,6 +693,63 @@ def dwa_fleet_obstacles(n_sets: int, seed: int = 0x0B57):
     return out
 
 
+# ---- a Config per robot: crb_dwa_control_fleet_batched ------------------------------------------------------------
+# Robot classes: the Config members each one sets apart from the reference's (:27-40).  Window sizes (speed x yaw-rate
+# samples) and rollout steps are at most about 2/3 of CRB_DWA_MAX_SPEED_SAMPLES, CRB_DWA_MAX_YAWRATE_SAMPLES and
+# CRB_DWA_MAX_STEPS, so that dwa_fleet_configs' +-15 % changes to every member stay within the limits.
+DWA_ROBOT_CLASSES = (
+    ("reference", {}),                                             # 5 x 80 samples, 30 steps
+    ("small_fast", dict(max_speed=2.0, min_speed=-0.3, max_yawrate=2.0, max_accel=1.0, robot_radius=0.3,
+                        max_dyawrate=3.0, v_reso=0.02, yawrate_reso=0.02, dt=0.1, predict_time=1.5,
+                        to_goal_cost_gain=1.2, speed_cost_gain=0.6)),      # 11 x 31, 15 steps
+    ("large_slow", dict(max_speed=0.4, min_speed=-0.1, max_yawrate=0.3, max_accel=0.05, robot_radius=2.0,
+                        max_dyawrate=0.2, v_reso=0.005, yawrate_reso=0.002, dt=0.2, predict_time=5.0,
+                        to_goal_cost_gain=0.7, speed_cost_gain=1.5)),      # 5 x 41, 26 steps
+    ("coarse_grid", dict(max_accel=0.5, v_reso=0.05, yawrate_reso=0.02)),  # 3 x 7, 30 steps
+    ("fine_grid", dict(max_accel=0.3, max_dyawrate=0.6, v_reso=0.002, yawrate_reso=0.0005, predict_time=2.0)),
+    ("short_horizon", dict(max_accel=0.4, dt=0.05, predict_time=0.6)),    # 5 x 40, 13 steps
+    ("long_horizon", dict(predict_time=8.0, robot_radius=0.5)),           # 5 x 80, 81 steps
+    ("no_reverse", dict(max_speed=1.2, min_speed=0.0, max_yawrate=1.0, max_accel=0.3, robot_radius=0.6,
+                        max_dyawrate=1.5, v_reso=0.015, yawrate_reso=0.01, dt=0.08, predict_time=2.4,
+                        to_goal_cost_gain=1.0, speed_cost_gain=0.8)),     # 4 x 25, 31 steps
+)
+
+
+def dwa_fleet_configs(n_configs: int, seed: int = 0xC1A55):
+    """n_configs robot classes (DwaParams): class k is DWA_ROBOT_CLASSES[k % 8] (the fine grid has 31 x 241 samples and
+    21 steps), exactly for k < 8 and with every member scaled by its own factor in [0.85, 1.15] from k = 8 on.
+    Every class is inside crb.h's limits.  Deterministic for a seed."""
+    from ._lib import DwaParams
+    pi = 3.141592653
+    ref = dict(max_speed=1.0, min_speed=-0.5, max_yawrate=40.0 * pi / 180.0, max_accel=0.2, robot_radius=1.0,
+               max_dyawrate=40.0 * pi / 180.0, v_reso=0.01, yawrate_reso=0.1 * pi / 180.0, dt=0.1, predict_time=3.0,
+               to_goal_cost_gain=1.0, speed_cost_gain=1.0)
+    names = [k for k, _ in DwaParams._fields_]
+    out = []
+    for k in range(n_configs):
+        d = dict(ref, **DWA_ROBOT_CLASSES[k % len(DWA_ROBOT_CLASSES)][1])
+        if k >= len(DWA_ROBOT_CLASSES):
+            scale = uniform(seed, 130, np.arange(k * 12, k * 12 + 12, dtype=np.uint64), 0.85, 1.15)
+            d = {m: d[m] * float(scale[j]) for j, m in enumerate(names)}
+        out.append(DwaParams(*(float(np.float32(d[m])) for m in names)))
+    return out
+
+
+def dwa_fleet_inputs(configs, config_of, seed: int = 0xC0FFEE):
+    """x [5,n], u [2,n], goal [2,n] for robots on classes configs[config_of[i]]: the robots of class c are
+    dwa_inputs(m_c, seed + c) with that class's speed and yaw-rate limits, so each sits within its own limits and one
+    in four sits at a speed limit and one in four at a yaw-rate limit.  Deterministic for a seed."""
+    config_of = np.asarray(config_of)
+    n = config_of.size
+    x, u, g = np.empty((5, n), np.float32), np.empty((2, n), np.float32), np.empty((2, n), np.float32)
+    for c in np.unique(config_of):
+        sel = np.nonzero(config_of == c)[0]
+        p = configs[int(c)]
+        x[:, sel], u[:, sel], g[:, sel] = dwa_inputs(sel.size, seed=seed + int(c), max_speed=p.max_speed,
+                                                     min_speed=p.min_speed, max_yawrate=p.max_yawrate)
+    return x, u, g
+
+
 def rrt_fleet_obstacles(n_sets: int, seed: int = 0x5CA7, lo: float = -2.0, hi: float = 15.0, max_k: int = 64):
     """n_sets scattered RRT maps ([m, 3] float32 rows (x, y, r)) over one planning area [lo, hi)^2: map s has 0 to max_k
     circles (rrt_scatter_obstacles, radii 0.3 to 1.2) from a seed of its own; every 16th map (s % 16 == 0) is empty.

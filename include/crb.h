@@ -28,6 +28,8 @@
  *   crb_dwa_control_many_batched        <- the same, each robot among its own obstacles (the reference takes ob
  *                                          per call)
  *   crb_dwa_motion_batched              <- motion()              src/dynamic_window_approach.cpp:43-50
+ *   crb_dwa_control_fleet_batched,      <- the same two, each robot with its own Config (the reference takes config
+ *   crb_dwa_motion_fleet_batched           per call)
  *   crb_mptg_optimize_batched           <- TrajectoryOptimizer::optimizer_traj()  include/trajectory_optimizer.h:53-200
  *                                         (MotionModel::generate_last_state, quadratic_interpolation,
  *                                          update of include/motion_model.h:59-150)
@@ -515,6 +517,41 @@ int crb_dwa_control_many_batched(crb_ctx* ctx, int64_t n, const float* x, float*
 /* x [5][n] in/out, u [2][n] (DEVICE; NULL allowed when n = 0).  dt finite and > 0.
  * Replaces: motion(x, u, dt) :43-50, the plant step of main() :194. */
 int crb_dwa_motion_batched(crb_ctx* ctx, int64_t n, float* x, const float* u, float dt);
+
+/* A Config per robot: dwa_control(x, u, config, goal, ob) takes its Config per call, and a fleet that mixes robot
+ * types has one per type.  A config table is a DEVICE array of n_configs crb_dwa_params records in this struct's own
+ * layout (12 floats, 48 bytes, max_speed at offset 0 ... speed_cost_gain at 44), so a std::vector<crb_dwa_params> is
+ * copied up as it is.  config_of [n] (int32, device) names each robot's record.
+ *
+ * crb_dwa_control_fleet_batched: x, u, goal and the obstacle store (k = 2) as in crb_dwa_control_many_batched.  Each
+ * record is checked on the device against the limits above, by the same function crb_dwa_rollout_points uses, and
+ * n_pts_i = crb_dwa_rollout_points(&configs[config_of[i]]).  For a robot whose record and list are good
+ * (CRB_DWA_OK), u, cost and best are bitwise those of crb_dwa_control_many_batched run with prm =
+ * &configs[config_of[i]] (best indexes the robot's own grid), and
+ *   traj [5*max_pts][n]  gets the first min(n_pts_i, max_pts) points of that call's traj (NaN when best = -1); rows
+ *                        past them are not written
+ *   traj_len [n]         int32 n_pts_i
+ * status [n] int32 CRB_DWA_*.  The config is checked before the list: CRB_DWA_BAD_CONFIG (u and cost NaN, best -1,
+ * traj_len 0, traj not written, nothing of the obstacle store read); then CRB_DWA_BAD_OBSTACLES (u and cost NaN,
+ * best -1, the first min(n_pts_i, max_pts) points of traj NaN, traj_len n_pts_i).  Other robots are unaffected.
+ * cost, best, traj, traj_len and status are optional (NULL = not written).  CRB_ERR_INVALID_ARG before any device
+ * work as crb_dwa_control_many_batched (without prm), unless n_configs >= 1, configs and config_of are given when
+ * n > 0, and 0 <= max_pts <= CRB_DWA_MAX_STEPS + 1.  n = 0 is a no-op.  One warp per robot; only enqueues
+ * (graph-capturable).
+ * Replaces: dwa_control(x, u, config, goal, ob) :148-155 with each robot's own config and ob.
+ *
+ * crb_dwa_motion_fleet_batched: crb_dwa_motion_batched with dt [n] (float, DEVICE) per robot: robot i is bitwise
+ * crb_dwa_motion_batched with dt[i].  dt is applied as given (NaN, 0 and negative included), as motion() does.
+ * x, u and dt may be NULL when n = 0.
+ * Replaces: motion(x, u, config.dt) :43-50 with each robot's config. */
+#define CRB_DWA_BAD_CONFIG 2 /* config_of[i] is outside [0, n_configs), or its record is outside the limits above
+                                (crb_dwa_rollout_points refuses it) */
+int crb_dwa_control_fleet_batched(crb_ctx* ctx, int64_t n, const float* x, float* u, const float* goal,
+                                  const float* ob, int64_t n_rows, const int64_t* ob_off, int32_t n_sets,
+                                  const int32_t* ob_of, const crb_dwa_params* configs, int32_t n_configs,
+                                  const int32_t* config_of, int32_t max_pts, float* cost, int32_t* best, float* traj,
+                                  int32_t* traj_len, int32_t* status);
+int crb_dwa_motion_fleet_batched(crb_ctx* ctx, int64_t n, float* x, const float* u, const float* dt);
 
 /* ---- model-predictive trajectory generation (include/trajectory_optimizer.h, include/motion_model.h) ---- */
 /* Shared by the batch: MotionModel's base_l and ds, and optimizer_traj's max_iter, cost_th and h_step. */

@@ -10,7 +10,8 @@
 //   resampling(px, pw, gen, uni_d)                src/particle_filter.cpp:120-148
 //   pf_localization_resampling(px, pw, xEst, PEst, z, u, ...)   the demo's tick :270-271 for a fleet, one launch
 //   solve_DARE / dlqr (4x4 and 5x5)               src/lqr_steer_control.cpp:75-96, lqr_speed_steer_control.cpp:85-106
-//   dwa_control(x, u, config, goal, ob), motion(x, u, dt)   src/dynamic_window_approach.cpp:148-155, :43-50
+//   dwa_control(x, u, config, goal, ob), motion(x, u, dt)   src/dynamic_window_approach.cpp:148-155, :43-50 (also over
+//                                                            vectors of robots, with one Config or a Config per robot)
 //   MotionModel, TrajectoryOptimizer::optimizer_traj(...)    include/motion_model.h, include/trajectory_optimizer.h
 //   calc_{uniform_polar,biased_polar,lane}_states, search_nearest_one_from_lookuptable, generate_path
 //                                                            src/state_lattice_planner.cpp:47-155
@@ -569,6 +570,90 @@ inline std::vector<std::vector<std::array<float, 5>>> dwa_control(
   return out;
 }
 
+// dwa_control for a mixed fleet, each robot with its own Config and its own obstacles: robot i is dwa_control(x[i],
+// u[i], config[i], goal[i], ob[i]) (u[i] set, its rollout of its own Config's length returned in element i, empty when
+// no sample is admissible), all in one launch of crb_dwa_control_fleet_batched.  Bitwise-equal Configs share one
+// record of the table.  A Config outside crb.h's limits throws before any device work.  Each ob[i] must have at most
+// CRB_DWA_MAX_OBSTACLES rows.
+template <class Config>
+inline std::vector<std::vector<std::array<float, 5>>> dwa_control(
+    const std::vector<std::array<float, 5>>& x, std::vector<std::array<float, 2>>& u,
+    const std::vector<Config>& config, const std::vector<std::array<float, 2>>& goal,
+    const std::vector<std::vector<std::array<float, 2>>>& ob) {
+  const size_t n = x.size();
+  if (u.size() != n || config.size() != n || goal.size() != n || ob.size() != n)
+    throw std::runtime_error("dwa_control: x, u, config, goal and ob differ in length");
+  std::vector<std::vector<std::array<float, 5>>> out(n);
+  if (n == 0) return out;
+  // the table: one record per bitwise-distinct Config, each checked here
+  std::vector<crb_dwa_params> table;
+  std::vector<int> n_pts;
+  std::vector<int32_t> of(n);
+  int max_pts = 0;
+  for (size_t i = 0; i < n; ++i) {
+    const crb_dwa_params prm = crb::dwa_params_of(config[i]);
+    size_t c = 0;
+    while (c < table.size() && std::memcmp(&table[c], &prm, sizeof(prm)) != 0) ++c;
+    if (c == table.size()) {
+      int k = 0;
+      crb::check(crb_dwa_rollout_points(&prm, &k), "crb_dwa_rollout_points");
+      table.push_back(prm);
+      n_pts.push_back(k);
+      max_pts = std::max(max_pts, k);
+    }
+    of[i] = (int32_t)c;
+  }
+  const size_t m = table.size();
+  crb_ctx* ctx = crb::Session::get();
+  // host: ob_off [n + 1] int64 | ob_of [n] int32 | config_of [n] int32 | x [5][n] | u [2][n] | goal [2][n] |
+  //       table [m][12] | ob [n_rows][2]
+  std::vector<int64_t> off(n + 1, 0);
+  for (size_t i = 0; i < n; ++i) off[i + 1] = off[i] + (int64_t)ob[i].size();
+  const size_t n_rows = (size_t)off[n];
+  std::vector<float> h(2 * (n + 1) + 2 * n + 9 * n + 12 * m + 2 * n_rows);
+  std::memcpy(h.data(), off.data(), off.size() * sizeof(int64_t));
+  std::memcpy(h.data() + 2 * (n + 1) + n, of.data(), n * sizeof(int32_t));
+  float* hx = h.data() + 4 * n + 2;
+  std::memcpy(hx + 9 * n, table.data(), m * sizeof(crb_dwa_params));
+  float* hob = hx + 9 * n + 12 * m;
+  for (size_t i = 0; i < n; ++i) {
+    const int32_t s = (int32_t)i;
+    std::memcpy(h.data() + 2 * (n + 1) + i, &s, 4);
+    for (int f = 0; f < 5; ++f) hx[f * n + i] = x[i][f];
+    for (int f = 0; f < 2; ++f) hx[(5 + f) * n + i] = u[i][f];
+    for (int f = 0; f < 2; ++f) hx[(7 + f) * n + i] = goal[i][f];
+    for (size_t k = 0; k < ob[i].size(); ++k) {
+      hob[2 * (off[i] + k)] = ob[i][k][0];
+      hob[2 * (off[i] + k) + 1] = ob[i][k][1];
+    }
+  }
+  // device: the host block | best [n] | traj [5 max_pts][n]; the arena comes from cudaMalloc, so ob_off is aligned
+  float* d = crb::Session::scratch(h.size() + n + 5 * (size_t)max_pts * n);
+  float *dx = d + 4 * n + 2, *dbest = d + h.size(), *dtraj = dbest + n;
+  crb::check(crb_memcpy_h2d(ctx, d, h.data(), h.size() * sizeof(float)), "h2d");
+  crb::check(crb_dwa_control_fleet_batched(ctx, (int64_t)n, dx, dx + 5 * n, dx + 7 * n,
+                                           dx + 9 * n + 12 * m, (int64_t)n_rows, (const int64_t*)d, (int32_t)n,
+                                           (const int32_t*)(d + 2 * (n + 1)), (const crb_dwa_params*)(dx + 9 * n),
+                                           (int32_t)m, (const int32_t*)(d + 2 * (n + 1) + n), max_pts, nullptr,
+                                           (int32_t*)dbest, dtraj, nullptr, nullptr),
+             "crb_dwa_control_fleet_batched");
+  std::vector<float> hu(2 * n), tr(5 * (size_t)max_pts * n);
+  std::vector<int32_t> best(n);
+  crb::check(crb_memcpy_d2h(ctx, hu.data(), dx + 5 * n, hu.size() * sizeof(float)), "d2h");
+  crb::check(crb_memcpy_d2h(ctx, best.data(), dbest, n * sizeof(int32_t)), "d2h");
+  crb::check(crb_memcpy_d2h(ctx, tr.data(), dtraj, tr.size() * sizeof(float)), "d2h");
+  for (size_t i = 0; i < n; ++i) {
+    u[i][0] = hu[i];
+    u[i][1] = hu[n + i];
+    if (best[i] < 0) continue;
+    const int k_pts = n_pts[(size_t)of[i]];
+    out[i].resize((size_t)k_pts);
+    for (int k = 0; k < k_pts; ++k)
+      for (int j = 0; j < 5; ++j) out[i][(size_t)k][(size_t)j] = tr[(size_t)(5 * k + j) * n + i];
+  }
+  return out;
+}
+
 // motion :43-50 (the plant step of main() :194)
 inline std::array<float, 5> motion(std::array<float, 5> x, std::array<float, 2> u, float dt) {
   crb_ctx* ctx = crb::Session::get();
@@ -577,6 +662,32 @@ inline std::array<float, 5> motion(std::array<float, 5> x, std::array<float, 2> 
   crb::check(crb_memcpy_h2d(ctx, dx + 5, u.data(), 2 * sizeof(float)), "h2d");
   crb::check(crb_dwa_motion_batched(ctx, 1, dx, dx + 5, dt), "crb_dwa_motion_batched");
   crb::check(crb_memcpy_d2h(ctx, x.data(), dx, 5 * sizeof(float)), "d2h");
+  return x;
+}
+
+// motion :43-50 for a fleet, each robot with its own dt (main()'s motion(x, u, config.dt) :194 with a Config per
+// robot): robot i is motion(x[i], u[i], dt[i]), dt applied as given, all in one launch of crb_dwa_motion_fleet_batched.
+inline std::vector<std::array<float, 5>> motion(std::vector<std::array<float, 5>> x,
+                                                const std::vector<std::array<float, 2>>& u,
+                                                const std::vector<float>& dt) {
+  const size_t n = x.size();
+  if (u.size() != n || dt.size() != n) throw std::runtime_error("motion: x, u and dt differ in length");
+  if (n == 0) return x;
+  crb_ctx* ctx = crb::Session::get();
+  // x [5][n] | u [2][n] | dt [n]
+  std::vector<float> h(8 * n);
+  for (size_t i = 0; i < n; ++i) {
+    for (int f = 0; f < 5; ++f) h[f * n + i] = x[i][f];
+    for (int f = 0; f < 2; ++f) h[(5 + f) * n + i] = u[i][f];
+    h[7 * n + i] = dt[i];
+  }
+  float* dx = crb::Session::scratch(h.size());
+  crb::check(crb_memcpy_h2d(ctx, dx, h.data(), h.size() * sizeof(float)), "h2d");
+  crb::check(crb_dwa_motion_fleet_batched(ctx, (int64_t)n, dx, dx + 5 * n, dx + 7 * n),
+             "crb_dwa_motion_fleet_batched");
+  crb::check(crb_memcpy_d2h(ctx, h.data(), dx, 5 * n * sizeof(float)), "d2h");
+  for (size_t i = 0; i < n; ++i)
+    for (int f = 0; f < 5; ++f) x[i][f] = h[f * n + i];
   return x;
 }
 
